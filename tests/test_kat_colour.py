@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from jxl_rs_b200 import abi
+from tests.f64_pipeline import bt709_exact, gamma_exact, hlg_exact, pq_exact
 
 OPSIN_INV = np.array([[11.031566901960783, -9.866943921568629, -0.16462299647058826],
                       [-3.254147380392157, 4.418770392156863, -0.16462299647058826],
@@ -125,23 +126,17 @@ def test_gamma_bt709_curves():
     v = samples(1)
     x = v.astype(np.float64)
     got = from_linear(abi_tf("GAMMA"), v, gamma=0.45)
-    want = np.sign(x) * np.abs(x) ** 0.45
+    want = gamma_exact(x, 0.45)
     assert np.all(np.abs(got - want) <= 1e-4 * np.maximum(np.abs(want), 1e-2))  # fast_powf: 3e-5 relative
     got = from_linear(abi_tf("BT709"), v)
-    a = np.abs(x)
-    want = np.sign(x) * np.where(a < 0.018, 4.5 * a, 1.099 * a ** 0.45 - 0.099)
+    want = bt709_exact(x)
     assert np.abs(got - want).max() <= 2e-6  # tf.rs:613-624 holds the rational form to 1e-6 of the naive one
 
 
 def test_pq_curve():
     for it in (10000.0, 4000.0, 255.0):
         v = samples(2)
-        x = np.abs(v.astype(np.float64))
-        m1, m2 = 2610 / 16384, 2523 / 4096 * 128
-        c1, c2, c3 = 3424 / 4096, 2413 / 4096 * 32, 2392 / 4096 * 32
-        xp = (x * it / 10000) ** m1
-        want = np.sign(v) * ((c1 + c2 * xp) / (1 + c3 * xp)) ** m2
-        want[v == 0] = 0
+        want = pq_exact(v.astype(np.float64), it)
         got = from_linear(abi_tf("PQ"), v, it=it)
         big = np.abs(v) >= 1e-4
         # The reference switches polynomials on the UNSCALED sample (tf.rs:269-275), so below 10000 nits the main
@@ -154,17 +149,7 @@ def test_hlg_curve():
     lum = (0.2627, 0.6780, 0.0593)
     for it in (1000.0, 255.0, 4000.0):
         v = samples(3)[:4000]
-        x = v.astype(np.float64)
-        sg = 1.2 * 1.111 ** np.log2(it / 1e3)
-        e = (1 - sg) / sg
-        if abs(e) >= 0.1:
-            mixed = x @ np.array(lum)
-            x = x * (mixed ** e)[:, None]
-        a = np.abs(x)
-        A = 0.17883277
-        B, Cc = 1 - 4 * A, 0.5599107295
-        with np.errstate(invalid="ignore", divide="ignore"):
-            want = np.sign(x) * np.where(a <= 1 / 12, np.sqrt(3 * a), A * np.log(np.maximum(12 * a - B, 1e-30)) + Cc)
+        want = hlg_exact(v.astype(np.float64), it, lum)
         got = from_linear(abi_tf("HLG"), v, it=it, lum=lum)
         assert np.abs(got - want).max() <= 1e-4  # fast_powf in the OOTF (3e-5 relative), fast_log2f in the OETF (5e-7)
 

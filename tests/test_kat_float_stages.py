@@ -11,8 +11,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-MIN_SIGMA = -3.90524291751269967465540850526868  # jxl/src/lib.rs:28
-INV_SIGMA_NUM = -1.1715728752538099024           # features/epf.rs:26
+from tests.f64_pipeline import MIN_SIGMA, epf_stage_f64, sigma_image_f64
 
 
 def _lib():
@@ -29,47 +28,6 @@ def _lib():
 # ---------------------------------------------------------------------------------------------------------------------
 # EPF
 # ---------------------------------------------------------------------------------------------------------------------
-OFF0 = [(0, -2), (-1, -1), (0, -1), (1, -1), (-2, 0), (-1, 0), (1, 0), (2, 0), (-1, 1), (0, 1), (1, 1), (0, 2)]  # epf0.rs:182-195
-OFF1 = [(0, -1), (-1, 0), (1, 0), (0, 1)]                                                                            # epf1.rs:118-123
-PLUS = [(0, -1), (-1, 0), (0, 0), (1, 0), (0, 1)]
-
-
-def epf_stage_f64(stage, img, inv_sigma, channel_scale, sigma_scale, border_sad_mul):
-    """img: (3, h, w) float64. Whole-image mirroring at the edges (render/simple_pipeline/run_stage.rs:127-134 with
-    util/mirror.rs:8 = numpy's 'symmetric' padding)."""
-    _, h, w = img.shape
-    R = 3
-    P = np.pad(img, ((0, 0), (R, R), (R, R)), mode="symmetric")
-
-    def sh(dx, dy):
-        return P[:, R + dy:R + dy + h, R + dx:R + dx + w]
-
-    offs = OFF0 if stage == 0 else OFF1
-    scale = np.asarray(channel_scale, np.float64)[:, None, None]
-    sads = []
-    for ox, oy in offs:
-        if stage == 2:  # epf2.rs:84-101: one absolute difference per channel
-            s = (np.abs(sh(ox, oy) - sh(0, 0)) * scale).sum(axis=0)
-        else:           # epf0.rs:157-168 / epf1.rs:98-101: plus-shaped sums
-            s = sum((np.abs(sh(px, py) - sh(px + ox, py + oy)) * scale).sum(axis=0) for px, py in PLUS)
-        sads.append(s)
-    ys, xs = np.mgrid[0:h, 0:w]
-    sig = inv_sigma[ys // 8, xs // 8]
-    sm = sigma_scale * 1.65
-    border = np.isin(ys % 8, (0, 7)) | np.isin(xs % 8, (0, 7))          # common.rs:31-41
-    inv_s = sig * np.where(border, sm * border_sad_mul, sm)
-    wts = [np.maximum(s * inv_s + 1.0, 0.0) for s in sads]
-    wsum = 1.0 + sum(wts)
-    out = (sh(0, 0) + sum(wt[None] * sh(ox, oy) for wt, (ox, oy) in zip(wts, offs))) / wsum[None]
-    return np.where((sig < MIN_SIGMA)[None], img, out)                    # sigma_mask: MIN_SIGMA > sigma passes through
-
-
-def sigma_image_f64(global_scale, raw_quant, sharpness, quant_mul, sharp_lut):  # features/epf.rs:54-79
-    quant_scale = 1.0 / (65536.0 / global_scale)
-    sigma_quant = quant_mul / (quant_scale * raw_quant.astype(np.float64) * INV_SIGMA_NUM)
-    return 1.0 / np.minimum(sigma_quant * np.asarray(sharp_lut, np.float64)[sharpness], -1e-4)
-
-
 @pytest.mark.parametrize("stage", [0, 1, 2])
 @pytest.mark.parametrize("shape", [(96, 64), (61, 43), (8, 8), (5, 3)])
 def test_epf_stage_against_f64_restatement(stage, shape):

@@ -6,46 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-
-def alpha(u):
-    return 1 / np.sqrt(2) if u == 0 else 1.0
-
-
-def dct_matrix(n):  # tests.rs:23-60 / 62-100
-    m = np.zeros((n, n))
-    for u in range(n):
-        for y in range(n):
-            m[u, y] = alpha(u) * np.cos((y + 0.5) * u * np.pi / n) * np.sqrt(2)
-    return m
-
-
-def slow_idct2d(inp):  # tests.rs:123-136
-    rows, cols = inp.shape
-    if rows < cols:
-        a = inp.T
-    else:
-        a = inp.reshape(-1).reshape(cols, rows)
-    b = dct_matrix(a.shape[0]).T @ a
-    c = b.T
-    return dct_matrix(c.shape[0]).T @ c
-
-
-def scales(n):  # tests.rs:138-147
-    i = np.arange(n)
-    return np.cos(i / (16 * n) * np.pi) * np.cos(i / (8 * n) * np.pi) * np.cos(i / (4 * n) * np.pi) * n
-
-
-def slow_reinterpreting_dct2d(inp):  # tests.rs:149-180
-    rows, cols = inp.shape
-    d1 = dct_matrix(rows) @ inp
-    d2 = dct_matrix(cols) @ d1.T
-    res = d2.T if rows < cols else d2
-    rs, cs = scales(rows), scales(cols)
-    if rows < cols:
-        res = res / (rs[:, None] * cs[None, :])
-    else:
-        res = res / (cs[:, None] * rs[None, :])
-    return res
+from tests.f64_pipeline import slow_idct2d, slow_reinterpreting_dct2d
 
 
 def check_close(a, b, tol):
