@@ -170,7 +170,11 @@ int jxg_batch_begin(void* ctx, uint32_t n_frames_hint, void** batch);
  * hf_bytes[sec_off[s] .. sec_off[s] + sec_len[s]). n_sections = passes * groups.
  * out/out_row_stride: destination for the frame's pixels; `out_is_device` says
  * whether it is a device pointer (left in HBM) or a host pointer (D2H copy is
- * part of jxg_batch_run + jxg_batch_wait). */
+ * part of jxg_batch_run + jxg_batch_wait). The device stores whole samples, so
+ * out_row_stride must be a multiple of the sample size: 4 bytes for RGBA_U8,
+ * RGB_F32 and XYB_F32_PLANAR, 2 for RGB_U16 and RGB_F16, any for RGB_U8. A
+ * device `out` must be aligned the same way. Otherwise the call returns
+ * JXG_ERR_INVALID_OUTPUT. (jxg_batch_add_parsed follows the same rule.) */
 int jxg_batch_add_frame(void* batch, const JxgFrameDesc* desc, const uint8_t* hf_bytes,
                         const uint64_t* sec_off, const uint32_t* sec_len, uint32_t n_sections,
                         void* out, size_t out_row_stride, int out_is_device);

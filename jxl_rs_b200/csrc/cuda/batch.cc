@@ -465,6 +465,13 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   const uint32_t orientation = (d->orientation == 0 || d->output_format == JXG_FORMAT_XYB_F32_PLANAR) ? 1u : d->orientation;
   const uint32_t disp_w = orientation >= 5 ? F.height : F.width, disp_h = orientation >= 5 ? F.width : F.height;
   if (out_row_stride < size_t(disp_w) * bpp) return set_error(JXG_ERR_INVALID_OUTPUT, "output row stride too small");
+  // The stores (and the orientation pass's word copies) write whole samples: rows, and a device buffer, must be
+  // aligned to the sample size (include/jxg.h).
+  const size_t sample_align = bpp == 3 ? 1 : (bpp == 6 ? 2 : 4);
+  if (out_row_stride % sample_align)
+    return set_error(JXG_ERR_INVALID_OUTPUT, "output row stride is not a multiple of the sample size");
+  if (out_is_device && reinterpret_cast<uintptr_t>(out) % sample_align)
+    return set_error(JXG_ERR_INVALID_OUTPUT, "device output is not aligned to the sample size");
   if (!trusted)
     if (int r = validate_desc(d, sec_len, n_sections)) return r;
   F.num_histograms = d->num_histograms;

@@ -2404,7 +2404,18 @@ __device__ __noinline__ void from_linear_other(const FrameDev& F, float (&v)[3])
     case JXG_TF_HLG: {  // tf.rs:381-395 (inverse OOTF), 481-497 (OETF)
       if (F.tf_hlg_exp != 0.0f) {
         const float mixed = fmaf(v[0], F.tf_lum[0], fmaf(v[1], F.tf_lum[1], v[2] * F.tf_lum[2]));
-        const float mult = exp2f(F.tf_hlg_exp * log2f(mixed));
+        float lg;
+        if (mixed > 0.0f) {
+          lg = log2f(mixed);
+        } else {
+          // Dark or out-of-gamut pixels. log2f gives NaN here; the reference's fast_log2f (util/fast_math.rs:128-137)
+          // splits the bits with wrapping integer arithmetic instead: the exponent of a negative value comes out 256
+          // higher (256 lower from |mixed| >= 2/3), the mantissa is that of |mixed|, and +0 comes out as -127.
+          const uint32_t bits = __float_as_uint(mixed);
+          const int32_t ex = int32_t(bits - 0x3f2aaaabu) >> 23;
+          lg = log2f(__uint_as_float(bits - (uint32_t(ex) << 23))) + float(ex);
+        }
+        const float mult = exp2f(F.tf_hlg_exp * lg);
 #pragma unroll
         for (int c = 0; c < 3; c++) v[c] *= mult;
       }

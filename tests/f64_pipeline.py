@@ -6,8 +6,9 @@ so that an implementation can be checked one stage at a time with its own input:
 
   A  coefficients -> XYB planes [3][yb*8][xb*8]   frame/group.rs:85-236,454-613, jxl_transforms/src/transform.rs:14-665
   B  Gaborish, EPF                                render/stages/gaborish.rs, features/epf.rs:54-79, render/stages/epf/
-  C  XYB -> linear, output curve, f32 / u8 store  render/stages/xyb.rs:197-241, color/tf.rs:13-44,114-150,268-304,
-                                                 stages/convert.rs:574-605 (linear, sRGB, BT.709 and PQ outputs)
+  C  XYB -> linear, output curve, stores         render/stages/xyb.rs:197-241, color/tf.rs:13-44,114-150,268-304,
+                                                 381-497, from_linear.rs:97-109 (every curve), stages/convert.rs:574-605,
+                                                 739-762,831-857 (u8, u16, f16), render/save.rs (orientation)
 
 Every stage also returns a magnitude M per output sample: the same computation on absolute values (|basis| on |input|,
 |weights| on |input|, first-order propagation through the non-linear steps). An f32 implementation of the stage is then
@@ -305,6 +306,9 @@ class Frame:
         self.opsin_biases = np.array(list(d.opsin_biases), np.float64)
         self.intensity_target = float(d.intensity_target)
         self.output_tf, self.orientation = int(d.output_tf), int(d.orientation)
+        self.output_gamma = float(d.output_gamma)
+        self.output_luminances = np.array(list(d.output_luminances), np.float64)
+        self.output_format = int(d.output_format)
         self.dequant = {}
 
     def matrix(self, t):
@@ -586,18 +590,123 @@ def linear_to_pq_f64(v, intensity_target, mag=None):
     return out, np.abs(out) + np.abs(slope) * mag
 
 
-# Gamma and HLG are left out: the reference evaluates them with fast_powf / fast_log2f (util/fast_math.rs, relative error
-# up to 3e-5, far above f32 rounding) and the CUDA kernels with exp2f / log2f, so no f32-rounding bound separates a right
-# implementation from a wrong one. test_kat_colour.py holds the oracle's curves to the reference's own bars instead.
-SUPPORTED_TF = (TF_LINEAR, TF_SRGB, TF_BT709, TF_PQ)
+LN2 = np.log(2.0)
+# CUDA's documented accuracy of the device functions the output curves use (CUDA C Programming Guide, "Mathematical
+# Functions"; the library is built without --use_fast_math): log2f 1 ulp, exp2f 2 ulp. One ulp of y is at most 2^-23 |y|,
+# i.e. 2 EPS |y|. They enter the magnitudes explicitly: numpy's own functions are more accurate, so a float32 emulation
+# alone would set too tight a bar.
+ULP_EXP2 = 2 * 2.0   # exp2f: 2 ulp of the result, in EPS |y|
+ULP_LOG2 = 2 * 1.0 + 1.0  # log2f: 1 ulp of the log, plus the rounding of the product g * log2 a, in EPS |g log2 a|
+# The reference's fast_powf / fast_log2f (util/fast_math.rs:151) are good to about 3e-5 relative: the bar the oracle,
+# which restates them, is held to on top of the f32 bound.
+FAST_REL = 3e-5
+_LOG2_P = _f32([-1.8503833400518310e-6, 1.4287160470083755, 7.4245873327820566e-1])  # fast_math.rs:116-125
+_LOG2_Q = _f32([9.9032814277590719e-1, 1.0096718572241148, 1.7409343003366853e-1])
+FAST_LOG2_ZERO = _LOG2_P[0] / _LOG2_Q[0] - 127.0  # fast_log2f(+0.0) = -127.0000019
+HLG_A = 0.17883277
+HLG_B, HLG_C = 1 - 4 * HLG_A, 0.5599107295
 
 
-def stage_c(fr, xyb, mag=None):
-    """xyb: filtered coded frame (3, h, w). Returns the RGB_F32 output (h, w, 3) and its magnitude (orientation 1)."""
-    if fr.orientation not in (0, 1):
-        raise NotImplementedError("orientation")
-    if fr.output_tf not in SUPPORTED_TF:
-        raise NotImplementedError(f"output transfer function {fr.output_tf}")
+def _concave_term(a, m, g, scale=1.0):
+    """Propagated error of scale * a^g (0 < g < 1) for an input error K EPS m, in EPS units: the slope at a, but never
+    more than (K EPS m)^g (the slope grows without bound at 0, the function's change does not)."""
+    kb = BOUND_K["C"] * EPS * m
+    with np.errstate(divide="ignore", invalid="ignore"):
+        slope = scale * g * np.maximum(a, 1e-300) ** (g - 1) * m
+        cap = scale * kb ** g / (BOUND_K["C"] * EPS)
+    return np.where(m > 0, np.minimum(slope, cap), 0.0)
+
+
+def linear_to_gamma_f64(v, g, mag=None):
+    """from_linear.rs:97-109 as the kernel computes it: sign(v) |v|^g, exactly (no fast_powf), 0 at 0. Magnitude:
+    |y| (1 ulp-terms of exp2f and log2f, the latter scaled by ln2 |g log2 a|) plus the input's through the slope.
+    Also returns the oracle's extra allowance: FAST_REL |y|."""
+    a = np.abs(v)
+    pos = a > 0
+    y = np.where(pos, np.where(pos, a, 1.0) ** g, 0.0)
+    out = np.copysign(y, v)
+    if mag is None:
+        return out
+    l2 = np.abs(g * np.log2(np.where(pos, a, 1.0)))
+    m = y * (ULP_EXP2 + ULP_LOG2 * LN2 * l2) + (_concave_term(a, mag, g) if g < 1 else g * (a + mag) ** (g - 1) * mag)
+    return out, m, FAST_REL * y
+
+
+def hlg_exponent(intensity_target):
+    """color/tf.rs:437-445 hlg_display_to_scene in float32, as the front-end computes it; 0 when |e| < 0.1 skips the
+    inverse OOTF (tf.rs:380-382). e < 0 above about 600 nits, e > 0 below about 160."""
+    f = np.float32
+    sg = f(1.2) * np.power(f(1.111), np.log2(f(intensity_target) / f(1e3)))
+    e = (f(1.0) - sg) / sg
+    return 0.0 if abs(float(e)) < 0.1 else float(e)
+
+
+def fast_log2_of_mixed(mixed):
+    """The log2 the inverse OOTF takes of the mixed luminance (tf.rs:386, fast_log2f: fast_math.rs:128-137), for the
+    sign cases where fast_log2f and log2 part:
+      mixed > 0             log2(mixed) (fast_log2f's own error is the oracle's FAST_REL allowance)
+      mixed < 0, |m| < 2/3  log2|mixed| + 256: the wrapping subtraction of 0x3f2aaaab carries the sign bit into the
+                            exponent (2/3 is where that subtraction changes sign: 0x3f2aaaab is the bits of 2/3)
+      mixed < 0, |m| >= 2/3 log2|mixed| - 256
+      mixed = +0            fast_log2f(0) = P0 / Q0 - 127 (the mantissa comes out as 1.0)
+      mixed = -0            the same + 256
+    Plain log2 is NaN for all the non-positive cases."""
+    a = np.abs(mixed)
+    neg = np.signbit(mixed)
+    with np.errstate(divide="ignore"):
+        lg = np.log2(np.where(a > 0, a, 1.0))
+    small = np.float32(a).view(np.uint32) < 0x3f2aaaab
+    lg = np.where(neg, lg + np.where(small, 256.0, -256.0), lg)
+    return np.where(a == 0, FAST_LOG2_ZERO + np.where(neg, 256.0, 0.0), lg)
+
+
+def linear_to_hlg_f64(rgb, intensity_target, luminances, mag=None):
+    """Inverse OOTF with the output luminances (tf.rs:384-391), then the HLG OETF (tf.rs:481-497), both exact: rgb and
+    mag (3, h, w). Magnitude of the OOTF factor mult = 2^(e log2 mixed), relative: exp2f and log2f ulps as for gamma,
+    plus the rounding of mixed through |e| / |mixed|. Where |mixed| is within the f32 bound of 0 its sign, and with it
+    the +256 branch, is not determined by f32 arithmetic: those samples get an infinite magnitude (any finite output).
+    OETF: sqrt(3a) up to 1/12 (slope capped as for gamma), a ln(12a - b) + c above (slope 12a / (12a - b), log2f ulp).
+    Returns (out, M, oracle allowance, mask of samples with an undetermined sign of mixed)."""
+    e = hlg_exponent(intensity_target)
+    x = np.asarray(rgb, np.float64)
+    mx = np.abs(x) if mag is None else mag
+    amb = np.zeros(x.shape[1:], bool)
+    if e != 0.0:
+        lum = np.asarray(luminances, np.float64)[:, None, None]
+        mixed = (x * lum).sum(axis=0)
+        mmix = 2.0 * (np.abs(lum) * mx).sum(axis=0)
+        L = e * fast_log2_of_mixed(mixed)
+        mult = 2.0 ** L
+        amb = np.abs(mixed) <= BOUND_K["C"] * EPS * mmix
+        with np.errstate(divide="ignore"):
+            rel = ULP_EXP2 + ULP_LOG2 * LN2 * np.abs(L) + np.abs(e) * mmix / np.abs(mixed)
+        x = x * mult[None]
+        mx = np.abs(x) * (1.0 + rel[None]) + mult[None] * mx
+        mx = np.where(amb[None], np.inf, mx)
+    a = np.abs(x)
+    low = a <= 1.0 / 12.0
+    arg = np.maximum(12.0 * a - HLG_B, 1e-300)
+    y = np.where(low, np.sqrt(3.0 * a), HLG_A * np.log(arg) + HLG_C)
+    out = np.copysign(y, x)
+    if mag is None:
+        return out
+    with np.errstate(invalid="ignore"):
+        m_low = 2.0 * y + _concave_term(a, mx, 0.5, np.sqrt(3.0))
+        m_high = (3.0 * y + HLG_A * LN2 * ULP_LOG2 * np.abs(np.log2(arg)) + HLG_A * (12.0 * a + arg) / arg
+                  + 12.0 * HLG_A / arg * mx)
+    m = np.where(low, m_low, m_high)
+    # the oracle: FAST_REL on mult times the OETF's slope d out / d ln a, and FAST_REL on its log term
+    allow = (np.where(low, 0.5 * y, 12.0 * HLG_A * a / arg) * FAST_REL * (e != 0.0)
+             + np.where(low, 0.0, FAST_REL * HLG_A * np.abs(np.log(arg))))
+    return out, m, allow, amb
+
+
+def stage_c(fr, xyb, mag=None, full=False):
+    """xyb: filtered coded frame (3, h, w). Returns the RGB_F32 output (h, w, 3) of the coded image (orientation 1:
+    `orient` turns it) and its magnitude. With full=True also the oracle's extra allowance for the approximate power and
+    log of gamma / HLG (0 elsewhere) and the mask of HLG samples whose mixed luminance has no determined sign."""
+    if fr.output_tf not in (TF_LINEAR, TF_SRGB, TF_GAMMA, TF_BT709, TF_PQ, TF_HLG):
+        raise ValueError(f"output transfer function {fr.output_tf}")
     m_in = np.abs(xyb) if mag is None else mag
     x, y, b = xyb
     mx, my, mb = m_in
@@ -613,15 +722,43 @@ def stage_c(fr, xyb, mag=None):
     mat = fr.opsin_inverse_matrix
     rgb = np.einsum("ij,jhw->ihw", mat, lms)  # xyb.rs:231-233
     mrgb = np.einsum("ij,jhw->ihw", np.abs(mat), mlms)
+    allow = np.zeros_like(rgb)
+    amb = np.zeros(rgb.shape[1:], bool)
     if fr.output_tf == TF_SRGB:
         rgb, mrgb = linear_to_srgb_f64(rgb, mrgb)
     elif fr.output_tf == TF_BT709:
         rgb, mrgb = linear_to_bt709_f64(rgb, mrgb)
     elif fr.output_tf == TF_PQ:
         rgb, mrgb = linear_to_pq_f64(rgb, fr.intensity_target, mrgb)
-    return rgb.transpose(1, 2, 0), mrgb.transpose(1, 2, 0)
+    elif fr.output_tf == TF_GAMMA:
+        rgb, mrgb, allow = linear_to_gamma_f64(rgb, fr.output_gamma, mrgb)
+    elif fr.output_tf == TF_HLG:
+        rgb, mrgb, allow, amb = linear_to_hlg_f64(rgb, fr.intensity_target, fr.output_luminances, mrgb)
+    out = (rgb.transpose(1, 2, 0), mrgb.transpose(1, 2, 0))
+    return out + (allow.transpose(1, 2, 0), amb) if full else out
 
 
+def linear_rgb_f64(fr, xyb):
+    """Stage C up to the output curve: display-referred linear RGB (h, w, 3), for sorting samples into value regions."""
+    lin = Frame.__new__(Frame)
+    lin.__dict__.update(fr.__dict__)
+    lin.output_tf = TF_LINEAR
+    return stage_c(lin, xyb)[0]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Orientation (render/save.rs, headers/image_metadata.rs:85-96 display_pixel)
+# ---------------------------------------------------------------------------------------------------------------------
+def orient(img, o):
+    """The coded image (h, w, ...) as the save stage places it for orientation o (0 counts as 1)."""
+    t = img.swapaxes(0, 1)
+    return {0: img, 1: img, 2: img[:, ::-1], 3: img[::-1, ::-1], 4: img[::-1], 5: t, 6: np.rot90(img, k=-1),
+            7: t[::-1, ::-1], 8: np.rot90(img, k=1)}[o]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Stores
+# ---------------------------------------------------------------------------------------------------------------------
 def u8_store_f64(rgb):
     """convert.rs:574-605: v * 255 + dither[(y + 13 c) % 32][(x + 23 c) % 32], clamped to [0, 255], before rounding."""
     h, w, _ = rgb.shape
@@ -630,29 +767,180 @@ def u8_store_f64(rgb):
     return np.clip(rgb * 255.0 + d, 0.0, 255.0)
 
 
+def u16_store_f64(v):
+    """convert.rs:739-762 at bit depth 16: clamp to [0, 1], scale by 65535, round to nearest (ties to even)."""
+    return np.rint(np.clip(v, 0.0, 1.0) * 65535.0)
+
+
+def f16_from_f32(v):
+    """util/float16.rs:82-141 f16::from_f32 on float32 values, at bit level; returns the uint16 codes. Normal halves are
+    rounded to nearest even (and may overflow to infinity), f32 zeros and subnormals give a signed zero, |v| below
+    2^-24 gives zero, and the f16 subnormal range 2^-24 <= |v| < 2^-14 is TRUNCATED, shifting one bit further than
+    IEEE (2^-15 becomes 2^-16). Infinities stay infinite, NaN becomes the quiet NaN 0x7e00 with its sign."""
+    bits = np.asarray(v, np.float32).view(np.uint32).astype(np.int64)
+    sign = ((bits >> 31) & 1) << 15
+    exp = (bits >> 23) & 0xFF
+    mant = bits & 0x7FFFFF
+    unb = exp - 127
+    shift = np.clip(-14 - unb, 0, 31)
+    sub = (mant | 0x800000) >> (shift + 14)
+    h_exp = unb + 15
+    h_mant = mant >> 13
+    up = (((mant >> 12) & 1) == 1) & (((mant & 0xFFF) != 0) | ((h_mant & 1) == 1))
+    h_mant = h_mant + up
+    normal = np.where(h_mant > 0x3FF, np.where(h_exp >= 30, 0x1F << 10, (h_exp + 1) << 10), (h_exp << 10) | h_mant)
+    code = np.select([exp == 0, exp == 255, unb < -24, unb < -14, unb > 15],
+                     [0, np.where(mant == 0, 0x1F << 10, (0x1F << 10) | 0x200), 0, sub, 0x1F << 10], normal)
+    return (sign | code).astype(np.uint16)
+
+
+def f16_value(codes):
+    return np.asarray(codes, np.uint16).view(np.float16).astype(np.float64)
+
+
+def f16_store_f64(v, tf):
+    """convert.rs:831-857 with the clamp of frame/render.rs:746-750 ([0, 1] for PQ, [-0.074, 1.1] for HLG), after the
+    f32 rounding of the value; returns the decoded half values."""
+    v = np.asarray(v, np.float64)
+    if tf == TF_PQ:
+        v = np.clip(v, 0.0, 1.0)
+    elif tf == TF_HLG:
+        v = np.clip(v, -0.074, 1.1)
+    return f16_value(f16_from_f32(np.float32(v)))
+
+
+FMT_U8, FMT_RGBA_U8, FMT_F32, FMT_XYB, FMT_U16, FMT_F16 = 0, 1, 2, 3, 4, 5  # include/jxg.h JXG_FORMAT_*
+
+
+def store(fmt, v, tf):
+    """The output samples of the coded image v (h, w, 3), as float64: u8 / u16 codes, decoded halves, or v for f32."""
+    if fmt in (FMT_U8, FMT_RGBA_U8):
+        return np.rint(u8_store_f64(v))
+    if fmt == FMT_U16:
+        return u16_store_f64(v)
+    if fmt == FMT_F16:
+        return f16_store_f64(v, tf)
+    return np.asarray(v, np.float64)
+
+
+def output_values(fmt, got):
+    """An output buffer (display orientation) as float64 samples (h, w, 3); RGBA must be opaque (alpha 255)."""
+    got = np.asarray(got)
+    if fmt == FMT_RGBA_U8:
+        assert (got[..., 3] == 255).all(), "RGBA alpha is not 255"
+        got = got[..., :3]
+    if fmt == FMT_F16:
+        return f16_value(got.view(np.uint16) if got.dtype != np.uint16 else got)
+    return got.astype(np.float64)
+
+
 def bound(stage, mag):
     return BOUND_K[stage] * EPS * mag + 1e-9
 
 
-def check(stage, got, ref, mag, what=""):
-    """Asserts the stage bound; the message reports the largest err / (2^-24 M)."""
-    err = np.abs(np.asarray(got, np.float64) - ref)
-    ratio = float((err / (EPS * mag + 1e-300)).max()) if err.size else 0.0
-    bad = err > bound(stage, mag)
+def check(stage, got, ref, mag, what="", extra=0.0):
+    """Asserts the stage bound (plus `extra`, the oracle's allowance for approximate functions); a NaN or infinite
+    sample where the reference is finite always fails. The message reports the largest err / (2^-24 M)."""
+    got = np.asarray(got, np.float64)
+    err = np.abs(got - ref)
+    with np.errstate(invalid="ignore"):
+        ratio = float(np.nanmax(np.where(np.isfinite(mag), err / (EPS * mag + 1e-300), 0.0))) if err.size else 0.0
+        bad = ~(err <= bound(stage, mag) + extra) | (np.isfinite(ref) & ~np.isfinite(got))
     assert not bad.any(), (f"{what} stage {stage}: {int(bad.sum())} of {bad.size} samples outside K={BOUND_K[stage]}; "
                            f"largest err/(2^-24 M) = {ratio:.3g}, largest err = {float(err.max()):.3g}")
     return ratio
 
 
-def check_u8(got, pre, mag, what=""):
-    """u8 output against the f64 value before rounding: equal to its rounding wherever that value is further than
-    max(1e-3, the f32 bound of stage C in LSB) from a rounding boundary, within 1 elsewhere."""
-    got = np.asarray(got, np.int32)
-    want = np.rint(pre).astype(np.int32)
-    margin = np.maximum(1e-3, 255.0 * bound("C", mag))
-    near = np.abs((pre - np.floor(pre)) - 0.5) <= margin
-    diff = np.abs(got - want)
-    assert diff.max(initial=0) <= 1, f"{what} u8: differs by {diff.max()}"
-    far_bad = (diff != 0) & ~near
-    assert not far_bad.any(), f"{what} u8: {int(far_bad.sum())} samples away from a rounding boundary differ"
-    return int((diff != 0).sum())
+def check_output(fmt, got, ref, mag, tf, orientation=1, what="", extra=0.0):
+    """An output buffer (display orientation) against stage C of the coded image (ref, mag: (h, w, 3)). F32: the stage
+    bound. Integer and half stores: every code must lie between store(ref - b) and store(ref + b), b the stage-C bound
+    (plus `extra`) of the sample. Every store is monotone, so this accepts exactly the codes an implementation exact to
+    f32 rounding could produce. Returns the largest err / (2^-24 M) (F32) or the number of codes != store(ref)."""
+    if fmt == FMT_F32:
+        return check("C", got, orient(ref, orientation), orient(mag, orientation), what, orient(extra, orientation)
+                     if np.ndim(extra) else extra)
+    g = output_values(fmt, got)
+    b = bound("C", mag) + extra
+    with np.errstate(invalid="ignore"):
+        lo, hi = (orient(store(fmt, ref + s * b, tf), orientation) for s in (-1.0, 1.0))
+    bad = ~((g >= lo) & (g <= hi))
+    assert g.shape == lo.shape, f"{what} format {fmt}: shape {g.shape}, want {lo.shape}"
+    assert not bad.any(), (f"{what} format {fmt}: {int(bad.sum())} of {bad.size} samples outside "
+                           f"[store(ref - b), store(ref + b)]; first at {np.argwhere(bad)[0].tolist()}: got "
+                           f"{g[bad][0]}, allowed [{lo[bad][0]}, {hi[bad][0]}]")
+    return int((g != orient(store(fmt, ref, tf), orientation)).sum())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Edge-value frames: a parsed frame whose LF field is overwritten so that the output stage sees chosen linear values
+# ---------------------------------------------------------------------------------------------------------------------
+BT2100_LUMINANCES = (0.2627, 0.6780, 0.0593)
+
+
+def edge_targets():
+    """Linear display RGB targets, one per 2x2-block cell: black; each sign pattern with a negative channel; a negative
+    luminance with positive channels; values above 1; and greys from 1e-7 to 3, 1.25x apart, which put samples on both
+    sides of every curve's breakpoint (sRGB 0.0031308, BT.709 0.018, PQ 1e-4, HLG 1/12) and into the f16 subnormals."""
+    t = [(0.0, 0.0, 0.0)]
+    for k in range(1, 8):
+        s = [-1.0 if k >> i & 1 else 1.0 for i in range(3)]
+        t += [(0.2 * s[0], 0.1 * s[1], 0.05 * s[2]), (0.02 * s[0], 0.03 * s[1], 0.01 * s[2])]
+    t += [(0.3, -0.2, 0.1), (-0.3, 0.05, 0.2), (0.05, -0.04, 0.3)]
+    t += [(1.5, 1.2, 1.1), (2.0, 0.5, 0.2)]
+    t += [(g, g, g) for g in 1e-7 * 1.25 ** np.arange(78)]
+    return np.array(t, np.float64)
+
+
+def edge_lf(fr, targets, intensity_target, cell=2):
+    """LF planes (3, yb, xb) float32 that decode to `targets` (n, 3) on flat blocks, by inverting XYB -> linear
+    (xyb.rs:197-241) through the frame's opsin matrix and biases in float64. Targets repeat in cells of cell x cell blocks."""
+    isc = 255.0 / intensity_target
+    lms = np.linalg.solve(fr.opsin_inverse_matrix, targets.T)  # (3, n)
+    cube = (lms - (fr.opsin_biases * isc)[:, None]) / isc
+    l, m, s = np.cbrt(cube) + np.cbrt(fr.opsin_biases)[:, None]
+    xyb = np.stack([(l - m) / 2, (l + m) / 2, s])
+    cy, cx = (fr.yb + cell - 1) // cell, (fr.xb + cell - 1) // cell
+    idx = np.arange(cy * cx).reshape(cy, cx) % len(targets)
+    idx = np.repeat(np.repeat(idx, cell, 0), cell, 1)[:fr.yb, :fr.xb]
+    return np.ascontiguousarray(xyb[:, idx].astype(np.float32))
+
+
+def edit_desc(d, lf=None, **fields):
+    """Overwrites fields of a JxgFrameDesc in place (output_luminances as a 3-sequence); lf: (3, yb, xb) float32 planes,
+    which the caller keeps alive while the descriptor is used. Returns the descriptor."""
+    for k, v in fields.items():
+        if k == "output_luminances":
+            for i in range(3):
+                d.output_luminances[i] = v[i]
+        else:
+            setattr(d, k, v)
+    if lf is not None:
+        for c in range(3):
+            d.lf[c] = lf[c].ctypes.data
+    return d
+
+
+# Curves that lift every small value out of the f16 subnormals: the powers 1/2.2 and 1/2.6 and HLG's sqrt at 100 nits
+# (the edge targets' smallest grey, 1e-7, maps to 6.6e-4 or more there).
+NO_F16_SUBNORMALS = ("gamma2.2", "dci", "hlg100")
+
+
+def edge_regions(lin, out, tf, luminances):
+    """Number of samples in each edge region, from the f64 linear RGB (h, w, 3) and the f64 output `out` of one frame.
+    Every region must be non-empty for a frame to keep its edge coverage."""
+    a = np.abs(lin)
+    neg = lin < -1e-3
+    r = {"black": int((a.max(axis=-1) < 1e-5).sum()), "above_1": int((lin > 1.0).sum()),
+         "f16_subnormal": int(((np.abs(out) < 2.0 ** -14) & (np.abs(out) > 2.0 ** -24)).sum())}
+    for k in range(1, 8):
+        want = np.array([bool(k >> i & 1) for i in range(3)])
+        r[f"signs{k}"] = int((neg == want).all(axis=-1).sum())
+    mixed = lin @ np.asarray(luminances, np.float64)
+    r["mixed_neg_with_pos"] = int(((mixed < -1e-3) & (lin > 1e-3).any(axis=-1)).sum())
+    bp = {TF_SRGB: 0.0031308, TF_BT709: 0.018, TF_PQ: 1e-4}.get(tf)
+    if tf == TF_HLG:  # the OETF's breakpoint, on the output side: sqrt(3 / 12) = 0.5
+        a, bp = np.abs(out), 0.5
+    if bp is not None:
+        r["below_breakpoint"] = int(((a < bp) & (a > bp / 1.5)).sum())
+        r["above_breakpoint"] = int(((a >= bp) & (a < bp * 1.5)).sum())
+    return r

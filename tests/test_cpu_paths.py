@@ -79,12 +79,13 @@ def test_synthetic_writer_round_trip(case):
 
 
 def test_orientation_is_applied_like_the_reference_save_stage():
-    """headers/image_metadata.rs:85-96 display_pixel, written here as numpy flips / transposes of the identity decode."""
+    """headers/image_metadata.rs:85-96 display_pixel, as numpy flips / transposes (f64_pipeline.orient) of the identity
+    decode."""
     import synth
+    from tests import f64_pipeline as fp
     from tests import oracle_binding as ob
     base, _ = ob.decode_file(synth.encode_synthetic(200, 120, 5, 0.5, 2, 1, 1), abi.FORMAT_RGB_U8)
-    want = {1: base, 2: base[:, ::-1], 3: base[::-1, ::-1], 4: base[::-1], 5: base.transpose(1, 0, 2),
-            6: np.rot90(base, k=-1), 7: base.transpose(1, 0, 2)[::-1, ::-1], 8: np.rot90(base, k=1)}
+    want = {o: fp.orient(base, o) for o in range(1, 9)}
     for o in range(1, 9):
         data = synth.encode_synthetic(200, 120, 5, 0.5, 2, 1, 1, orientation=o)
         info = ob.file_info(data)

@@ -118,7 +118,7 @@ def _check_frames(ctx, datas, what):
         rc = fp.check("C", rgb[i], c, mc, what)
         fr8 = fp.Frame(pf.desc(abi.FORMAT_RGB_U8)[0])
         c8, mc8 = fp.stage_c(fr8, xyb[i].astype(np.float64))
-        fp.check_u8(rgb8[i], fp.u8_store_f64(c8), mc8, what)
+        fp.check_output(fp.FMT_U8, rgb8[i], c8, mc8, fr8.output_tf, 1, what)
         report.append((ra, rb, rc))
     print(what, "largest err/(2^-24 M) per stage:", report)
 

@@ -87,16 +87,25 @@ def test_orientation(ctx, orientation):
 
 @pytest.mark.parametrize("orientation,colour", [(1, 0), (6, 0), (1, 5), (1, 6)])
 def test_sixteen_bit_output_samples(ctx, orientation, colour):
-    """a17: U16 (convert.rs:717-786) and F16 (convert.rs:789-857, clamp ranges of PQ / HLG outputs frame/render.rs:746-750)
-    against the oracle: u16 within 1 LSB (= 1.5e-5), f16 within one half-precision step; interior vector tiles, edge tiles
-    and the orientation post-pass all carry 6-byte pixels."""
+    """a17: U16 (convert.rs:717-786) and F16 (convert.rs:789-857, clamp ranges of PQ / HLG outputs frame/render.rs:746-750):
+    every code between store(ref - b) and store(ref + b), ref the float64 stage C of the GPU's own filtered planes and b
+    its f32 bound (tests/f64_pipeline.py); the oracle's codes must meet the same rule on its own planes. Interior
+    tiles, edge tiles and the orientation post-pass all carry 6-byte pixels."""
     import synth
     import torch
     import jxl_rs_b200 as j
+    from tests import f64_pipeline as fp
     from tests import oracle_binding as ob
     w, h = 333, 271
     data = synth.encode_synthetic(w, h, 77, 0.5, 2, 1, 1, orientation=orientation, colour=colour)
     fr = j.ParsedFrame(data)
+    xyb = torch.empty((3, h, w), dtype=torch.float32).pin_memory()
+    b = j.Batch(ctx, 1)
+    b.add(fr, xyb.data_ptr(), w * 4, abi.FORMAT_XYB_F32_PLANAR, False)
+    b.run()
+    b.wait()
+    b.close()
+    _, taps = ob.decode_file(data, abi.FORMAT_RGB_F32, taps=True)
     for fmt, dt in ((abi.FORMAT_RGB_U16, torch.uint16), (abi.FORMAT_RGB_F16, torch.float16)):
         ref, _ = ob.decode_file(data, fmt)
         out = torch.empty((fr.height, fr.width, 3), dtype=dt).pin_memory()
@@ -105,15 +114,12 @@ def test_sixteen_bit_output_samples(ctx, orientation, colour):
         b.run()
         b.wait()
         b.close()
-        if fmt == abi.FORMAT_RGB_U16:
-            got = out.view(torch.int16).numpy().view(np.uint16).astype(np.int64)
-            assert np.abs(got - ref.astype(np.int64)).max() <= 64  # 1e-3 of full scale, the float tolerance of the stages before
-            assert np.mean(got == ref) > 0.5
-        else:
-            got = out.view(torch.int16).numpy().view(np.float16).astype(np.float64)
-            r = ref.astype(np.float64)
-            assert np.all(np.isfinite(got))
-            assert np.abs(got - r).max() <= 1e-3 * max(1.0, np.abs(r).max()) + 2 ** -11
+        d = fp.Frame(fr.desc(fmt)[0])
+        got = out.view(torch.int16).numpy().view(np.uint16)
+        for codes, planes, who in ((got, xyb.numpy(), "GPU"), (ref, taps["xyb_filtered"], "oracle")):
+            c, mc, allow, _ = fp.stage_c(d, planes.astype(np.float64), full=True)
+            fp.check_output(fmt, codes, c, mc, d.output_tf, d.orientation, f"{who} format {fmt}",
+                            allow if who == "oracle" else 0.0)
 
 
 @pytest.mark.parametrize("colour", [1, 2, 3, 4, 5, 6, 7])
