@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../jxl_rs_b200/csrc/host/frame.h"  // library dequant tables, natural orders, geometry tables
+#include "../jxl_rs_b200/csrc/host/quant.h"  // custom dequant tables
 #include "entropy_writer.h"
 
 namespace jxs {
@@ -51,6 +52,14 @@ struct Params {
   // 3 P3 / D65 / PQ at 1000 nits, 4 BT2100 / D65 / HLG at 1000 nits, 5 custom primaries / DCI white / BT709, 6 grey sRGB,
   // 7 DCI transfer function with the E white point
   uint32_t colour = 0;
+  uint32_t x_qm_scale = 3, b_qm_scale = 2;  // FrameHeader, 0..7 (group.rs:395-396)
+  // Custom dequantisation matrices, one entry per table index (see jxs_encode_synthetic_ex); all mode 0 = all_default
+  struct DequantSpec {
+    uint32_t mode = 0;                                   // quant_weights.rs:128 (0 library, 1..7)
+    std::vector<std::pair<uint32_t, unsigned>> fields;   // (value, bits) after the mode, in the reader's order
+    std::vector<int32_t> raw;                            // mode 7: 3 channels of 8*REQUIRED_SIZE_X columns
+  };
+  std::vector<DequantSpec> dequant = {};                 // empty or kNumQuantTables entries
 };
 
 // Worker threads inside one encode (jxs_set_threads): only loops whose result does not depend on the order of
@@ -340,7 +349,10 @@ static void plan_transforms(Frame& f) {
     for (uint32_t bx = 0; bx < f.xb; bx++) {
       if (f.transform_map[size_t(by) * f.xb + bx] != 255) continue;
       int t = 0;
-      if (f.p.profile >= 1) {
+      if (f.p.profile == 4) {  // also IDENTITY, DCT2X2 and AFV0-3 (random coefficients, see random_coeff_type)
+        static const int kTypes[10] = {0, 12, 13, 3, 1, 2, 14, 15, 16, 17};
+        t = kTypes[rng.below(10)];
+      } else if (f.p.profile >= 1) {
         uint32_t r = rng.below(100);
         t = r < 70 ? 0 : r < 80 ? 12 : r < 90 ? 13 : 3;  // DCT, DCT4X8, DCT8X4, DCT4X4
       }
@@ -351,6 +363,10 @@ static void plan_transforms(Frame& f) {
       if (f.transform_map[size_t(by) * f.xb + bx] & 128) f.blocks.push_back(Varblock{uint16_t(bx), uint16_t(by), uint8_t(f.transform_map[size_t(by) * f.xb + bx] & 127)});
 }
 
+// IDENTITY, DCT2X2 and AFV0-3 have no forward transform here: their varblocks get the block mean as LF and random
+// sparse quantised coefficients, valid input for the decoder but not a picture of the source.
+static bool random_coeff_type(int t) { return t == 1 || t == 2 || (t >= 14 && t <= 17); }
+
 // Transforms one varblock of one channel: returns coefficients in *storage*
 // layout plus the cy x cx LF samples.
 static void forward_varblock(int t, const float* px, size_t stride, std::vector<float>& co, std::vector<float>& lf) {
@@ -358,11 +374,12 @@ static void forward_varblock(int t, const float* px, size_t stride, std::vector<
   const int R = 8 * cy, C = 8 * cx;
   co.assign(size_t(R) * C, 0.0f);
   lf.assign(size_t(cx) * cy, 0.0f);
-  if (t == 12 || t == 13 || t == 3) {
+  if (t == 12 || t == 13 || t == 3 || random_coeff_type(t)) {
     float mean = 0;
     for (int y = 0; y < 8; y++)
       for (int x = 0; x < 8; x++) mean += px[size_t(y) * stride + x];
     lf[0] = mean / 64.0f;
+    if (random_coeff_type(t)) return;
     if (t == 12) {  // DCT4X8: halves along y, each 4 rows x 8 cols (transform.rs:638-661)
       float D[2][32];
       for (int h = 0; h < 2; h++) forward_dct2d(px + size_t(h) * 4 * stride, stride, 4, 8, D[h]);
@@ -621,7 +638,34 @@ std::vector<uint8_t> encode(const Params& p) {
   f.global_scale = std::max<uint32_t>(1, std::min<uint32_t>(65535, uint32_t(std::lround(4587.0 / std::max(0.05f, p.distance)))));
   f.quant_lf = 16;
   const float inv_global_scale = 65536.0f / float(f.global_scale);
-  const float x_dm = std::pow(1.0f / 1.25f, 3.0f - 2.0f), b_dm = std::pow(1.0f / 1.25f, 2.0f - 2.0f);  // x_qm_scale 3, b_qm_scale 2
+  const float x_dm = std::pow(1.0f / 1.25f, float(p.x_qm_scale) - 2.0f), b_dm = std::pow(1.0f / 1.25f, float(p.b_qm_scale) - 2.0f);
+  // the dequantisation tables the decoder will use, computed by the front-end from the fields as written
+  std::vector<float> custom_tables[jxg::kNumQuantTables];
+  const float* tables[jxg::kNumQuantTables];
+  for (int i = 0; i < jxg::kNumQuantTables; i++) {
+    tables[i] = jxg::library_dequant_table(i).data();
+    if (p.dequant.empty() || p.dequant[i].mode == 0) continue;
+    const Params::DequantSpec& s = p.dequant[i];
+    try {
+      jxg::QuantEncoding e;
+      if (s.mode == 7) {
+        e.mode = jxg::QuantEncoding::kRaw;
+        e.qtable_den = jxg::f16_bits_to_float(uint16_t(s.fields.at(0).first));
+        e.qtable = s.raw;
+      } else {
+        BitWriter w;
+        w.write(s.mode, 3);
+        for (auto& fb : s.fields) w.write(fb.first, fb.second);
+        std::vector<uint8_t> bytes = w.finish();
+        jxg::BitReader br(bytes.data(), bytes.size());
+        e = jxg::read_quant_encoding(i, br, jxg::FrameHeader(), nullptr);
+      }
+      custom_tables[i] = jxg::compute_dequant_table(e, i);
+      tables[i] = custom_tables[i].data();
+    } catch (const jxg::Error&) {
+      // an encoding the decoder refuses: written as given, the coefficients quantised with the library table
+    }
+  }
   Rng rng(p.seed ^ 0x5151ull);
   plan_transforms(f);
   const size_t nb = size_t(f.xb) * f.yb;
@@ -671,7 +715,7 @@ std::vector<uint8_t> encode(const Params& p) {
         f.lfq[2][o] = int32_t(std::lround((lf[2][i] - yy * 1.0f) / lf_fac[2]));
       }
     // HF (group.rs:100-177 inverted, without the decoder-side bias adjustment)
-    const float* mat = jxg::library_dequant_table(jxg::quant_table_for_transform(t)).data();
+    const float* mat = tables[jxg::quant_table_for_transform(t)];
     const float rq = float(f.raw_quant[size_t(vb.by) * f.xb + vb.bx]);
     const float sy = inv_global_scale / rq, sx = sy * x_dm, sb = sy * b_dm;
     const size_t ci = size_t(vb.by / 8) * cxb + vb.bx / 8;
@@ -683,6 +727,13 @@ std::vector<uint8_t> encode(const Params& p) {
       if (a < 0.58f) return int32_t(0);
       return int32_t(std::copysign(std::floor(a + 0.42f), v));
     };
+    if (random_coeff_type(t)) {  // about one coefficient in four, in [-3, 3]; position 0 is the LF sample
+      Rng cr(p.seed * 0x2545F4914F6CDD1Dull + bi);
+      for (size_t k = 1; k < num_coeffs; k++)
+        for (int c = 0; c < 3; c++)
+          if (cr.below(4) == 0) q[size_t(c) * num_coeffs + k] = int32_t(cr.below(7)) - 3;
+      return;
+    }
     const int R = 8 * int(cy), C = 8 * int(cx);
     const bool plain_dct = !(t == 12 || t == 13 || t == 3);
     for (size_t k = 0; k < num_coeffs; k++) {
@@ -849,7 +900,25 @@ std::vector<uint8_t> encode(const Params& p) {
   }
 
   BitWriter hf_global;
-  hf_global.write(1, 1);                              // dequant matrices all_default
+  bool all_default = true;
+  for (const auto& s : p.dequant) all_default &= s.mode == 0;
+  hf_global.write(all_default ? 1 : 0, 1);            // DequantMatrices all_default (quant_weights.rs:1093)
+  if (!all_default)
+    for (int i = 0; i < jxg::kNumQuantTables; i++) {  // QuantEncoding::decode (quant_weights.rs:117-255)
+      const Params::DequantSpec& s = p.dequant[i];
+      hf_global.write(s.mode, 3);
+      for (auto& fb : s.fields) hf_global.write(fb.first, fb.second);
+      if (s.mode == 7) {  // decode_quant_table (modular/mod.rs:1083-1122): stream 1 + 3 num_lf_groups + i, local tree
+        const uint32_t w = 8u * jxg::kQuantTableRows[i], h = 8u * jxg::kQuantTableCols[i];
+        std::vector<Chan> ch(3);
+        for (int c = 0; c < 3; c++) {
+          ch[c].w = w;
+          ch[c].h = h;
+          ch[c].d.assign(s.raw.begin() + size_t(c) * w * h, s.raw.begin() + size_t(c + 1) * w * h);
+        }
+        write_modular(hf_global, ch, 5);
+      }
+    }
   hf_global.write(0, ceil_log2(f.num_groups));        // num_histograms - 1
   hf_global.write(2, 2);                              // used_orders selector 2 => natural orders
   write_code(hf_global, ac_code);
@@ -958,7 +1027,7 @@ std::vector<uint8_t> encode(const Params& p) {
   out.write(1, 1);  // CustomTransformData all_default
   out.zero_pad_to_byte();
   // FrameHeader (frame_header.rs:267-444)
-  const bool default_header = p.epf_iters == 2 && p.gab == 1;
+  const bool default_header = p.epf_iters == 2 && p.gab == 1 && p.x_qm_scale == 3 && p.b_qm_scale == 2;
   if (default_header) {
     out.write(1, 1);
   } else {
@@ -967,8 +1036,8 @@ std::vector<uint8_t> encode(const Params& p) {
     out.write(0, 1);       // VarDCT
     out.write_u64(0);      // flags
     out.write(0, 2);       // upsampling = 1
-    out.write(3, 3);       // x_qm_scale
-    out.write(2, 3);       // b_qm_scale
+    out.write(p.x_qm_scale, 3);
+    out.write(p.b_qm_scale, 3);
     out.write(0, 2);       // num_passes = 1
     out.write(0, 1);       // have_crop
     out.write(0, 2);       // blending mode Replace
@@ -1038,6 +1107,56 @@ int64_t jxs_encode_synthetic(uint32_t width, uint32_t height, uint64_t seed, flo
     // bits 12..15: orientation - 1, bits 16..19: colour encoding variant
     jxs::Params p{width, height, seed, distance, epf_iters, gab, profile & 0xff, (profile >> 8) & 1, (profile >> 9) & 3,
                   ((profile >> 12) & 7) + 1, (profile >> 16) & 15};
+    std::vector<uint8_t> b = jxs::encode(p);
+    if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
+    return int64_t(b.size());
+  } catch (std::exception& e) {
+    g_err = e.what();
+    return -1;
+  }
+}
+
+// jxs_encode_synthetic with the frame header's x_qm_scale / b_qm_scale and custom dequantisation matrices.
+// dequant: for each of the 17 table indices in turn, the mode (0..7), then
+//   modes 1..7: the number n of fields that follow the mode in the bitstream, then n (value, bits) pairs;
+//   mode 7:     additionally 3 * 64 * REQUIRED_SIZE_X * REQUIRED_SIZE_Y raw entries (int32, each channel in raster
+//               order, 8 * REQUIRED_SIZE_X wide), written as a Modular sub-bitstream after the fields.
+// dequant_len 0: all library tables (the same bitstream as jxs_encode_synthetic).
+int64_t jxs_encode_synthetic_ex(uint32_t width, uint32_t height, uint64_t seed, float distance, uint32_t epf_iters,
+                                uint32_t gab, uint32_t profile, uint32_t x_qm_scale, uint32_t b_qm_scale,
+                                const uint32_t* dequant, size_t dequant_len, uint8_t* out, size_t cap) {
+  try {
+    jxs::Params p{width, height, seed, distance, epf_iters, gab, profile & 0xff, (profile >> 8) & 1, (profile >> 9) & 3,
+                  ((profile >> 12) & 7) + 1, (profile >> 16) & 15};
+    if (x_qm_scale > 7 || b_qm_scale > 7) throw std::runtime_error("x_qm_scale / b_qm_scale must be 0..7");
+    p.x_qm_scale = x_qm_scale;
+    p.b_qm_scale = b_qm_scale;
+    size_t pos = 0;
+    auto next = [&]() -> uint32_t {
+      if (pos >= dequant_len) throw std::runtime_error("dequant array too short");
+      return dequant[pos++];
+    };
+    if (dequant_len) {
+      p.dequant.resize(jxg::kNumQuantTables);
+      for (int i = 0; i < jxg::kNumQuantTables; i++) {
+        jxs::Params::DequantSpec& s = p.dequant[i];
+        s.mode = next();
+        if (s.mode > 7) throw std::runtime_error("dequant mode above 7");
+        if (s.mode == 0) continue;
+        const uint32_t n = next();
+        for (uint32_t k = 0; k < n; k++) {
+          const uint32_t v = next(), bits = next();
+          if (bits > 32) throw std::runtime_error("dequant field wider than 32 bits");
+          s.fields.emplace_back(v, bits);
+        }
+        if (s.mode == 7) {
+          if (s.fields.size() != 1 || s.fields[0].second != 16) throw std::runtime_error("RAW takes one 16-bit field");
+          s.raw.resize(size_t(3) * 64 * jxg::kQuantTableRows[i] * jxg::kQuantTableCols[i]);
+          for (auto& v : s.raw) v = int32_t(next());
+        }
+      }
+      if (pos != dequant_len) throw std::runtime_error("dequant array too long");
+    }
     std::vector<uint8_t> b = jxs::encode(p);
     if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
     return int64_t(b.size());

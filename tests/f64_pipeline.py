@@ -14,8 +14,10 @@ Every stage also returns a magnitude M per output sample: the same computation o
 |weights| on |input|, first-order propagation through the non-linear steps). An f32 implementation of the stage is then
 bounded by |got - ref| <= K * 2^-24 * M + 1e-9 with one K per stage (BOUND_K; DESIGN.md section 4).
 
-The only constants read as data are oracle/afv_basis.inc and oracle/dither_table.inc, and the library's default
-dequantisation matrices (quant_weights.rs), taken from the front-end through jxo_t_dequant_table.
+The only constants read as data are oracle/afv_basis.inc, oracle/dither_table.inc and the parameter literals of the
+library's dequantisation matrices. The matrices themselves come from tests/f64_quant.py, the float64 restatement of
+quant_weights.rs: the library defaults, or the custom encodings a frame was written with (Frame(d, encodings=...)).
+Stage A's M carries the f32 rounding of the implementation's table (f64_quant.K_Q).
 """
 import ctypes as C
 import os
@@ -262,28 +264,30 @@ def _arr(ptr, ctype, shape):
     return np.ctypeslib.as_array(C.cast(ptr, C.POINTER(ctype)), shape).copy()
 
 
-def dequant_table(t):
-    """(3, 64*cx*cy) library default matrix of transform type t (quant_weights.rs), from the front-end."""
-    from tests import oracle_binding as ob
-    lib = ob.load()
-    lib.jxo_t_dequant_table.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_size_t]
-    lib.jxo_t_dequant_table.restype = C.c_uint32
-    n = 64 * COV_X[t] * COV_Y[t]
-    out = np.zeros((3, n), np.float32)
-    for c in range(3):
-        assert lib.jxo_t_dequant_table(t, c, out[c].ctypes.data, n) == n
-    return out.astype(np.float64)
+def dequant_table(t, encodings=None):
+    """(3, 64*cx*cy) dequantisation matrix of transform type t and its magnitude (f64_quant.table_for_transform)."""
+    from tests import f64_quant as fq
+    return fq.table_for_transform(t, encodings)
 
 
 class Frame:
-    """The fields of a JxgFrameDesc the float path reads, as numpy arrays (edited by the sensitivity tests)."""
+    """The fields of a JxgFrameDesc the float path reads, as numpy arrays (edited by the sensitivity tests).
+    encodings: the 17 dequantisation encodings the frame was written with (None: library table), required when the
+    descriptor carries custom tables, so that stage A never takes its matrices from the code under test."""
 
-    def __init__(self, d):
+    def __init__(self, d, encodings=None):
         self.width, self.height = int(d.width), int(d.height)
         self.xb, self.yb = (self.width + 7) // 8, (self.height + 7) // 8
         xb, yb = self.xb, self.yb
-        if any(d.dequant_tables[i] for i in range(17)):
-            raise NotImplementedError("custom dequantisation matrices")
+        custom = [bool(d.dequant_tables[i]) for i in range(17)]
+        if encodings is None and any(custom):
+            raise ValueError("the frame has custom dequantisation matrices: pass the encodings it was written with")
+        if encodings is not None:
+            assert len(encodings) == 17
+            want = [e is not None for e in encodings]
+            if want != custom:
+                raise ValueError(f"custom tables {custom} in the frame, encodings given for {want}")
+        self.encodings = encodings
         self.global_scale, self.x_qm_scale, self.b_qm_scale = int(d.global_scale), int(d.x_qm_scale), int(d.b_qm_scale)
         self.quant_biases = np.array(list(d.quant_biases), np.float64)
         self.base_x, self.base_b, self.color_factor = float(d.base_correlation_x), float(d.base_correlation_b), int(d.color_factor)
@@ -312,8 +316,9 @@ class Frame:
         self.dequant = {}
 
     def matrix(self, t):
+        """(table, M) of transform type t; sensitivity tests may plant their own in self.dequant."""
         if t not in self.dequant:
-            self.dequant[t] = dequant_table(t)
+            self.dequant[t] = dequant_table(t, self.encodings)
         return self.dequant[t]
 
 
@@ -344,6 +349,7 @@ def cfl_tile(b):
 
 def stage_a(fr, coeffs):
     """coeffs: [groups][3][65536] i32. Returns (planes, M), each [3][yb*8][xb*8] float64."""
+    from tests import f64_quant as fq
     planes = np.zeros((3, fr.yb * 8, fr.xb * 8))
     mag = np.zeros_like(planes)
     g, bx, by, ts, off = varblocks(fr)
@@ -365,9 +371,10 @@ def stage_a(fr, coeffs):
         rq = fr.raw_quant[bys, bxs].astype(np.float64)
         sy = inv_gs / rq  # dequant_block (group.rs:153-156)
         scale = np.stack([sy * x_dm, sy, sy * b_dm])[:, :, None]
-        mat = fr.matrix(t)[:, None, :]
-        d = adj * mat * scale
-        md = np.abs(d)
+        mat, mmat = fr.matrix(t)
+        d = adj * mat[:, None, :] * scale
+        # |d| for the rounding of d, plus the table's own f32 error, K_q 2^-24 M_table, in units of K_A 2^-24
+        md = np.abs(d) * (1.0 + fq.K_Q / BOUND_K["A"] * (mmat / mat)[:, None, :])
         ty, tx = cfl_tile(bys), cfl_tile(bxs)
         x_cc = (fr.base_x + fr.ytox[ty, tx] / fr.color_factor)[:, None]  # color_correlation_map.rs:76-88
         b_cc = (fr.base_b + fr.ytob[ty, tx] / fr.color_factor)[:, None]

@@ -159,7 +159,7 @@ def test_fault_transposed_dequant_matrix():
     data = _synthetic((300, 280, 9, 1.0, 2, 1, 1, 0, 0))
     fr = _frame(data)
     assert (fr.transform_map == 128 | 6).any()
-    fr.dequant[6] = fp.dequant_table(6).reshape(3, 8, 16).transpose(0, 2, 1).reshape(3, 128)
+    fr.dequant[6] = tuple(m.reshape(3, 8, 16).transpose(0, 2, 1).reshape(3, 128) for m in fp.dequant_table(6))
     _stage_a_fails(data, fr)
 
 
