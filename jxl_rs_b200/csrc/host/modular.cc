@@ -297,6 +297,37 @@ GroupHeader GroupHeader::read(BitReader& br) {
   return g;
 }
 
+// tree.rs:39-155 (validate_tree): every split must divide the range its ancestors leave for its property
+// (left child: property > val, right child: property <= val), and no node may lie deeper than 2048. Depth first with
+// the ranges of the current root-to-node path only; each frame restores the range its parent narrowed.
+static void validate_tree(const std::vector<TreeNode>& nodes, uint32_t num_properties) {
+  constexpr uint32_t kHeightLimit = 2048;
+  std::vector<std::pair<int32_t, int32_t>> range(num_properties, {INT32_MIN, INT32_MAX});
+  struct Frame {
+    uint32_t node, depth, stage;  // stage 0: enter, 1: left child done, 2: both done
+    int32_t restore_prop;         // < 0: nothing to restore (root)
+    std::pair<int32_t, int32_t> restore;
+  };
+  std::vector<Frame> stack{Frame{0, 0, 0, -1, {0, 0}}};
+  while (!stack.empty()) {
+    Frame f = stack.back();
+    stack.pop_back();
+    if (f.depth > kHeightLimit) fail("MA tree too tall");
+    const TreeNode& n = nodes[f.node];
+    if (n.property < 0 || f.stage == 2) {
+      if (f.restore_prop >= 0) range[size_t(f.restore_prop)] = f.restore;
+      continue;
+    }
+    const size_t p = size_t(n.property);
+    const auto [lo, hi] = range[p];
+    if (lo > n.val || hi <= n.val) fail("MA tree split on an empty range");
+    f.stage++;
+    stack.push_back(f);
+    stack.push_back(Frame{f.stage == 1 ? n.left : n.right, f.depth + 1, 0, n.property, range[p]});
+    range[p] = f.stage == 1 ? std::pair<int32_t, int32_t>{n.val + 1, hi} : std::pair<int32_t, int32_t>{lo, n.val};
+  }
+}
+
 ModularTree ModularTree::read(BitReader& br, size_t size_limit) {
   // tree.rs:284-358; contexts: 0 splitval, 1 property, 2 predictor, 3 offset, 4 mul_log, 5 mul_bits
   ModularTree t;
@@ -333,6 +364,7 @@ ModularTree ModularTree::read(BitReader& br, size_t size_limit) {
   }
   r.check_final_state(br);
   t.num_properties = max_property + 1;
+  validate_tree(t.nodes, t.num_properties);
   t.code = EntropyCode::decode((t.nodes.size() + 1) / 2, br, true);
   return t;
 }

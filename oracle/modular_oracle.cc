@@ -78,6 +78,80 @@ int jxo_modular_orientation(const uint8_t* data, size_t size) {
   }
 }
 
+// What the trees and headers of a Modular file use, as one JSON object (test report of the features a file reaches):
+// predictors and split properties of every tree (global and HF-group local), leaves with an offset / a multiplier,
+// global and local transforms, non-default WeightedHeaders, local trees, prefix / LZ77 codes, geometry.
+// Returns the length of the text (written when it fits in cap), or a negative error code.
+int64_t jxo_modular_features(const uint8_t* data, size_t size, char* out, size_t cap) {
+  try {
+    auto ms = jxg::parse_modular_file(data, size);
+    std::vector<int> preds(14, 0), props(256, 0);
+    size_t offset_leaves = 0, mul_leaves = 0, local_trees = 0, custom_wp = 0, local_tr = 0;
+    bool prefix = false, lz77 = false;
+    auto scan = [&](const jxg::ModularTree& t) {
+      for (const jxg::TreeNode& n : t.nodes) {
+        if (n.property >= 0) {
+          props[size_t(n.property)] = 1;
+        } else {
+          preds[n.left] = 1;
+          offset_leaves += n.val != 0;
+          mul_leaves += n.right != 1;
+        }
+      }
+      prefix |= t.code.use_prefix;
+      lz77 |= t.code.lz77_enabled;
+    };
+    auto is_default_wp = [](const jxg::WeightedHeader& w) {
+      const jxg::WeightedHeader d;
+      return std::memcmp(&w, &d, sizeof(d)) == 0;
+    };
+    auto transforms = [](const jxg::GroupHeader& g) {
+      std::string s;
+      for (const jxg::ModularTransform& t : g.transforms) {
+        if (!s.empty()) s += ",";
+        if (t.id == 0) s += "\"rct" + std::to_string(t.rct_type) + "\"";
+        else if (t.id == 1)
+          s += "\"palette(c=" + std::to_string(t.num_channels) + ",colors=" + std::to_string(t.num_colors) +
+               ",deltas=" + std::to_string(t.num_deltas) + ",pred=" + std::to_string(t.predictor_id) + ")\"";
+        else s += "\"squeeze(" + std::to_string(t.squeezes.size()) + " steps)\"";
+      }
+      return "[" + s + "]";
+    };
+    if (ms->has_global_tree) scan(ms->global_tree);
+    custom_wp += !is_default_wp(ms->global_header.wp);
+    for (const jxg::ModularGroupStream& st : ms->hf) {
+      if (st.empty) continue;
+      if (st.local_tree) {
+        local_trees++;
+        scan(*st.local_tree);
+      }
+      custom_wp += !is_default_wp(st.header.wp);
+      local_tr += st.header.transforms.size();
+    }
+    auto list = [](const std::vector<int>& v) {
+      std::string s;
+      for (size_t i = 0; i < v.size(); i++)
+        if (v[i]) s += (s.empty() ? "" : ",") + std::to_string(i);
+      return "[" + s + "]";
+    };
+    const std::string j = "{\"predictors\":" + list(preds) + ",\"split_properties\":" + list(props) +
+                          ",\"offset_leaves\":" + std::to_string(offset_leaves) + ",\"multiplier_leaves\":" +
+                          std::to_string(mul_leaves) + ",\"global_transforms\":" + transforms(ms->global_header) +
+                          ",\"local_transforms\":" + std::to_string(local_tr) + ",\"custom_wp_headers\":" +
+                          std::to_string(custom_wp) + ",\"local_trees\":" + std::to_string(local_trees) +
+                          ",\"prefix\":" + (prefix ? "true" : "false") + ",\"lz77\":" + (lz77 ? "true" : "false") +
+                          ",\"group_dim\":" + std::to_string(ms->header.group_dim()) + ",\"groups\":" +
+                          std::to_string(ms->header.num_groups()) + ",\"grey\":" +
+                          (ms->num_color_channels == 1 ? "true" : "false") + ",\"orientation\":" +
+                          std::to_string(ms->file.orientation) + "}";
+    if (j.size() < cap) std::memcpy(out, j.c_str(), j.size() + 1);
+    return int64_t(j.size());
+  } catch (jxg::Error& e) {
+    g_jxo_modular_error = e.what();
+    return e.code;
+  }
+}
+
 // out: interleaved RGB u8 (grey is replicated); planes (optional): 3 full-size i32 planes before the u8 conversion.
 int jxo_decode_modular_file(const uint8_t* data, size_t size, uint8_t* out, size_t out_row_stride, int32_t* planes) {
   try {

@@ -32,6 +32,8 @@ def _lib():
         _LIB.jxs_encode_modular_ex.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                C.c_void_p, C.c_void_p, C.c_size_t]
         _LIB.jxs_modular_last_error.restype = C.c_char_p
+        _LIB.jxs_encode_modular_tokens.restype = C.c_int64
+        _LIB.jxs_encode_modular_tokens.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
     return _LIB
 
 
@@ -154,4 +156,75 @@ def encode_modular(width, height, seed, rct=6, squeeze=0, tree_kind=1, source=No
     if n > cap:
         buf = C.create_string_buffer(n)
         n = lib.jxs_encode_modular_ex(width, height, seed, rct, squeeze, tree_kind, palette, src, buf, n)
+    return buf.raw[:n]
+
+
+def _tree_words(tree):
+    """A tree in BFS order: ("split", property, value) or ("leaf", predictor, offset, mul_log, mul_bits)."""
+    words = [len(tree)]
+    for n in tree:
+        if n[0] == "split":
+            words += [n[1] + 1, n[2], 0, 0, 0]
+        else:
+            words += [0, n[1], n[2], n[3], n[4]]
+    return words
+
+
+def _transform_words(transforms):
+    words = [len(transforms)]
+    for t in transforms:
+        words.append(t["id"])
+        if t["id"] == 0:
+            words += [t["begin"], t["rct_type"]]
+        elif t["id"] == 1:
+            words += [t["begin"], t["num_c"], t["num_colors"], t["num_deltas"], t["predictor"]]
+        else:
+            words.append(len(t["squeezes"]))
+            for sq in t["squeezes"]:
+                words += [int(sq[0]), int(sq[1]), sq[2], sq[3]]
+    return words
+
+
+def encode_modular_tokens(spec) -> bytes:
+    """One Modular frame written exactly as described; the writer predicts nothing and checks nothing (frames a decoder
+    must refuse can be written). `spec` is a dict:
+      width, height, group_shift (group size 128 << group_shift), grey, orientation (1..8), prefix (prefix codes
+      instead of ANS), hybrid (split_exponent, msb, lsb) of every symbol cluster;
+      tree: the global MA tree in BFS order, nodes ("split", property, value) / ("leaf", predictor, offset, mul_log,
+      mul_bits); its leaf ids (BFS order) are the symbol contexts;
+      sections: one per stream in TOC order without HfGlobal (global, then LF groups, then HF groups), each None (no
+      bytes) or a dict with use_global_tree, wp (None: all_default, else the 11 fields p1c p2c p3ca..p3ce w0..w3),
+      transforms (for the global section: the frame's global transforms) as dicts {"id": 0, "begin", "rct_type"},
+      {"id": 1, "begin", "num_c", "num_colors", "num_deltas", "predictor"}, {"id": 2, "squeezes": [(horizontal,
+      in_place, begin, num_c), ...]}, and tokens: None (the group header only) or a list of (context, u32 value);
+      with tokens, "tree" is the local tree when use_global_tree is false."""
+    words = [spec["width"], spec["height"], spec.get("group_shift", 1), int(spec.get("grey", 0)),
+             spec.get("orientation", 1), int(spec.get("prefix", 0))] + list(spec.get("hybrid", (4, 2, 0)))
+    words += _tree_words(spec["tree"])
+    words.append(len(spec["sections"]))
+    for s in spec["sections"]:
+        if s is None:
+            words.append(0)
+            continue
+        words.append(1 if s.get("tokens") is None else 2)
+        words.append(int(s.get("use_global_tree", True)))
+        wp = s.get("wp")
+        words += [1] + [0] * 11 if wp is None else [0] + list(wp)
+        words += _transform_words(s.get("transforms", []))
+        if s.get("tokens") is not None:
+            words += _tree_words(s.get("tree", []) if not s.get("use_global_tree", True) else [])
+            toks = s["tokens"]
+            words.append(len(toks))
+            for c, v in toks:
+                words += [c, v]
+    lib = _lib()
+    arr = (C.c_uint32 * len(words))(*[int(w) & 0xFFFFFFFF for w in words])
+    cap = max(1 << 16, 8 * len(words))
+    buf = C.create_string_buffer(cap)
+    n = lib.jxs_encode_modular_tokens(arr, len(words), buf, cap)
+    if n < 0:
+        raise RuntimeError("token-level Modular encode failed: " + lib.jxs_modular_last_error().decode())
+    if n > cap:
+        buf = C.create_string_buffer(n)
+        n = lib.jxs_encode_modular_tokens(arr, len(words), buf, n)
     return buf.raw[:n]

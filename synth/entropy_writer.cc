@@ -421,13 +421,15 @@ static AnsCode build_code_syms(size_t num_contexts, const std::vector<uint8_t>& 
                                const std::vector<const std::vector<Sym>*>& streams, uint32_t min_log_alpha, bool use_prefix);
 
 AnsCode build_code(size_t num_contexts, const std::vector<uint8_t>& cluster_of_ctx, uint32_t num_clusters,
-                   const std::vector<const std::vector<Token>*>& streams, uint32_t min_log_alpha, bool use_prefix) {
-  HybridCfg cfg;
+                   const std::vector<const std::vector<Token>*>& streams, uint32_t min_log_alpha, bool use_prefix,
+                   const HybridCfg& cfg) {
   std::vector<std::vector<Sym>> syms;
   for (auto* s : streams) syms.push_back(plain_symbols(*s, cfg));
   std::vector<const std::vector<Sym>*> ptrs;
   for (auto& v : syms) ptrs.push_back(&v);
-  return build_code_syms(num_contexts, cluster_of_ctx, num_clusters, ptrs, min_log_alpha, use_prefix);
+  AnsCode code = build_code_syms(num_contexts, cluster_of_ctx, num_clusters, ptrs, min_log_alpha, use_prefix);
+  code.cfg = cfg;
+  return code;
 }
 
 AnsCode build_code_lz77(size_t num_contexts, const std::vector<uint8_t>& cluster_of_ctx, uint32_t num_clusters,

@@ -134,9 +134,11 @@ struct AnsCode {
 
 // Normalises counts to sum 4096 with every used symbol >= 1.
 std::vector<uint16_t> normalize_counts(const std::vector<uint64_t>& counts, size_t alphabet);
-// Builds a code from tokens: `cluster_of_ctx` (size num_contexts, values < num_clusters) given by the caller.
+// Builds a code from tokens: `cluster_of_ctx` (size num_contexts, values < num_clusters) given by the caller; every
+// cluster uses the hybrid-uint configuration `cfg`.
 AnsCode build_code(size_t num_contexts, const std::vector<uint8_t>& cluster_of_ctx, uint32_t num_clusters,
-                   const std::vector<const std::vector<Token>*>& streams, uint32_t min_log_alpha = 5, bool use_prefix = false);
+                   const std::vector<const std::vector<Token>*>& streams, uint32_t min_log_alpha = 5, bool use_prefix = false,
+                   const HybridCfg& cfg = HybridCfg());
 // Convenience: one cluster per context when num_contexts <= 8, else quantile clustering into <= max_clusters.
 std::vector<uint8_t> cluster_contexts(size_t num_contexts, const std::vector<const std::vector<Token>*>& streams,
                                       uint32_t max_clusters, uint32_t& num_clusters, const HybridCfg& cfg);

@@ -590,6 +590,290 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
   return bytes;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Token-level Modular writer: serialises a frame whose trees, transforms, group headers and symbols were all chosen by
+// the caller (tests/modular_ref.py decodes forward and records what a decoder must read). It predicts nothing and
+// validates nothing, so frames a decoder must refuse can be written too. Flat u32 description, in this order:
+//   width, height, group_size_shift (0..3), grey, orientation (1..8), prefix codes, hybrid-uint split_exponent, msb,
+//   lsb, the global tree, the number of sections (1 + LF groups + HF groups, in TOC order without HfGlobal), then
+//   per section: kind (0: no bytes, 1: group header only, 2: group header + local tree + symbols), and for kind > 0:
+//   use_global_tree, WeightedHeader default flag and its 11 fields (p1c p2c p3ca..p3ce w0..w3), the transforms, then
+//   for kind 2: the local tree (empty when use_global_tree) and the symbols as count, (context, value) pairs.
+// A tree is its node count followed by 5 words per node in BFS order: a split is {property + 1, split value, 0, 0, 0},
+// a leaf {0, predictor, offset, mul_log, mul_bits}. Transforms are a count, then per transform its id followed by
+// RCT: begin, type; palette: begin, num_c, num_colors, num_deltas, predictor; Squeeze: count, then per step
+// horizontal, in_place, begin, num_c.
+namespace {
+
+struct WordReader {
+  const uint32_t* w;
+  size_t n, i = 0;
+  uint32_t next() {
+    if (i >= n) throw std::runtime_error("token description ends early");
+    return w[i++];
+  }
+};
+
+struct TokTree {
+  std::vector<uint32_t> words;  // 5 per node
+  size_t leaves = 0;
+};
+
+TokTree read_tok_tree(WordReader& r) {
+  TokTree t;
+  const uint32_t n = r.next();
+  for (uint32_t i = 0; i < 5 * n; i++) t.words.push_back(r.next());
+  for (uint32_t i = 0; i < n; i++) t.leaves += t.words[5 * i] == 0;
+  return t;
+}
+
+// u2S field (headers/encodings.rs:76-98) with the four (bits, offset) distributions: the first one that holds v.
+void write_u2s(BitWriter& bw, uint32_t v, const uint32_t (&d)[4][2]) {
+  for (uint32_t s = 0; s < 4; s++) {
+    const uint32_t bits = d[s][0], off = d[s][1];
+    if (v < off) continue;
+    if (bits == 0 ? v == off : uint64_t(v - off) < (uint64_t(1) << bits)) {
+      bw.u2s_sel(s, v - off, bits);
+      return;
+    }
+  }
+  throw std::runtime_error("value not representable in its u2S field");
+}
+
+void copy_transforms(WordReader& r, BitWriter& bw) {  // GroupHeader transforms (headers/modular.rs:62-140)
+  static const uint32_t kBegin[4][2] = {{3, 0}, {6, 8}, {10, 72}, {13, 1096}};
+  const uint32_t nt = r.next();
+  write_u2s(bw, nt, {{0, 0}, {0, 1}, {4, 2}, {8, 18}});
+  for (uint32_t i = 0; i < nt; i++) {
+    const uint32_t id = r.next();
+    bw.write(id, 2);
+    if (id == 0) {
+      write_u2s(bw, r.next(), kBegin);
+      write_u2s(bw, r.next(), {{0, 6}, {2, 0}, {4, 2}, {6, 10}});
+    } else if (id == 1) {
+      write_u2s(bw, r.next(), kBegin);
+      write_u2s(bw, r.next(), {{0, 1}, {0, 3}, {0, 4}, {13, 1}});
+      write_u2s(bw, r.next(), {{8, 0}, {10, 256}, {12, 1280}, {16, 5376}});
+      write_u2s(bw, r.next(), {{0, 0}, {8, 1}, {10, 257}, {16, 1281}});
+      bw.write(r.next(), 4);
+    } else if (id == 2) {
+      const uint32_t ns = r.next();
+      write_u2s(bw, ns, {{0, 0}, {4, 1}, {6, 9}, {8, 41}});
+      for (uint32_t s = 0; s < ns; s++) {
+        bw.write(r.next(), 1);
+        bw.write(r.next(), 1);
+        write_u2s(bw, r.next(), kBegin);
+        write_u2s(bw, r.next(), {{0, 1}, {0, 2}, {0, 3}, {4, 4}});
+      }
+    } else {
+      throw std::runtime_error("transform id must be 0, 1 or 2");
+    }
+  }
+}
+
+// Tree symbols (tree.rs:284-351) under their own six-context code, then nothing else: the caller writes the code of
+// the tree's leaves.
+void write_tok_tree(BitWriter& bw, const TokTree& t) {
+  std::vector<Token> tt;
+  for (size_t i = 0; i < t.words.size(); i += 5) {
+    const uint32_t* n = &t.words[i];
+    tt.push_back(Token{1, n[0]});
+    if (n[0]) {
+      tt.push_back(Token{0, pack_signed(int32_t(n[1]))});
+    } else {
+      tt.push_back(Token{2, n[1]});
+      tt.push_back(Token{3, pack_signed(int32_t(n[2]))});
+      tt.push_back(Token{4, n[3]});
+      tt.push_back(Token{5, n[4]});
+    }
+  }
+  uint32_t tnc;
+  HybridCfg tcfg;
+  std::vector<uint8_t> tmap = cluster_contexts(6, {&tt}, 8, tnc, tcfg);
+  AnsCode tcode = build_code(6, tmap, tnc, {&tt});
+  write_code(bw, tcode);
+  write_tokens(bw, tcode, tt);
+}
+
+// One cluster per leaf (up to 255 leaves), so that a decoder which takes another leaf reads another histogram.
+AnsCode leaf_code(size_t leaves, const std::vector<const std::vector<Token>*>& streams, bool prefix, const HybridCfg& cfg) {
+  const size_t nctx = std::max<size_t>(leaves, 1);
+  uint32_t nc = 0;
+  std::vector<uint8_t> cmap;
+  if (nctx <= 255) {
+    for (size_t i = 0; i < nctx; i++) cmap.push_back(uint8_t(i));
+    nc = uint32_t(nctx);
+  } else {
+    cmap = cluster_contexts(nctx, streams, 16, nc, cfg);
+  }
+  for (auto* s : streams)
+    for (const Token& t : *s)
+      if (t.ctx >= nctx) throw std::runtime_error("symbol context beyond the tree's leaves");
+  return build_code(nctx, cmap, nc, streams, 5, prefix, cfg);
+}
+
+}  // namespace
+
+std::vector<uint8_t> encode_modular_tokens(const uint32_t* words, size_t nwords) {
+  WordReader r{words, nwords};
+  const uint32_t W = r.next(), H = r.next(), gshift = r.next(), grey = r.next(), orientation = r.next();
+  const bool prefix = r.next() != 0;
+  HybridCfg cfg;
+  cfg.split_exponent = r.next();
+  cfg.msb = r.next();
+  cfg.lsb = r.next();
+  if (gshift > 3 || orientation < 1 || orientation > 8 || !W || !H) throw std::runtime_error("bad frame geometry");
+  const TokTree global = read_tok_tree(r);
+  struct Section {
+    uint32_t kind = 0;
+    BitWriter header;  // group header (+ local tree when not using the global one) is written once the codes exist
+    TokTree local;
+    bool use_global = true;
+    std::vector<Token> toks;
+  };
+  const uint32_t nsec = r.next();
+  std::vector<Section> secs(nsec);
+  for (Section& s : secs) {
+    s.kind = r.next();
+    if (s.kind == 0) continue;
+    s.use_global = r.next() != 0;
+    s.header.write(s.use_global, 1);
+    const uint32_t wp_default = r.next();
+    uint32_t wp[11];
+    for (uint32_t& v : wp) v = r.next();
+    s.header.write(wp_default, 1);
+    if (!wp_default) {
+      for (int i = 0; i < 7; i++) s.header.write(wp[i], 5);
+      for (int i = 7; i < 11; i++) s.header.write(wp[i], 4);
+    }
+    copy_transforms(r, s.header);
+    if (s.kind < 2) continue;
+    s.local = read_tok_tree(r);
+    const uint32_t nt = r.next();
+    for (uint32_t i = 0; i < nt; i++) {
+      const uint32_t ctx = r.next();
+      s.toks.push_back(Token{ctx, r.next()});
+    }
+  }
+  if (r.i != r.n) throw std::runtime_error("token description has trailing words");
+
+  // the global code covers every section that uses the global tree
+  std::vector<const std::vector<Token>*> gstreams;
+  for (const Section& s : secs)
+    if (s.kind == 2 && s.use_global) gstreams.push_back(&s.toks);
+  const AnsCode gcode = leaf_code(global.leaves, gstreams, prefix, cfg);
+  auto section_bits = [&](Section& s, BitWriter& out) {
+    if (s.kind == 0) return;
+    append_bits(out, s.header);
+    if (s.kind < 2) return;
+    if (s.use_global) {
+      write_tokens(out, gcode, s.toks);
+    } else {
+      write_tok_tree(out, s.local);
+      const AnsCode lcode = leaf_code(s.local.leaves, {&s.toks}, prefix, cfg);
+      write_code(out, lcode);
+      write_tokens(out, lcode, s.toks);
+    }
+  };
+
+  const uint32_t group_dim = 128u << gshift;
+  const uint32_t xg = (W + group_dim - 1) / group_dim, yg = (H + group_dim - 1) / group_dim, num_groups = xg * yg;
+  const uint32_t lf_dim = group_dim * 8;
+  const uint32_t num_lf_groups = ((W + lf_dim - 1) / lf_dim) * ((H + lf_dim - 1) / lf_dim);
+  if (nsec != 1 + num_lf_groups + num_groups) throw std::runtime_error("section count does not match the geometry");
+
+  BitWriter lf_global;
+  lf_global.write(1, 1);  // LfQuantFactors all_default
+  lf_global.write(1, 1);  // global tree present
+  write_tok_tree(lf_global, global);
+  write_code(lf_global, gcode);
+  section_bits(secs[0], lf_global);
+  std::vector<BitWriter> groups(nsec - 1);
+  for (uint32_t i = 1; i < nsec; i++) section_bits(secs[i], groups[i - 1]);
+
+  BitWriter out;
+  out.write(0xff, 8);
+  out.write(0x0a, 8);
+  auto write_dim = [&](uint32_t v) {
+    uint32_t m = v - 1;
+    if (m < (1u << 9)) out.u2s_sel(0, m, 9);
+    else if (m < (1u << 13)) out.u2s_sel(1, m, 13);
+    else if (m < (1u << 18)) out.u2s_sel(2, m, 18);
+    else out.u2s_sel(3, m, 30);
+  };
+  out.write(0, 1);  // small = false
+  write_dim(H);
+  out.write(0, 3);  // ratio 0
+  write_dim(W);
+  // ImageMetadata (image_metadata.rs:197-236)
+  out.write(0, 1);                // all_default
+  out.write(1, 1);                // extra_fields
+  out.write(orientation - 1, 3);
+  out.write(0, 1);                // have_intrinsic_size
+  out.write(0, 1);                // have_preview
+  out.write(0, 1);                // have_animation
+  out.write(0, 1);                // bit depth: integer samples
+  out.u2s_sel(0);                 //            8 bits
+  out.write(1, 1);                // modular_16bit_buffers
+  out.u2s_sel(0);                 // no extra channels
+  out.write(0, 1);                // xyb_encoded = false
+  if (!grey) {
+    out.write(1, 1);              // ColorEncoding all_default (sRGB)
+  } else {                        // color_encoding.rs:166-196: grey, D65, sRGB curve, relative intent
+    out.write(0, 1);
+    out.write(0, 1);              // want_icc
+    out.u2s_sel(1);               // colour space Gray
+    out.u2s_sel(1);               // white point D65
+    out.write(0, 1);              // have_gamma
+    out.u2s_sel(2, 13 - 2, 4);    // transfer function sRGB (13)
+    out.u2s_sel(1);               // rendering intent relative
+  }
+  out.write(1, 1);                // ToneMapping all_default
+  out.write_u64(0);               // extensions
+  out.write(1, 1);                // CustomTransformData all_default
+  out.zero_pad_to_byte();
+  // FrameHeader (frame_header.rs:267-444)
+  out.write(0, 1);   // all_default
+  out.write(0, 2);   // RegularFrame
+  out.write(1, 1);   // Modular
+  out.write_u64(0);  // flags
+  out.write(0, 1);   // do_ycbcr
+  out.write(0, 2);   // upsampling 1
+  out.write(gshift, 2);
+  out.write(0, 2);   // one pass
+  out.write(0, 1);   // have_crop
+  out.write(0, 2);   // blending Replace
+  out.write(1, 1);   // is_last
+  out.write(0, 2);   // name length 0
+  out.write(0, 1);   // RestorationFilter all_default = 0
+  out.write(0, 1);   // gab off
+  out.write(0, 2);   // epf off
+  out.write_u64(0);  // restoration filter extensions
+  out.write_u64(0);  // frame header extensions
+  std::vector<std::vector<uint8_t>> sections;
+  BitWriter hf_global;  // empty for Modular frames
+  if (num_groups == 1) {
+    BitWriter all_bits;
+    append_bits(all_bits, lf_global);
+    append_bits(all_bits, groups[0]);
+    append_bits(all_bits, hf_global);
+    append_bits(all_bits, groups[1]);
+    sections.push_back(all_bits.finish());
+  } else {
+    sections.push_back(lf_global.finish());
+    for (uint32_t g = 0; g < num_lf_groups; g++) sections.push_back(groups[g].finish());
+    sections.push_back(hf_global.finish());
+    for (uint32_t g = 0; g < num_groups; g++) sections.push_back(groups[num_lf_groups + g].finish());
+  }
+  out.write(0, 1);  // TOC not permuted
+  out.zero_pad_to_byte();
+  for (auto& s : sections) write_toc_entry(out, uint32_t(s.size()));
+  out.zero_pad_to_byte();
+  std::vector<uint8_t> bytes = out.finish();
+  for (auto& s : sections) bytes.insert(bytes.end(), s.begin(), s.end());
+  return bytes;
+}
+
 }  // namespace jxs
 
 extern "C" {
@@ -643,6 +927,18 @@ int64_t jxs_encode_modular_ex(uint32_t width, uint32_t height, uint64_t seed, ui
                               uint32_t tree_kind, uint32_t palette, const uint8_t* source_rgb, uint8_t* out, size_t cap) {
   try {
     std::vector<uint8_t> b = jxs::encode_modular(width, height, seed, rct, squeeze, tree_kind, source_rgb, palette);
+    if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
+    return int64_t(b.size());
+  } catch (std::exception& e) {
+    g_merr = e.what();
+    return -1;
+  }
+}
+
+// The token-level writer (encode_modular_tokens above): `words` is the flat frame description.
+int64_t jxs_encode_modular_tokens(const uint32_t* words, size_t nwords, uint8_t* out, size_t cap) {
+  try {
+    std::vector<uint8_t> b = jxs::encode_modular_tokens(words, nwords);
     if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
     return int64_t(b.size());
   } catch (std::exception& e) {
