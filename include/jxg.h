@@ -190,7 +190,9 @@ int jxg_batch_rerun_device(void* batch, void* cuda_stream);
 void jxg_batch_end(void* batch);
 
 /* Parity taps: copy intermediate planes of frame `f` of a finished batch to
- * host. coeffs: 3 planes of i32, dense per group in decode order (group.rs:53). */
+ * host. coeffs: 3 planes of i32, dense per group in decode order (group.rs:53).
+ * xyb: the 3 padded XYB planes (f32) after dequant + IDCT; `stage` must be 0
+ * (JXG_ERR_ARGUMENT otherwise). Meaningful after a run stopped with debug stop 2. */
 int jxg_batch_read_coeffs(void* batch, uint32_t f, int32_t* out, size_t out_len);
 int jxg_batch_read_xyb(void* batch, uint32_t f, int stage, float* out, size_t out_len);
 
@@ -201,7 +203,8 @@ int jxg_batch_read_xyb(void* batch, uint32_t f, int stage, float* out, size_t ou
 int jxg_batch_set_deferred_copy(void* batch, int threads);
 
 /* Debug/parity: 0 = run everything (default), 1 = stop after the entropy kernel,
- * 2 = stop after dequant+IDCT (planes readable with stage 0). */
+ * 2 = stop after dequant+IDCT (planes readable with jxg_batch_read_xyb stage 0).
+ * JXG_ERR_ARGUMENT for a NULL batch or any other stage. */
 int jxg_batch_set_debug_stop(void* batch, int stage);
 
 /* Per-stage device timing with CUDA events on the launching stream (bench.py roofline):

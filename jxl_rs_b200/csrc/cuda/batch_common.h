@@ -126,7 +126,9 @@ DeviceStreams device_streams(int device);  // created on first use
 struct Context {
   int device = 0;
   cudaStream_t stream = nullptr;
-  cudaStream_t copy_stream = nullptr;  // D2H of finished frame ranges overlaps the filtering of later ranges
+  // Output copies of a batch leave on the device's D2H stream (DeviceStreams::d2h) in up to kMaxRanges frame ranges: the
+  // copy of a finished range overlaps the filtering of the later ones.
+  cudaStream_t d2h = nullptr;
   static constexpr int kMaxRanges = 8;
   cudaEvent_t range_done[kMaxRanges] = {nullptr}, copy_done = nullptr;
   DevBuf dequant_default, dequant_default_off, natural_orders, natural_order_off;
@@ -134,8 +136,7 @@ struct Context {
   // intermediates and the pinned staging arena survive jxg_batch_end so that a
   // steady-state decode loop does no cudaMalloc / cudaHostAlloc.
   PinnedArena blob;
-  DevBuf d_blob, d_frames, d_sections, d_streams, d_streams_lean, d_lean_cta, d_streams_fast, d_streams_slow, d_nz_base, d_tiles, d_ftiles, d_coeffs, d_block_off, d_nz, d_planes_a,
-      d_planes_b, d_status, d_out, d_lean_desc, d_lean_nblk, d_orient, d_lean_warp, d_big, d_lzwin;
+  DevBuf d_blob, d_coeffs, d_block_off, d_nz, d_planes_a, d_status, d_out, d_lean_desc, d_lean_nblk, d_orient, d_lzwin;
   bool batch_live = false;
   // pinned status readback buffer, owned by the context: cudaHostAlloc / cudaFreeHost synchronise the whole
   // device, so they must not happen per batch when batches of several contexts are in flight

@@ -119,7 +119,6 @@ struct BatchDev {
   uint8_t* nz;          // [streams][passes][3][1024]
   uint64_t* nz_base;    // per stream offset into nz (bytes)
   float* planes_a;
-  float* planes_b;
   int32_t* status;      // per stream
   uint32_t* queue;      // [frames] work-queue cursors of the persistent entropy kernel
   const uint32_t* lean_cta_first;  // [frames] first CTA of each frame in k_entropy_lean's grid

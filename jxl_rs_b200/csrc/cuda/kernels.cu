@@ -1,14 +1,15 @@
-// sm_90a kernels of the VarDCT hot path (first correct version).
+// sm_90a kernels of the VarDCT hot path.
 //
-//   k_entropy   K1  one warp per (frame, group) stream: ANS / prefix decode of the
-//                   AC coefficients with the JPEG XL context model
-//                   (jxl/src/frame/group.rs:454-578, entropy_coding/*.rs)
-//   k_dequant_idct K2 one CTA per group: dequant + chroma-from-luma + LLF + inverse
-//                   variable-block DCT (group.rs:100-250, jxl_transforms/src/transform.rs)
-//   k_gaborish  K3  3x3 smoothing (render/stages/gaborish.rs)
-//   k_epf       K4  edge-preserving filter passes 0/1/2 (render/stages/epf/*.rs)
-//   k_xyb_store K5  XYB -> linear -> sRGB -> u8/f32 interleaved store
-//                   (render/stages/{xyb,from_linear,convert}.rs, color/tf.rs)
+//   k_block_plan     varblock descriptors of every (frame, group) stream
+//   k_entropy_lean   K1  decode of the AC coefficients with the JPEG XL context model (jxl/src/frame/group.rs:454-578,
+//   k_entropy_fast       entropy_coding/*.rs): persistent lanes for single-pass ANS frames (lean), prefix-coded
+//   k_entropy            frames (fast), multi-pass and LZ77 frames
+//   k_idct_small     K2  one CTA per group: dequant + chroma-from-luma + LLF + inverse variable-block DCT
+//   k_dequant_idct       (group.rs:100-250, jxl_transforms/src/transform.rs); small and large varblocks
+//   k_filters_store  K3-K5 fused Gaborish -> EPF 0/1/2 -> XYB -> output transfer curve -> store
+//                    (render/stages/{gaborish,epf/*,xyb,from_linear,convert}.rs, color/tf.rs)
+//   k_orient         orientation post-pass of frames with orientation != 1
+//   k_expand_coeffs  coefficient lists -> dense layout (jxg_batch_read_coeffs)
 //
 // No tensor cores: there is no dense contraction on this path; everything is
 // HBM / latency bound integer and f32 work.
@@ -2188,155 +2189,6 @@ __device__ __forceinline__ int mirror(int v, int s) {  // util/mirror.rs:8
   return v;
 }
 
-struct TileDev {  // 32x8-pixel tiles over all frames of the batch
-  const uint32_t* tile_prefix;  // [num_frames + 1]
-  uint32_t num_frames;
-};
-
-__device__ __forceinline__ bool locate_tile(const BatchDev& B, const TileDev& T, uint32_t tile, uint32_t& f, int& x, int& y) {
-  uint32_t lo = 0, hi = T.num_frames;
-  while (hi - lo > 1) {
-    uint32_t mid = (lo + hi) >> 1;
-    if (T.tile_prefix[mid] <= tile) lo = mid;
-    else hi = mid;
-  }
-  f = lo;
-  const FrameDev& F = B.frames[f];
-  uint32_t local = tile - T.tile_prefix[f];
-  uint32_t tiles_x = (F.width + 31) / 32;
-  x = int((local % tiles_x) * 32 + threadIdx.x);
-  y = int((local / tiles_x) * 8 + threadIdx.y);
-  return x < int(F.width) && y < int(F.height);
-}
-
-// gaborish.rs:40-88
-__global__ void __launch_bounds__(256) k_gaborish(const BatchDev B, const TileDev T, const float* src, float* dst) {
-  uint32_t f;
-  int x, y;
-  if (!locate_tile(B, T, blockIdx.x, f, x, y)) return;
-  const FrameDev& F = B.frames[f];
-  const int w = int(F.width), h = int(F.height);
-  const int xl = mirror(x - 1, w), xr = mirror(x + 1, w), yt = mirror(y - 1, h), yb = mirror(y + 1, h);
-  const size_t st = F.plane_stride;
-  if (!F.gab) {  // frame without Gaborish inside a mixed batch: pass through
-#pragma unroll
-    for (int c = 0; c < 3; c++) dst[F.plane_base + c * F.plane_size + y * st + x] = src[F.plane_base + c * F.plane_size + y * st + x];
-    return;
-  }
-#pragma unroll
-  for (int c = 0; c < 3; c++) {
-    const float* p = src + F.plane_base + c * F.plane_size;
-    const float *t = p + yt * st, *m = p + y * st, *b = p + yb * st;
-    float sum = m[x] * F.gab_k0[c];
-    sum = fmaf(F.gab_k1[c], t[x] + m[xl] + b[x] + m[xr], sum);
-    sum = fmaf(F.gab_k2[c], t[xl] + t[xr] + b[xl] + b[xr], sum);
-    dst[F.plane_base + c * F.plane_size + y * st + x] = sum;
-  }
-}
-
-// features/epf.rs:54-79
-__device__ __forceinline__ float inv_sigma_at(const BatchDev& B, const FrameDev& F, int x, int y) {
-  const size_t bidx = size_t(y >> 3) * F.xb + (x >> 3);
-  const int32_t raw_quant = reinterpret_cast<const int32_t*>(B.blob + F.raw_quant_off)[bidx];
-  const uint32_t sharp = (B.blob + F.epf_off)[bidx];
-  const float kInvSigmaNum = -1.1715728752538099024f;
-  float sigma_quant = F.epf_quant_mul / (F.quant_scale * float(raw_quant) * kInvSigmaNum);
-  float sigma = fminf(sigma_quant * F.epf_sharp_lut[sharp], -1e-4f);
-  return 1.0f / sigma;
-}
-
-// epf0.rs / epf1.rs / epf2.rs; STAGE selects the neighbourhood.
-template <int STAGE>
-__global__ void __launch_bounds__(256) k_epf(const BatchDev B, const TileDev T, const float* src, float* dst) {
-  uint32_t f;
-  int x, y;
-  if (!locate_tile(B, T, blockIdx.x, f, x, y)) return;
-  const FrameDev& F = B.frames[f];
-  const bool enabled = STAGE == 0 ? F.epf_iters >= 3 : (STAGE == 1 ? F.epf_iters >= 1 : F.epf_iters >= 2);
-  const int w = int(F.width), h = int(F.height);
-  const size_t st = F.plane_stride;
-  const float* p[3] = {src + F.plane_base, src + F.plane_base + F.plane_size, src + F.plane_base + 2 * F.plane_size};
-  float* q[3] = {dst + F.plane_base, dst + F.plane_base + F.plane_size, dst + F.plane_base + 2 * F.plane_size};
-  auto at = [&](int c, int xx, int yy) { return p[c][size_t(mirror(yy, h)) * st + mirror(xx, w)]; };
-  const float kMinSigma = -3.90524291751269967465540850526868f;
-  const float inv_sigma_px = inv_sigma_at(B, F, x, y);
-  const size_t o = size_t(y) * st + x;
-  if (!enabled || inv_sigma_px < kMinSigma) {
-#pragma unroll
-    for (int c = 0; c < 3; c++) q[c][o] = p[c][o];
-    return;
-  }
-  const float sigma_scale = STAGE == 0 ? F.epf_pass0_sigma_scale : (STAGE == 1 ? 1.0f : F.epf_pass2_sigma_scale);
-  const float sm = sigma_scale * 1.65f, bsm = sm * F.epf_border_sad_mul;
-  const bool border = ((y & 7) == 0 || (y & 7) == 7) || ((x & 7) == 0 || (x & 7) == 7);
-  const float inv_s = inv_sigma_px * (border ? bsm : sm);
-  if (STAGE == 2) {
-    const int off[4][2] = {{0, -1}, {-1, 0}, {1, 0}, {0, 1}};
-    float cc[3] = {p[0][o], p[1][o], p[2][o]};
-    float wacc = 1.0f, acc[3] = {cc[0], cc[1], cc[2]};
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-      float nb[3] = {at(0, x + off[k][0], y + off[k][1]), at(1, x + off[k][0], y + off[k][1]), at(2, x + off[k][0], y + off[k][1])};
-      float sad = fmaf(fabsf(nb[0] - cc[0]), F.epf_channel_scale[0],
-                       fmaf(fabsf(nb[1] - cc[1]), F.epf_channel_scale[1], fabsf(nb[2] - cc[2]) * F.epf_channel_scale[2]));
-      float wt = fmaxf(fmaf(sad, inv_s, 1.0f), 0.0f);
-      wacc += wt;
-#pragma unroll
-      for (int c = 0; c < 3; c++) acc[c] = fmaf(wt, nb[c], acc[c]);
-    }
-    float inv_w = 1.0f / wacc;
-#pragma unroll
-    for (int c = 0; c < 3; c++) q[c][o] = acc[c] * inv_w;
-    return;
-  }
-  constexpr int N = STAGE == 0 ? 12 : 4;
-  const int off0[12][2] = {{0, -2}, {-1, -1}, {0, -1}, {1, -1}, {-2, 0}, {-1, 0}, {1, 0}, {2, 0}, {-1, 1}, {0, 1}, {1, 1}, {0, 2}};
-  const int off1[4][2] = {{0, -1}, {-1, 0}, {1, 0}, {0, 1}};
-  const int plus[5][2] = {{0, -1}, {-1, 0}, {0, 0}, {1, 0}, {0, 1}};
-  float sads[N];
-#pragma unroll
-  for (int k = 0; k < N; k++) sads[k] = 0.0f;
-#pragma unroll
-  for (int c = 0; c < 3; c++) {
-    // window of radius 3 (stage 0) / 2 (stage 1) around the pixel
-    constexpr int RAD = STAGE == 0 ? 3 : 2;
-    float win[2 * RAD + 1][2 * RAD + 1];
-#pragma unroll
-    for (int dy = -RAD; dy <= RAD; dy++)
-#pragma unroll
-      for (int dx = -RAD; dx <= RAD; dx++) {
-        if (abs(dx) + abs(dy) <= RAD) win[dy + RAD][dx + RAD] = at(c, x + dx, y + dy);
-      }
-    const float scale = F.epf_channel_scale[c];
-#pragma unroll
-    for (int k = 0; k < N; k++) {
-      const int ox = STAGE == 0 ? off0[k][0] : off1[k][0], oy = STAGE == 0 ? off0[k][1] : off1[k][1];
-      float s = 0.0f;
-#pragma unroll
-      for (int j = 0; j < 5; j++)
-        s += fabsf(win[plus[j][1] + RAD][plus[j][0] + RAD] - win[plus[j][1] + oy + RAD][plus[j][0] + ox + RAD]);
-      sads[k] = fmaf(scale, s, sads[k]);
-    }
-  }
-  float wsum = 1.0f;
-#pragma unroll
-  for (int k = 0; k < N; k++) {
-    sads[k] = fmaxf(fmaf(sads[k], inv_s, 1.0f), 0.0f);
-    wsum += sads[k];
-  }
-  const float inv_w = 1.0f / wsum;
-#pragma unroll
-  for (int c = 0; c < 3; c++) {
-    float v = p[c][o];
-#pragma unroll
-    for (int k = N - 1; k >= 0; k--) {
-      const int ox = STAGE == 0 ? off0[k][0] : off1[k][0], oy = STAGE == 0 ? off0[k][1] : off1[k][1];
-      v = fmaf(at(c, x + ox, y + oy), sads[k], v);
-    }
-    q[c][o] = v * inv_w;
-  }
-}
-
 // color/tf.rs:13-44
 __device__ __forceinline__ float linear_to_srgb(float v) {
   const float P[5] = {-5.135152395e-4f, 5.287254571e-3f, 3.903842876e-1f, 1.474205315f, 7.352629620e-1f};
@@ -2431,7 +2283,6 @@ __device__ __noinline__ void from_linear_other(const FrameDev& F, float (&v)[3])
   }
 }
 
-// xyb.rs:197-241 + from_linear + convert.rs:574-598 + save (interleave)
 // 16-bit stores of one colour sample. U16: ConvertF32ToU16Stage (convert.rs:739-762: clamp to [0, 1], scale by
 // 2^16 - 1, round to nearest, ties to even like the AVX2 store). F16: ConvertF32ToF16Stage (convert.rs:831-857) with the
 // clamp range frame/render.rs:746-750 gives PQ and HLG outputs.
@@ -2449,67 +2300,6 @@ __device__ __forceinline__ uint16_t sample16(const FrameDev& F, float v) {
     return uint16_t(sign | (((mag & 0x007fffffu) | 0x00800000u) >> (uint32_t(-14 - unbiased) + 14)));
   }
   return __half_as_ushort(__float2half_rn(v));
-}
-
-__global__ void __launch_bounds__(256) k_xyb_store(const BatchDev B, const TileDev T, const float* src) {
-  uint32_t f;
-  int x, y;
-  if (!locate_tile(B, T, blockIdx.x, f, x, y)) return;
-  const FrameDev& F = B.frames[f];
-  const size_t o = size_t(y) * F.plane_stride + x;
-  float vx = src[F.plane_base + o], vy = src[F.plane_base + F.plane_size + o], vb = src[F.plane_base + 2 * F.plane_size + o];
-  uint8_t* row = static_cast<uint8_t*>(F.out_ptr) + size_t(y) * F.out_row_stride;
-  if (F.output_format == JXG_FORMAT_XYB_F32_PLANAR) {
-    uint8_t* base = static_cast<uint8_t*>(F.out_ptr);
-    reinterpret_cast<float*>(base + (size_t(0) * F.height + y) * F.out_row_stride)[x] = vx;
-    reinterpret_cast<float*>(base + (size_t(1) * F.height + y) * F.out_row_stride)[x] = vy;
-    reinterpret_cast<float*>(base + (size_t(2) * F.height + y) * F.out_row_stride)[x] = vb;
-    return;
-  }
-  float l = vy + vx - F.bias_cbrt[0], m = vy - vx - F.bias_cbrt[1], s = vb - F.bias_cbrt[2];
-  float l2 = l * l, m2 = m * m, s2 = s * s;
-  float sl = l * F.intensity_scale, sm = m * F.intensity_scale, ss = s * F.intensity_scale;
-  l = fmaf(l2, sl, F.scaled_bias[0]);
-  m = fmaf(m2, sm, F.scaled_bias[1]);
-  s = fmaf(s2, ss, F.scaled_bias[2]);
-  float v[3];
-  v[0] = fmaf(F.opsin[0], l, fmaf(F.opsin[1], m, F.opsin[2] * s));
-  v[1] = fmaf(F.opsin[3], l, fmaf(F.opsin[4], m, F.opsin[5] * s));
-  v[2] = fmaf(F.opsin[6], l, fmaf(F.opsin[7], m, F.opsin[8] * s));
-  if (F.output_tf == JXG_TF_SRGB) {
-#pragma unroll
-    for (int c = 0; c < 3; c++) v[c] = linear_to_srgb(v[c]);
-  } else if (F.output_tf != JXG_TF_LINEAR) {
-    from_linear_other(F, v);
-  }
-  if (F.output_format == JXG_FORMAT_RGB_F32) {
-    float* dst = reinterpret_cast<float*>(row) + size_t(x) * 3;
-    dst[0] = v[0];
-    dst[1] = v[1];
-    dst[2] = v[2];
-    return;
-  }
-  if (F.output_format == JXG_FORMAT_RGB_U16 || F.output_format == JXG_FORMAT_RGB_F16) {
-    uint16_t* dst = reinterpret_cast<uint16_t*>(row) + size_t(x) * 3;
-#pragma unroll
-    for (int c = 0; c < 3; c++) dst[c] = sample16(F, v[c]);
-    return;
-  }
-  uint8_t px[4];
-#pragma unroll
-  for (int c = 0; c < 3; c++) {
-    float d = c_dither[((y + 13 * c) & 31) * 32 + ((x + 23 * c) & 31)];
-    float sc = fminf(fmaxf(v[c] * 255.0f + d, 0.0f), 255.0f);
-    px[c] = uint8_t(__float2int_rn(sc));  // round-to-nearest-even, as the AVX store (jxl_simd avx.rs:609)
-  }
-  if (F.output_format == JXG_FORMAT_RGBA_U8) {
-    px[3] = 255;
-    reinterpret_cast<uchar4*>(row)[x] = make_uchar4(px[0], px[1], px[2], px[3]);
-  } else {
-    row[x * 3 + 0] = px[0];
-    row[x * 3 + 1] = px[1];
-    row[x * 3 + 2] = px[2];
-  }
 }
 
 // ===========================================================================
@@ -2532,7 +2322,6 @@ struct FusedTiles {
   uint32_t num_frames;
   uint32_t tile_begin;          // first tile of this launch (frame ranges are launched separately so that the
                                 // D2H copy of finished frames overlaps the filtering of the next ones)
-  uint32_t tile_end;            // one past the last tile of this launch (the persistent kernel strides up to it)
 };
 
 template <bool GAB, int EPF>
@@ -2899,52 +2688,32 @@ __device__ __forceinline__ void tile_sigma(const BatchDev& B, const FrameDev& F,
   }
 }
 
-// A tile of the persistent kernel's walk: its frame, origin and whether the vector path takes it.
+// A filter tile: its frame, origin and whether the vector path takes it.
 struct TileRef {
   const FrameDev* F;
   int x0, y0;
   bool mine;  // the frame has this kernel's filter configuration
-  bool vec;   // interior tile with an aligned output row: vector path (and asynchronous prefetch)
+  bool vec;   // interior tile with an aligned output row: vector path
 };
 
-constexpr int kV4Rows = 3 * (kTH + 8);       // window rows of the three planes: one bulk copy each
-constexpr uint32_t kV4RowBytes = (kTW + 8) * 4;
-
-// Window of the vector path fetched by the asynchronous copy engine: one cp.async.bulk per window row and plane
-// (288 bytes, 16-byte aligned on both sides), all completing on one mbarrier. Called by the first kV4Rows threads.
-__device__ __forceinline__ void v4_prefetch(const FrameDev& F, const float* src_planes, float* buf, int x0, int y0, uint64_t* bar) {
-  constexpr int WW = kTW + 8, WH = kTH + 8, NC = WW * WH;
-  const int r = threadIdx.x;
-  if (r >= kV4Rows) return;
-  const int c = r / WH, ly = r % WH;
-  const float* g = src_planes + F.plane_base + size_t(c) * F.plane_size + size_t(y0 - 4 + ly) * F.plane_stride + (x0 - 4);
-  bulk_load(buf + c * NC + ly * WW, g, kV4RowBytes, bar);
-}
-
-// X holds (or receives) the tile's window, Y is the second plane buffer. After EPF stage 1 the Y buffer is dead, so
-// the window of the CTA's next tile is fetched into it while stage 2, the colour conversion and the store run.
+// Gaborish + EPF iters 2 on an interior tile, four pixels per thread: bufA receives the tile's window, bufB is the
+// second plane buffer.
 __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev& F, const float* src_planes, float* bufA,
-                                               float* bufB, float* maps, float* sig, float* sig_next, int x0, int y0,
-                                               bool prefetched, uint64_t* bar, uint32_t& bar_parity, const TileRef& next) {
+                                               float* bufB, float* maps, float* sig, int x0, int y0) {
   using C = FCfg<true, 2>;
   constexpr int H = 4, WW = C::WW, WH = C::WH, NC = C::NC, QW = WW / 4;
   static_assert(C::H == H && WW == 72 && WH == 40, "vector path is written for the halo-4 configuration");
   const int wx0 = x0 - H, wy0 = y0 - H;
   const int sbx0 = wx0 >> 3, sby0 = wy0 >> 3;
-  if (prefetched) {
-    mbar_wait(bar, bar_parity);  // the copies were started during the previous tile; sig was filled then as well
-    bar_parity ^= 1;
-  } else {
-    // ---- load ----
-    for (int q = threadIdx.x; q < QW * WH; q += blockDim.x) {
-      const int ly = q / QW, o = ly * WW + (q % QW) * 4;
-      const float* g = src_planes + F.plane_base + size_t(wy0 + ly) * F.plane_stride + wx0 + (q % QW) * 4;
+  // ---- load ----
+  for (int q = threadIdx.x; q < QW * WH; q += blockDim.x) {
+    const int ly = q / QW, o = ly * WW + (q % QW) * 4;
+    const float* g = src_planes + F.plane_base + size_t(wy0 + ly) * F.plane_stride + wx0 + (q % QW) * 4;
 #pragma unroll
-      for (int c = 0; c < 3; c++) st4(bufA + c * NC + o, __ldg(reinterpret_cast<const float4*>(g + c * F.plane_size)));
-    }
-    tile_sigma<C::SBW, C::SBH>(B, F, sig, sbx0, sby0, threadIdx.x, blockDim.x);
-    __syncthreads();
+    for (int c = 0; c < 3; c++) st4(bufA + c * NC + o, __ldg(reinterpret_cast<const float4*>(g + c * F.plane_size)));
   }
+  tile_sigma<C::SBW, C::SBH>(B, F, sig, sbx0, sby0, threadIdx.x, blockDim.x);
+  __syncthreads();
   // ---- Gaborish (gaborish.rs:40-88): rows 1..38, bufA -> bufB ----
   for (int q = threadIdx.x; q < QW * (WH - 2); q += blockDim.x) {
     const int ly = 1 + q / QW, o = ly * WW + (q % QW) * 4;
@@ -3039,15 +2808,6 @@ __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev
     }
   }
   __syncthreads();
-  if (next.vec) {
-    // bufB is dead from here on: fetch the next tile's window into it (the generic-proxy reads of stage 1 are ordered
-    // before the asynchronous writes by the barrier above plus the proxy fence), and its sigma blocks on idle threads
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    v4_prefetch(*next.F, src_planes, bufB, next.x0, next.y0, bar);
-    if (int(threadIdx.x) >= kV4Rows)
-      tile_sigma<C::SBW, C::SBH>(B, *next.F, sig_next, (next.x0 - H) >> 3, (next.y0 - H) >> 3, int(threadIdx.x) - kV4Rows,
-                                 int(blockDim.x) - kV4Rows);
-  }
   // ---- EPF stage 2 (epf2.rs) on the 64x32 core + colour + store ----
   epf_maps_v4<WW, NC>(bufA, maps, 3, WH - 3, cs0, cs1, cs2);
   __syncthreads();
@@ -3164,7 +2924,6 @@ __device__ __forceinline__ TileRef locate_tile(const BatchDev& B, const FusedTil
   r.F = nullptr;
   r.x0 = r.y0 = 0;
   r.mine = r.vec = false;
-  if (tile_id >= T.tile_end) return r;
   uint32_t lo = 0, hi = T.num_frames;
   while (hi - lo > 1) {
     uint32_t mid = (lo + hi) >> 1;
@@ -3198,77 +2957,12 @@ __global__ void __launch_bounds__(kFilterThreads) k_filters_store(const BatchDev
   const bool interior = r.x0 - C::H >= 0 && r.y0 - C::H >= 0 && r.x0 + kTW + C::H <= int(F.width) && r.y0 + kTH + C::H <= int(F.height);
   if (GAB && EPF == 2 && r.vec) {
     __shared__ float s_sig[FCfg<true, 2>::SBW * FCfg<true, 2>::SBH];
-    uint32_t parity = 0;
-    TileRef none;
-    none.F = nullptr;
-    none.x0 = none.y0 = 0;
-    none.mine = none.vec = false;
-    filter_tile_v4(B, F, src_planes, smem, smem + 3 * FCfg<true, 2>::NC, smem + 6 * FCfg<true, 2>::NC, s_sig, s_sig, r.x0, r.y0, false,
-                   nullptr, parity, none);
+    filter_tile_v4(B, F, src_planes, smem, smem + 3 * FCfg<true, 2>::NC, smem + 6 * FCfg<true, 2>::NC, s_sig, r.x0, r.y0);
   } else if (interior) {
     filter_tile<GAB, EPF, true>(B, F, src_planes, smem, r.x0, r.y0);
   } else {
     filter_tile<GAB, EPF, false>(B, F, src_planes, smem, r.x0, r.y0);
   }
-}
-
-// Gaborish + EPF iters 2 can also run persistently (JXG_FILTERS_PERSISTENT=1): 2 CTAs per SM stride over the launch's tiles,
-// interior tiles take the vector path with their window prefetched by bulk copies during the previous tile's last
-// phase; edge tiles (and frames with unaligned output rows) take the generic path in the same shared memory.
-__global__ void __launch_bounds__(kFilterThreads, 2) k_filters_v4(const BatchDev B, const FusedTiles T, const float* src_planes) {
-  using C = FCfg<true, 2>;
-  extern __shared__ float smem[];
-  __shared__ __align__(8) uint64_t s_bar;
-  __shared__ float s_sig[2][C::SBW * C::SBH];
-  if (threadIdx.x == 0) {
-    mbar_init(&s_bar, kV4Rows);
-    mbar_fence_init();
-  }
-  __syncthreads();
-  float* bufX = smem;               // holds the current tile's window
-  float* bufY = smem + 3 * C::NC;
-  float* maps = smem + 6 * C::NC;
-  uint32_t parity = 0, cur = 0;
-  bool prefetched = false;
-  uint32_t tile = T.tile_begin + blockIdx.x;
-  TileRef r = locate_tile<true, 2>(B, T, tile);
-  while (tile < T.tile_end) {
-    const TileRef next = locate_tile<true, 2>(B, T, tile + gridDim.x);
-    if (r.mine) {
-      if (r.vec) {
-        filter_tile_v4(B, *r.F, src_planes, bufX, bufY, maps, s_sig[cur], s_sig[cur ^ 1], r.x0, r.y0, prefetched, &s_bar, parity, next);
-        prefetched = next.vec;
-        if (prefetched) {  // the next window is arriving in bufY
-          float* t = bufX; bufX = bufY; bufY = t;
-          cur ^= 1;
-        }
-      } else {
-        const FrameDev& F = *r.F;
-        const bool interior = r.x0 - C::H >= 0 && r.y0 - C::H >= 0 && r.x0 + kTW + C::H <= int(F.width) && r.y0 + kTH + C::H <= int(F.height);
-        if (interior) filter_tile<true, 2, true>(B, F, src_planes, smem, r.x0, r.y0);
-        else filter_tile<true, 2, false>(B, F, src_planes, smem, r.x0, r.y0);
-      }
-      __syncthreads();  // every reader of this tile's buffers is done before the next tile writes them
-    }
-    r = next;
-    tile += gridDim.x;
-  }
-}
-
-// Experiment knobs (read once): JXG_FILTER_THREADS = threads per filter CTA (multiple of 32, 128..512; the kernels stride
-// by blockDim.x), JXG_FILTERS_PERSISTENT = 1 selects the persistent prefetching kernel for Gaborish + EPF 2.
-static int filter_threads() {
-  static const int n = [] {
-    const char* e = getenv("JXG_FILTER_THREADS");
-    int v = e ? atoi(e) : kFilterThreads;
-    v = (v / 32) * 32;
-    return v < 128 ? 128 : (v > kFilterThreads ? kFilterThreads : v);
-  }();
-  return n;
-}
-static bool filters_persistent() {
-  static const bool on = getenv("JXG_FILTERS_PERSISTENT") && atoi(getenv("JXG_FILTERS_PERSISTENT")) != 0;
-  return on;
 }
 
 int sm_count() {
@@ -3280,20 +2974,10 @@ int sm_count() {
 
 template <bool GAB, int EPF>
 static void launch_filters(const BatchDev& B, const FusedTiles& FT, uint32_t tiles, cudaStream_t stream) {
-  if (GAB && EPF == 2 && filters_persistent()) {
-    const uint32_t resident = 2 * uint32_t(sm_count());
-    const uint32_t grid = tiles < resident ? tiles : resident;
-    k_filters_v4<<<grid, filter_threads(), FCfg<true, 2>::kSmemBytes, stream>>>(B, FT, B.planes_a);
-    return;
-  }
-  k_filters_store<GAB, EPF><<<tiles, filter_threads(), FCfg<GAB, EPF>::kSmemBytes, stream>>>(B, FT, B.planes_a);
+  k_filters_store<GAB, EPF><<<tiles, kFilterThreads, FCfg<GAB, EPF>::kSmemBytes, stream>>>(B, FT, B.planes_a);
 }
 template <bool GAB, int EPF>
 static cudaError_t configure_filters() {
-  if (GAB && EPF == 2) {
-    cudaError_t e = cudaFuncSetAttribute(k_filters_v4, cudaFuncAttributeMaxDynamicSharedMemorySize, int(FCfg<true, 2>::kSmemBytes));
-    if (e != cudaSuccess) return e;
-  }
   return cudaFuncSetAttribute(k_filters_store<GAB, EPF>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                               int(FCfg<GAB, EPF>::kSmemBytes));
 }
@@ -3358,87 +3042,31 @@ cudaError_t configure_kernels() {
   if ((e = cudaFuncSetAttribute(k_idct_small<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(small_smem_bytes<1>()))) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(k_idct_small<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(small_smem_bytes<2>()))) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(k_dequant_idct, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kLargeSmemBytes))) != cudaSuccess) return e;
-  // One shared-memory carve-out for every kernel of the pipeline. An SM can only change its L1 / shared-memory split when
-  // it is empty, so a filter CTA (92 KB) or transform CTA (68 - 101 KB) of one batch cannot join an SM that still holds
-  // entropy CTAs of another batch launched with a small carve-out: kernels of different streams then only overlap in the
-  // entropy kernel's tail. JXG_CARVEOUT = percentage of the unified memory given to shared memory (-1, the default, leaves the
-  // driver's per-kernel choice). 100 costs the entropy kernel its L1 and gained nothing at 3 resident batches; 75 was
-  // within noise of the default.
-  int pct = -1;
-  if (const char* env = getenv("JXG_CARVEOUT")) pct = atoi(env);
-  if (pct >= 0) {
-#define JXG_CARVE(k) \
-  if ((e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct)) != cudaSuccess) return e;
-#define JXG_CARVE_LEAN(SV)                 \
-  JXG_CARVE((k_entropy_lean<SV, true, true>))   \
-  JXG_CARVE((k_entropy_lean<SV, true, false>))  \
-  JXG_CARVE((k_entropy_lean<SV, false, true>))  \
-  JXG_CARVE((k_entropy_lean<SV, false, false>)) \
-  JXG_CARVE((k_entropy_fast<SV>))
-#define JXG_CARVE_WIDE(SV)                 \
-  JXG_CARVE((k_entropy_lean<SV, true, true>))   \
-  JXG_CARVE((k_entropy_lean<SV, true, false>))  \
-  JXG_CARVE((k_entropy_lean<SV, false, true>))  \
-  JXG_CARVE((k_entropy_lean<SV, false, false>))
-    JXG_CARVE_LEAN(1)
-    JXG_CARVE_LEAN(2)
-    JXG_CARVE_LEAN(4)
-    JXG_CARVE_LEAN(8)
-    JXG_CARVE_WIDE(16)
-    JXG_CARVE_WIDE(32)
-    JXG_CARVE(k_entropy)
-    JXG_CARVE(k_block_plan)
-    JXG_CARVE((k_idct_small<0>))
-    JXG_CARVE((k_idct_small<1>))
-    JXG_CARVE((k_idct_small<2>))
-    JXG_CARVE(k_dequant_idct)
-    JXG_CARVE(k_filters_v4)
-    JXG_CARVE((k_filters_store<false, 0>))
-    JXG_CARVE((k_filters_store<false, 1>))
-    JXG_CARVE((k_filters_store<false, 2>))
-    JXG_CARVE((k_filters_store<false, 3>))
-    JXG_CARVE((k_filters_store<true, 0>))
-    JXG_CARVE((k_filters_store<true, 1>))
-    JXG_CARVE((k_filters_store<true, 2>))
-    JXG_CARVE((k_filters_store<true, 3>))
-    JXG_CARVE(k_orient)
-#undef JXG_CARVE_LEAN
-#undef JXG_CARVE_WIDE
-#undef JXG_CARVE
-  }
   return cudaSuccess;
 }
 
-int launch_pipeline(const BatchDev& B, const uint32_t* tile_prefix, uint32_t total_tiles, uint32_t max_epf_iters,
-                    bool any_gab, cudaStream_t stream, size_t coeff_bytes, const float** final_planes, int debug_stop,
-                    cudaEvent_t* ev, const uint32_t* fused_prefix, uint32_t fused_tiles, uint32_t filter_cfg_mask,
-                    bool lean_all_420, uint32_t lean_S, uint32_t lean_ctas, bool lean_ctx_smem, cudaStream_t post_stream,
-                    cudaEvent_t handoff) {
+int launch_pipeline(const BatchDev& B, cudaStream_t stream, int debug_stop, cudaEvent_t* ev, bool lean_all_420,
+                    uint32_t lean_S, uint32_t lean_ctas, bool lean_ctx_smem, cudaStream_t post_stream, cudaEvent_t handoff) {
   // ev (optional, kNumStages + 1 events): ev[i] is recorded before stage i, ev[i+1] after it; stages that do not
   // run record nothing (the host pairs consecutive recorded events).
   int launches = 0;
   auto mark = [&](int i) {
     if (ev) cudaEventRecord(ev[i], stream);
   };
-  mark(0);
-  (void)coeff_bytes;  // no dense coefficient array any more: nothing to clear
+  mark(0);  // stage 0 (memset) is empty: there is no dense coefficient array to clear
   mark(1);
   k_block_plan<<<(B.num_streams + 3) / 4, 128, 0, stream>>>(B);
   launches++;
   if (B.num_lean) {
-    // Persistent lanes, scheduled per frame by the host (batch.cc schedule_lean): S lanes per warp, lean_ctas CTAs.
+    // Persistent lanes, scheduled per frame by the host (batch.cc schedule_lean): S = 4 or 8 lanes per warp, lean_ctas CTAs.
     cudaMemsetAsync(B.queue, 0, sizeof(uint32_t) * B.num_frames, stream);
     const uint32_t S = lean_S, grid = lean_ctas;
     const int smem = lean_ctx_smem ? int(kLeanCtxSmem) : 0;
 #define JXG_LEAN(SV, KV, CV) k_entropy_lean<SV, KV, CV><<<grid, 128, smem, stream>>>(B)
-#define JXG_LEAN_S(KV, CV)                                    \
-  do {                                                        \
-    if (S == 1) JXG_LEAN(1, KV, CV);                          \
-    else if (S == 2) JXG_LEAN(2, KV, CV);                     \
-    else if (S == 4) JXG_LEAN(4, KV, CV);                     \
-    else if (S == 8) JXG_LEAN(8, KV, CV);                     \
-    else if (S == 16) JXG_LEAN(16, KV, CV);                   \
-    else JXG_LEAN(32, KV, CV);                                \
+#define JXG_LEAN_S(KV, CV)             \
+  do {                                 \
+    if (S == 8) JXG_LEAN(8, KV, CV);   \
+    else JXG_LEAN(4, KV, CV);          \
   } while (0)
     if (lean_all_420) {
       if (lean_ctx_smem) JXG_LEAN_S(true, true);
@@ -3453,8 +3081,7 @@ int launch_pipeline(const BatchDev& B, const uint32_t* tile_prefix, uint32_t tot
   }
   if (B.num_fast) {
     // streams per warp: aim at about one resident wave (592 schedulers x ~4 warps)
-    uint32_t per = (B.num_fast + 2367) / 2368;
-    if (const char* e = getenv("JXG_ENTROPY_S")) per = uint32_t(atoi(e));  // experiment knob
+    const uint32_t per = (B.num_fast + 2367) / 2368;
     if (per <= 1) k_entropy_fast<1><<<(B.num_fast + 3) / 4, 128, 0, stream>>>(B);
     else if (per <= 2) k_entropy_fast<2><<<(B.num_fast + 7) / 8, 128, 0, stream>>>(B);
     else if (per <= 4) k_entropy_fast<4><<<(B.num_fast + 15) / 16, 128, 0, stream>>>(B);
@@ -3466,7 +3093,6 @@ int launch_pipeline(const BatchDev& B, const uint32_t* tile_prefix, uint32_t tot
     launches++;
   }
   mark(2);
-  if (final_planes) *final_planes = B.planes_a;
   if (debug_stop == 1) return launches;
   if (post_stream != stream) {  // two-stage pipeline: the transforms and filters of this batch continue on the post stream
     cudaEventRecord(handoff, stream);
@@ -3480,70 +3106,7 @@ int launch_pipeline(const BatchDev& B, const uint32_t* tile_prefix, uint32_t tot
   k_dequant_idct<<<B.num_streams, kIdctWarps * 32, kLargeSmemBytes, stream>>>(B);
   launches++;
   mark(3);
-  if (debug_stop == 2) return launches;
-  if (debug_stop != 3) {  // default: fused filter + colour + store kernel, launched per frame range by the caller
-    if (final_planes) *final_planes = nullptr;
-    return launches;
-  }
-  TileDev T{tile_prefix, B.num_frames};
-  dim3 blk(32, 8);
-  const float* cur = B.planes_a;
-  float* nxt = B.planes_b;
-  auto swap = [&] {
-    const float* t = cur;
-    cur = nxt;
-    nxt = const_cast<float*>(t);
-  };
-  if (any_gab) {
-    k_gaborish<<<total_tiles, blk, 0, stream>>>(B, T, cur, nxt);
-    launches++;
-    swap();
-  }
-  mark(4);
-  if (max_epf_iters >= 3) {
-    k_epf<0><<<total_tiles, blk, 0, stream>>>(B, T, cur, nxt);
-    launches++;
-    swap();
-  }
-  mark(5);
-  if (max_epf_iters >= 1) {
-    k_epf<1><<<total_tiles, blk, 0, stream>>>(B, T, cur, nxt);
-    launches++;
-    swap();
-  }
-  mark(6);
-  if (max_epf_iters >= 2) {
-    k_epf<2><<<total_tiles, blk, 0, stream>>>(B, T, cur, nxt);
-    launches++;
-    swap();
-  }
-  mark(7);
-  k_xyb_store<<<total_tiles, blk, 0, stream>>>(B, T, cur);
-  launches++;
-  mark(8);
-  if (final_planes) *final_planes = cur;
-  return launches;
-}
-
-// Upload of the staging blob by the SMs: 16-byte loads from the pinned host arena (the device reaches it through UVA),
-// 16-byte stores to the device copy. Used instead of cudaMemcpyAsync when copy-engine work of other batches (the D2H
-// copies of finished frames) would sit in front of this batch's H2D copy: see batch.cc jxg_batch_run.
-__global__ void __launch_bounds__(256) k_upload(const uint4* __restrict__ src, uint4* __restrict__ dst, size_t n16) {
-  const size_t stride = size_t(gridDim.x) * blockDim.x;
-  size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  for (; i + 3 * stride < n16; i += 4 * stride) {  // four loads in flight per thread: the host link's latency is microseconds
-    const uint4 a = src[i], b = src[i + stride], c = src[i + 2 * stride], d = src[i + 3 * stride];
-    dst[i] = a;
-    dst[i + stride] = b;
-    dst[i + 2 * stride] = c;
-    dst[i + 3 * stride] = d;
-  }
-  for (; i < n16; i += stride) dst[i] = src[i];
-}
-
-void launch_upload(const void* host_pinned, void* dev, size_t bytes, cudaStream_t stream) {
-  const size_t n16 = (bytes + 15) / 16;  // both buffers are allocated in 16-byte multiples and 16-byte aligned
-  k_upload<<<64, 256, 0, stream>>>(static_cast<const uint4*>(host_pinned), static_cast<uint4*>(dev), n16);
+  return launches;  // the fused filter + colour + store kernel is launched per frame range by the caller
 }
 
 // Parity tap: the coefficient lists of one frame expanded into the reference's dense decode-order layout
@@ -3589,7 +3152,7 @@ int launch_filter_range(const BatchDev& B, const uint32_t* fused_prefix, uint32_
                         uint32_t filter_cfg_mask, cudaStream_t stream) {
   int launches = 0;
   if (!tile_count) return 0;
-  FusedTiles FT{fused_prefix, B.num_frames, tile_begin, tile_begin + tile_count};
+  FusedTiles FT{fused_prefix, B.num_frames, tile_begin};
   for (int cfg = 0; cfg < 8; cfg++) {
     if (!(filter_cfg_mask & (1u << cfg))) continue;
     switch (cfg) {

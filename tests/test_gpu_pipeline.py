@@ -161,3 +161,31 @@ def test_c_abi_rejects_inconsistent_descriptors():
                    setter("orientation", 9), setter("output_tf", 77), setter("global_scale", 0)):
         assert try_add(mutate) == -22, mutate  # JXG_ERR_ARGUMENT
     ctx.close()
+
+
+def test_c_abi_rejects_unknown_debug_stages():
+    """Debug stops 0-2 and XYB tap stage 0 are the only stages there are: a NULL batch or any other stage is
+    JXG_ERR_ARGUMENT, and stage 0 of a run stopped after the transforms still reads."""
+    import torch
+    import jxl_rs_b200 as j
+    import synth
+    fr = j.ParsedFrame(synth.encode_synthetic(300, 200, 9, 0.5, 2, 1, 1))
+    ctx = j.JxgContext(0)
+    out = torch.empty((3, 200, 300), dtype=torch.float32).pin_memory()
+    b = j.Batch(ctx, 1)
+    try:
+        lib = b._lib
+        assert lib.jxg_batch_set_debug_stop(None, 2) == -22  # JXG_ERR_ARGUMENT
+        for stage in (-1, 3, 4):
+            assert lib.jxg_batch_set_debug_stop(b._h, stage) == -22, stage
+        assert lib.jxg_batch_set_debug_stop(b._h, 2) == 0
+        b.add(fr, out.data_ptr(), 300 * 4, abi.FORMAT_XYB_F32_PLANAR, False)
+        b.run()
+        b.wait()
+        assert np.isfinite(b.read_xyb(0, 0)).all()
+        for stage in (1, 2):
+            with pytest.raises(abi.JxgError):
+                b.read_xyb(0, stage)
+    finally:
+        b.close()
+        ctx.close()

@@ -23,5 +23,4 @@ run() {  # name depth env...
 run fifo_d4 4
 run fifo_d5 5
 run fifo_d5_nomarks 5 E2E_MARKS=
-run upk_d4 4 JXG_UPLOAD_KERNEL=1
 echo "=== done ($(date +%T))" | tee -a "$OUT/session.log"
