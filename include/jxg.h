@@ -259,8 +259,11 @@ int jxg_parsed_desc(void* parsed, uint32_t output_format, JxgFrameDesc* desc, co
  * the same state from Frame::decode_lf_global / decode_lf_group (frame/decode.rs:307-497).
  * Device scope: 8-bit RGB / grey, one pass, global transforms RCT and Squeeze, group-local RCT, ANS or prefix codes,
  * all 14 predictors incl. the weighted one, all properties incl. those of reference channels, the global palette
- * transform without delta entries (transforms/palette.rs:165-199). Delta palettes and LZ77 in group streams return
- * JXG_ERR_UNSUPPORTED (no CPU fallback). Output: interleaved RGB u8 (grey replicated). */
+ * transform without delta entries (transforms/palette.rs:165-199), LZ77 in group streams (decode.rs:286-330, the window
+ * in device memory: min(2^20, pixels) x 4 bytes per LZ77 stream). Delta palettes return JXG_ERR_UNSUPPORTED (no CPU
+ * fallback). A group stream that fails (ANS checksum, over-read, an LZ77 copy before any symbol or a copy length
+ * overflow: JXG_ERR_LZ77) is reported by jxg_modular_batch_wait; the other streams still decode. Output: interleaved
+ * RGB u8 (grey replicated). */
 int jxg_modular_parse_file(const uint8_t* data, size_t size, void** parsed, JxgImageInfo* info);
 void jxg_modular_parsed_free(void* parsed);
 int jxg_modular_batch_begin(void* ctx, void** batch);
@@ -275,6 +278,9 @@ int jxg_modular_batch_rerun_device(void* batch, void* cuda_stream);
 int jxg_modular_batch_read_planes(void* batch, uint32_t f, int32_t* out, size_t out_len);
 /* ms[0]: whole batch on the device, ms[1]: group-stream decode kernel (+ local RCT). */
 int jxg_modular_batch_stats(void* batch, uint64_t* h2d_bytes, uint64_t* d2h_bytes, uint64_t* kernel_launches, float* ms);
+/* Group streams of the frames added so far whose code uses LZ77; of those, the ones whose copies all have distance 1
+ * (Histograms::is_rle, the shape of libjxl's fastest lossless mode); device bytes of their symbol windows. */
+int jxg_modular_batch_lz77_stats(void* batch, uint32_t* lz77_streams, uint32_t* rle_streams, uint64_t* window_bytes);
 void jxg_modular_batch_end(void* batch);
 /* Parity tap (no device needed): the table form of one channel's MA-tree walk as the Modular path builds it - the device
  * counterpart of the single-property specialisations of frame/modular/decode/specialized_trees.rs:197-372.

@@ -48,6 +48,9 @@ struct ModularBatch {
   std::vector<int> level_kind;
   std::vector<MJobDev> store_jobs;
   uint64_t arena_elems = 0, wp_bytes = 0, out_bytes = 0;
+  uint64_t lz_window_elems = 0;             // symbol windows of the LZ77 streams, one per stream
+  uint32_t lz77_streams = 0, rle_streams = 0;  // streams with LZ77; of those, streams whose copies all have distance 1
+  uint32_t num_plain = 0;                   // streams without LZ77: the first ones of `order`
   std::vector<uint32_t> stream_frame_group;  // for error reports
   bool uploaded = false;
   uint64_t launches = 0, h2d = 0, d2h = 0;
@@ -65,9 +68,15 @@ uint64_t blob_append(ModularBatch* b, const void* p, size_t bytes, size_t align 
 }
 
 uint32_t add_code(ModularBatch* b, const jxg::EntropyCode& c) {
-  if (c.lz77_enabled) throw jxg::Error(JXG_ERR_UNSUPPORTED, "LZ77 in Modular group streams is not implemented on the device path");
   MCodeDev d;
   memset(&d, 0, sizeof(d));
+  if (c.lz77_enabled) {
+    d.lz_enabled = 1;
+    d.lz_min_symbol = c.lz77_min_symbol;
+    d.lz_min_length = c.lz77_min_length;
+    d.lz_len_cfg = c.lz77_length_uint.packed();
+    d.lz_dist_cluster = c.lz_dist_cluster;
+  }
   d.use_prefix = c.use_prefix;
   d.log_alpha = c.log_alpha_size;
   d.num_clusters = c.num_clusters;
@@ -322,6 +331,15 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t st
     }
     d.num_rct = uint32_t(b->rcts.size()) - d.first_rct;
     if (d.num_rct) b->rct_streams.push_back(uint32_t(b->streams.size()));
+    if (tree->code.lz77_enabled) {
+      uint64_t pixels = 0;
+      for (const jxg::ModularRect& r : st.rects) pixels += uint64_t(r.w) * r.h;
+      d.dist_multiplier = st.dist_multiplier;
+      d.lz_window_off = b->lz_window_elems;
+      b->lz_window_elems += std::min<uint64_t>(pixels, uint64_t(1) << 20);  // one symbol per pixel
+      b->lz77_streams++;
+      if (tree->code.is_rle()) b->rle_streams++;
+    }
     b->streams.push_back(d);
   }
   f.num_streams = uint32_t(b->streams.size()) - f.first_stream;
@@ -395,12 +413,13 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
   B.status = static_cast<int32_t*>(cx->d_status.p);
   B.queue = reinterpret_cast<uint32_t*>(B.status + b->streams.size());
   B.num_streams = uint32_t(b->streams.size());
+  B.lz_window = static_cast<uint32_t*>(cx->d_modular_lzwin.p);
   // host-decoded planes: blob -> arena (device to device)
   for (const MFrame& f : b->frames)
     if (f.host_planes_elems)
       CUDA_TRY(cudaMemcpyAsync(B.planes + f.arena_base, B.blob + f.host_planes_blob, f.host_planes_elems * 4,
                                cudaMemcpyDeviceToDevice, s));
-  uint64_t launches = uint64_t(launch_modular_decode(B, b->lanes_per_warp, uint32_t(b->rct_streams.size()), s));
+  uint64_t launches = uint64_t(launch_modular_decode(B, b->num_plain, b->lanes_per_warp, uint32_t(b->rct_streams.size()), s));
   if (b->ev_decode) CUDA_TRY(cudaEventRecord(b->ev_decode, s));
   const MJobDev* jobs = static_cast<const MJobDev*>(b->d_jobs.p);
   size_t job_cursor = 0;
@@ -514,15 +533,25 @@ int jxg_modular_batch_run(void* bp, void* cuda_stream) {
   CUDA_TRY(cudaSetDevice(cx->device));
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : cx->stream;
   b->h2d = b->d2h = 0;
-  // longest section first (the decode kernel's queue is a longest-processing-time schedule)
+  // streams without LZ77, then those with it (each group has its own decode launch); longest section first within
+  // each (the decode kernel's queue is a longest-processing-time schedule)
   b->order.resize(b->streams.size());
   for (uint32_t i = 0; i < b->order.size(); i++) b->order[i] = i;
-  std::stable_sort(b->order.begin(), b->order.end(), [&](uint32_t x, uint32_t y) { return b->streams[x].sec_len > b->streams[y].sec_len; });
+  auto lz = [&](uint32_t i) { return b->codes[b->streams[i].code].lz_enabled != 0; };
+  std::stable_sort(b->order.begin(), b->order.end(), [&](uint32_t x, uint32_t y) {
+    return lz(x) != lz(y) ? lz(y) : b->streams[x].sec_len > b->streams[y].sec_len;
+  });
+  b->num_plain = uint32_t(b->streams.size()) - b->lz77_streams;
   if (int r = cx->d_blob.ensure(cx->blob.size + 64)) return r;
   if (int r = cx->d_planes_a.ensure(std::max<size_t>(b->arena_elems * 4, 16))) return r;
   if (int r = cx->d_status.ensure((b->streams.size() + 8) * 4)) return r;
   if (int r = cx->d_out.ensure(std::max<size_t>(b->out_bytes, 16))) return r;
   if (int r = b->d_wp.ensure(std::max<size_t>(b->wp_bytes, 16))) return r;
+  if (b->lz_window_elems && cx->d_modular_lzwin.ensure(b->lz_window_elems * 4)) {
+    cudaGetLastError();
+    return set_error(JXG_ERR_UNSUPPORTED, "no device memory for the LZ77 windows of the batch (" +
+                                              std::to_string(b->lz_window_elems * 4) + " bytes)");
+  }
   for (size_t i = 0; i < b->frames.size(); i++) {
     MFrame& f = b->frames[i];
     b->store_jobs[i].out = f.out_is_device ? f.out : static_cast<uint8_t*>(cx->d_out.p) + f.dev_out_off;
@@ -614,6 +643,15 @@ int jxg_modular_batch_stats(void* bp, uint64_t* h2d, uint64_t* d2h, uint64_t* la
     cudaEventElapsedTime(&ms[1], b->ev0, b->ev_decode);
     cudaGetLastError();
   }
+  return JXG_OK;
+}
+
+int jxg_modular_batch_lz77_stats(void* bp, uint32_t* lz77_streams, uint32_t* rle_streams, uint64_t* window_bytes) {
+  ModularBatch* b = static_cast<ModularBatch*>(bp);
+  if (!b) return JXG_ERR_ARGUMENT;
+  if (lz77_streams) *lz77_streams = b->lz77_streams;
+  if (rle_streams) *rle_streams = b->rle_streams;
+  if (window_bytes) *window_bytes = b->lz_window_elems * 4;
   return JXG_OK;
 }
 

@@ -12,6 +12,9 @@ struct MCodeDev {  // one EntropyCode (decode.rs:36-58), tables in the blob
   uint64_t ans_off;          // u64[num_clusters << log_alpha] alias buckets (ans.rs:31-39)
   uint64_t huff_off;         // u32[] bits | value << 16
   uint64_t huff_offset_off;  // u32[num_clusters]
+  // LZ77 (decode.rs:36-45): tokens >= lz_min_symbol start a copy of hybrid(lz_len_cfg) + lz_min_length symbols, whose
+  // distance is read from cluster lz_dist_cluster
+  uint32_t lz_enabled, lz_min_symbol, lz_min_length, lz_len_cfg, lz_dist_cluster, lz_pad;
 };
 
 struct MStreamDev {  // one ModularHF(group) section
@@ -27,6 +30,10 @@ struct MStreamDev {  // one ModularHF(group) section
   uint32_t wp_params[11];   // p1c, p2c, p3ca..p3ce, w[4]
   uint64_t wp_scratch_off;  // bytes into wp_scratch
   uint32_t first_rct, num_rct;
+  // LZ77 streams: the widest channel of the stream (the distance multiplier, bitstream.rs:193-202) and the element
+  // offset of the stream's window (min(2^20, pixels) u32 entries) in MBatchDev::lz_window
+  uint32_t dist_multiplier;
+  uint64_t lz_window_off;
 };
 
 // Channel walk. The decisions of the MA tree on the channel index and the stream id are constant for a channel; when
@@ -73,9 +80,13 @@ struct MBatchDev {
   int32_t* status;
   uint32_t* queue;
   uint32_t num_streams;
+  uint32_t* lz_window;  // symbol windows of the LZ77 streams
 };
 
-int launch_modular_decode(const MBatchDev& B, uint32_t lanes_per_warp, uint32_t num_rct_streams, cudaStream_t stream);
+// The first num_plain entries of B.order are streams without LZ77, the remaining B.num_streams - num_plain use it: each
+// group is decoded by its own launch of k_modular_decode (B.queue[0] / B.queue[1]), then the local RCTs run.
+int launch_modular_decode(const MBatchDev& B, uint32_t num_plain, uint32_t lanes_per_warp, uint32_t num_rct_streams,
+                          cudaStream_t stream);
 // kind: 0 RCT, 1 horizontal unsqueeze, 2 vertical unsqueeze, 3 store, 4 palette look-up
 void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint32_t max_w, uint32_t max_h, int32_t* planes,
                          cudaStream_t stream);

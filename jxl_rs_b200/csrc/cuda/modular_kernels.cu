@@ -2,7 +2,8 @@
 //   k_modular_decode   per-pixel MA-tree walk + predictor (+ weighted predictor) + ANS / prefix symbol decode of the
 //                      ModularHF sections: one lane per (frame, group) stream, persistent lanes pulling streams
 //                      (longest first) from a device queue            <- modular/decode/channel.rs:220, tree.rs:189-280,
-//                                                                        predict.rs:148-527, decode/common.rs:85
+//                      streams with LZ77 in a launch of their own        predict.rs:148-527, decode/common.rs:85,
+//                                                                        entropy_coding/decode.rs:286-330
 //   k_modular_local_rct  inverse RCT of a group's local transforms     <- transforms/rct.rs:9-40 (apply_local.rs)
 //   k_modular_rct / k_unsqueeze_h / k_unsqueeze_v  global inverse transforms over full planes
 //                                                                     <- transforms/rct.rs, squeeze.rs:144-195,390,577
@@ -68,7 +69,7 @@ struct MBr {  // bit reader over an 8-byte aligned, zero padded section copy (bi
   }
 };
 
-struct MSym {  // symbol reader state of one stream (decode.rs:177-405 without LZ77)
+struct MSym {  // symbol reader state of one stream (decode.rs:177-405; LZ77 state in MLz)
   MBr br;
   uint32_t ans_state;
   const uint8_t* cmap;
@@ -79,7 +80,7 @@ struct MSym {  // symbol reader state of one stream (decode.rs:177-405 without L
   uint32_t use_prefix, log_alpha;
 };
 
-__device__ __forceinline__ uint32_t m_read_clustered(MSym& s, uint32_t cluster) {
+__device__ __forceinline__ uint32_t m_token(MSym& s, uint32_t cluster) {
   uint32_t token;
   if (s.use_prefix) {  // huffman.rs:446-457
     const uint32_t* t = s.huff + __ldg(s.huff_offset + cluster);
@@ -108,8 +109,11 @@ __device__ __forceinline__ uint32_t m_read_clustered(MSym& s, uint32_t cluster) 
     if (next < (1u << 16)) next = (next << 16) | s.br.read(16);
     s.ans_state = next;
   }
-  // hybrid_uint.rs:87-102
-  const uint32_t cfg = __ldg(s.cfg + cluster);
+  return token;
+}
+
+// hybrid_uint.rs:87-102
+__device__ __forceinline__ uint32_t m_hybrid(MSym& s, uint32_t cfg, uint32_t token) {
   const uint32_t split_exponent = cfg & 0xff, msb = (cfg >> 8) & 0xff, lsb = (cfg >> 16) & 0xff;
   const uint32_t split_token = 1u << split_exponent;
   if (token < split_token) return token;
@@ -121,7 +125,73 @@ __device__ __forceinline__ uint32_t m_read_clustered(MSym& s, uint32_t cluster) 
   return (((hi << nbits) | bits) << lsb) | low;
 }
 
-__device__ __forceinline__ uint32_t m_read_unsigned(MSym& s, uint32_t ctx) { return m_read_clustered(s, __ldg(s.cmap + ctx)); }
+__device__ __forceinline__ uint32_t m_read_clustered(MSym& s, uint32_t cluster) {
+  const uint32_t token = m_token(s, cluster);
+  return m_hybrid(s, __ldg(s.cfg + cluster), token);
+}
+
+// LZ77 state of one stream (decode.rs:73-147). All channels of the stream share it: the window, the count of decoded
+// symbols and a pending copy carry across channel boundaries.
+constexpr uint32_t kLzMask = (1u << 20) - 1;  // WINDOW_MASK: the window is a ring of 2^20 symbols
+struct MLz {
+  uint32_t* win;  // min(2^20, pixels of the stream) entries: positions below 2^20 index it directly
+  uint32_t decoded, to_copy, copy_pos;
+  uint32_t mult, min_symbol, min_length, len_cfg, dist_cluster;
+  uint32_t err;  // a copy before any symbol, or a length overflow (decode.rs:300-317)
+};
+
+__constant__ int8_t c_special_dist[120][2] = {  // SPECIAL_DISTANCES (decode.rs:87-101): (dx, dy)
+    {0, 1},  {1, 0},  {1, 1},  {-1, 1}, {0, 2},  {2, 0},  {1, 2},  {-1, 2}, {2, 1},  {-2, 1}, {2, 2},  {-2, 2},
+    {0, 3},  {3, 0},  {1, 3},  {-1, 3}, {3, 1},  {-3, 1}, {2, 3},  {-2, 3}, {3, 2},  {-3, 2}, {0, 4},  {4, 0},
+    {1, 4},  {-1, 4}, {4, 1},  {-4, 1}, {3, 3},  {-3, 3}, {2, 4},  {-2, 4}, {4, 2},  {-4, 2}, {0, 5},  {3, 4},
+    {-3, 4}, {4, 3},  {-4, 3}, {5, 0},  {1, 5},  {-1, 5}, {5, 1},  {-5, 1}, {2, 5},  {-2, 5}, {5, 2},  {-5, 2},
+    {4, 4},  {-4, 4}, {3, 5},  {-3, 5}, {5, 3},  {-5, 3}, {0, 6},  {6, 0},  {1, 6},  {-1, 6}, {6, 1},  {-6, 1},
+    {2, 6},  {-2, 6}, {6, 2},  {-6, 2}, {4, 5},  {-4, 5}, {5, 4},  {-5, 4}, {3, 6},  {-3, 6}, {6, 3},  {-6, 3},
+    {0, 7},  {7, 0},  {1, 7},  {-1, 7}, {5, 5},  {-5, 5}, {7, 1},  {-7, 1}, {4, 6},  {-4, 6}, {6, 4},  {-6, 4},
+    {2, 7},  {-2, 7}, {7, 2},  {-7, 2}, {3, 7},  {-3, 7}, {7, 3},  {-7, 3}, {5, 6},  {-5, 6}, {6, 5},  {-6, 5},
+    {8, 0},  {4, 7},  {-4, 7}, {7, 4},  {-7, 4}, {8, 1},  {8, 2},  {6, 6},  {-6, 6}, {8, 3},  {5, 7},  {-5, 7},
+    {7, 5},  {-7, 5}, {8, 4},  {6, 7},  {-6, 7}, {7, 6},  {-7, 6}, {8, 5},  {7, 7},  {-7, 7}, {8, 6},  {8, 7},
+};
+
+// One symbol of `cluster` (decode.rs:286-330). Without LZ77 this is m_read_clustered. With it, a pending copy comes
+// before the token read and ignores the pixel's cluster; every symbol, copied or not, is pushed to the window. The
+// pull reads its slot before the push writes: a copy at distance 2^20 reads the slot the push then overwrites.
+template <bool LZ>
+__device__ __forceinline__ uint32_t m_read(MSym& s, MLz& z, uint32_t cluster) {
+  if (!LZ) return m_read_clustered(s, cluster);
+  uint32_t sym;
+  if (z.to_copy) {
+    z.to_copy--;
+    sym = z.win[z.copy_pos++ & kLzMask];
+  } else {
+    const uint32_t tok = m_token(s, cluster);
+    if (tok < z.min_symbol) {
+      sym = m_hybrid(s, __ldg(s.cfg + cluster), tok);
+    } else {
+      if (z.decoded == 0) {  // lz77_repeat
+        z.err = 1;
+        return 0;
+      }
+      const uint32_t n = m_hybrid(s, z.len_cfg, tok - z.min_symbol);
+      if (n > 0xffffffffu - z.min_length) {
+        z.err = 1;
+        return 0;
+      }
+      const uint32_t dsym = m_read_clustered(s, z.dist_cluster);
+      uint32_t d = dsym - 120;  // apply_copy (decode.rs:107-122)
+      if (dsym < 120) {
+        const int64_t v = int64_t(z.mult * uint32_t(c_special_dist[dsym][1])) + c_special_dist[dsym][0] - 1;
+        d = (v < 0 || v > int64_t(0xffffffffu)) ? 0u : uint32_t(v);
+      }
+      const uint32_t distance = min(min(d, kLzMask) + 1u, z.decoded);
+      z.copy_pos = z.decoded - distance;
+      z.to_copy = n + z.min_length - 1;  // the first copied symbol is returned now
+      sym = z.win[z.copy_pos++ & kLzMask];
+    }
+  }
+  z.win[z.decoded++ & kLzMask] = sym;
+  return sym;
+}
 
 __device__ __forceinline__ int32_t m_unpack_signed(uint32_t u) { return int32_t((u >> 1) ^ (((~u) & 1u) - 1u)); }
 __device__ __forceinline__ int32_t wadd(int32_t a, int32_t b) { return int32_t(uint32_t(a) + uint32_t(b)); }
@@ -246,9 +316,10 @@ __device__ __forceinline__ int32_t m_predict32(uint32_t predictor, int32_t L, in
 // One channel whose tree walk is a table over one property (MRectDev::walk == kWalkLut): per pixel the property, one
 // table load (predictor, cluster, leaf), the predictor and the symbol. specialized_trees.rs:197-372 is the CPU form.
 // PROP: the property (2..15), -1 = single leaf, -2 = read from the rect at run time. Pixels with all neighbours inside
-// the channel (y >= 2, 2 <= x < w - 2) skip the edge rules of predict.rs:64-103.
-template <bool WP, int PROP>
-__device__ __forceinline__ void m_channel_lut(const MBatchDev& B, const MRectDev& rc, MSym& sym, MWp& wp, const int4* nodes) {
+// the channel (y >= 2, 2 <= x < w - 2) skip the edge rules of predict.rs:64-103. LZ: the stream's code uses LZ77.
+template <bool WP, int PROP, bool LZ>
+__device__ __forceinline__ void m_channel_lut(const MBatchDev& B, const MRectDev& rc, MSym& sym, MLz& lz, MWp& wp,
+                                              const int4* nodes) {
   const uint32_t w = rc.w, h = rc.h;
   const int prop_rt = int(rc.walk >> 8);
   int32_t* const base = B.planes + rc.base;
@@ -289,7 +360,7 @@ __device__ __forceinline__ void m_channel_lut(const MBatchDev& B, const MRectDev
       }
       prev_p9 = p9;
       const int32_t guess = m_predict32(e & 15u, left, n, nw, ne, ww, nn, nee, wp_pred);
-      const int32_t dec = m_unpack_signed(m_read_clustered(sym, (e >> 4) & 255u));
+      const int32_t dec = m_unpack_signed(m_read<LZ>(sym, lz, (e >> 4) & 255u));
       int32_t val;
       if (e & (1u << 12)) {
         val = wadd(guess, dec);
@@ -347,7 +418,8 @@ __device__ __forceinline__ void m_channel_lut(const MBatchDev& B, const MRectDev
 }  // namespace
 
 // One lane per stream; lanes >= S of a warp idle. Persistent: finished lanes pull the next stream from B.queue.
-template <int S>
+// LZ: every stream of the launch uses LZ77 (the others run without the window code).
+template <int S, bool LZ>
 __global__ void __launch_bounds__(128) k_modular_decode(const MBatchDev B, const uint32_t total_lanes) {
   const uint32_t warp = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (lane >= S) return;
@@ -365,6 +437,16 @@ __global__ void __launch_bounds__(128) k_modular_decode(const MBatchDev B, const
     sym.log_alpha = code.log_alpha;
     sym.ans_state = 0x130000u;
     if (!code.use_prefix) sym.ans_state = sym.br.read(32);  // ans.rs:431
+    MLz lz;
+    if (LZ) {
+      lz.win = B.lz_window + st.lz_window_off;
+      lz.decoded = lz.to_copy = lz.copy_pos = lz.err = 0;
+      lz.mult = st.dist_multiplier;
+      lz.min_symbol = code.lz_min_symbol;
+      lz.min_length = code.lz_min_length;
+      lz.len_cfg = code.lz_len_cfg;
+      lz.dist_cluster = code.lz_dist_cluster;
+    }
     const int4* const nodes = reinterpret_cast<const int4*>(B.blob + st.tree_off);
     const int4 root = __ldg(nodes);
     MWp wp;
@@ -399,14 +481,14 @@ __global__ void __launch_bounds__(128) k_modular_decode(const MBatchDev B, const
       }
       if ((rc.walk & 0xff) == kWalkLut) {
         if (use_wp) {
-          m_channel_lut<true, -2>(B, rc, sym, wp, nodes);
+          m_channel_lut<true, -2, LZ>(B, rc, sym, lz, wp, nodes);
         } else {
           switch (rc.walk >> 8) {  // the property is a compile-time constant of the channel loop
-            case 9: m_channel_lut<false, 9>(B, rc, sym, wp, nodes); break;
-            case 10: m_channel_lut<false, 10>(B, rc, sym, wp, nodes); break;
-            case 13: m_channel_lut<false, 13>(B, rc, sym, wp, nodes); break;
-            case kLutNoProperty: m_channel_lut<false, -1>(B, rc, sym, wp, nodes); break;
-            default: m_channel_lut<false, -2>(B, rc, sym, wp, nodes); break;
+            case 9: m_channel_lut<false, 9, LZ>(B, rc, sym, lz, wp, nodes); break;
+            case 10: m_channel_lut<false, 10, LZ>(B, rc, sym, lz, wp, nodes); break;
+            case 13: m_channel_lut<false, 13, LZ>(B, rc, sym, lz, wp, nodes); break;
+            case kLutNoProperty: m_channel_lut<false, -1, LZ>(B, rc, sym, lz, wp, nodes); break;
+            default: m_channel_lut<false, -2, LZ>(B, rc, sym, lz, wp, nodes); break;
           }
         }
         continue;
@@ -515,7 +597,7 @@ __global__ void __launch_bounds__(128) k_modular_decode(const MBatchDev B, const
             }
           }
           guess += int64_t(nd.y);
-          const int32_t dec = m_unpack_signed(m_read_unsigned(sym, ctx));
+          const int32_t dec = m_unpack_signed(m_read<LZ>(sym, lz, __ldg(sym.cmap + ctx)));
           const int32_t val = int32_t(guess + int64_t(uint32_t(nd.w)) * int64_t(dec));  // decode/common.rs:85
           if (use_wp) wp.update(val, x, y);
           row[x] = val;
@@ -529,7 +611,8 @@ __global__ void __launch_bounds__(128) k_modular_decode(const MBatchDev B, const
       }
     }
     int err = 0;
-    if (sym.br.bitpos > uint64_t(st.sec_len) * 8u) err = JXG_ERR_OUT_OF_BOUNDS;
+    if (LZ && lz.err) err = JXG_ERR_LZ77;
+    else if (sym.br.bitpos > uint64_t(st.sec_len) * 8u) err = JXG_ERR_OUT_OF_BOUNDS;
     else if (!code.use_prefix && sym.ans_state != 0x130000u) err = JXG_ERR_ANS_CHECKSUM;
     B.status[B.order[sidx]] = err;
   }
@@ -686,17 +769,33 @@ __global__ void __launch_bounds__(256) k_modular_store(const MJobDev* jobs, cons
 // ---------------------------------------------------------------------------
 // host-side launchers
 // ---------------------------------------------------------------------------
-int launch_modular_decode(const MBatchDev& B, uint32_t lanes_per_warp, uint32_t num_rct_streams, cudaStream_t stream) {
+template <bool LZ>
+void launch_decode(const MBatchDev& B, uint32_t lanes_per_warp, cudaStream_t stream) {
+  const uint32_t S = lanes_per_warp <= 1 ? 1 : (lanes_per_warp <= 2 ? 2 : 4);
+  const uint32_t warps = (B.num_streams + S - 1) / S;
+  const uint32_t grid = min((warps + 3) / 4, uint32_t(sm_count()) * 8u);
+  const uint32_t total_lanes = grid * 4 * S;
+  if (S == 1) k_modular_decode<1, LZ><<<grid, 128, 0, stream>>>(B, total_lanes);
+  else if (S == 2) k_modular_decode<2, LZ><<<grid, 128, 0, stream>>>(B, total_lanes);
+  else k_modular_decode<4, LZ><<<grid, 128, 0, stream>>>(B, total_lanes);
+}
+
+int launch_modular_decode(const MBatchDev& B, uint32_t num_plain, uint32_t lanes_per_warp, uint32_t num_rct_streams,
+                          cudaStream_t stream) {
   int launches = 0;
-  if (B.num_streams) {
-    cudaMemsetAsync(B.queue, 0, sizeof(uint32_t), stream);
-    const uint32_t S = lanes_per_warp <= 1 ? 1 : (lanes_per_warp <= 2 ? 2 : 4);
-    const uint32_t warps = (B.num_streams + S - 1) / S;
-    const uint32_t grid = min((warps + 3) / 4, uint32_t(sm_count()) * 8u);
-    const uint32_t total_lanes = grid * 4 * S;
-    if (S == 1) k_modular_decode<1><<<grid, 128, 0, stream>>>(B, total_lanes);
-    else if (S == 2) k_modular_decode<2><<<grid, 128, 0, stream>>>(B, total_lanes);
-    else k_modular_decode<4><<<grid, 128, 0, stream>>>(B, total_lanes);
+  if (B.num_streams) cudaMemsetAsync(B.queue, 0, 2 * sizeof(uint32_t), stream);
+  if (num_plain) {
+    MBatchDev P = B;
+    P.num_streams = num_plain;
+    launch_decode<false>(P, lanes_per_warp, stream);
+    launches++;
+  }
+  if (B.num_streams > num_plain) {  // longest first among the LZ77 streams too, with their own queue counter
+    MBatchDev L = B;
+    L.order = B.order + num_plain;
+    L.num_streams = B.num_streams - num_plain;
+    L.queue = B.queue + 1;
+    launch_decode<true>(L, lanes_per_warp, stream);
     launches++;
   }
   if (num_rct_streams) {

@@ -150,6 +150,7 @@ void parse_hf_stream_header(ModularFrameState& ms, ModularGroupStream& st, BitRe
     fail("no global MA tree");
   }
   st.data_bitpos = br.total_bits_read();
+  for (const ModularChannel& c : shapes) st.dist_multiplier = std::max(st.dist_multiplier, c.w);
   br.check();
 }
 

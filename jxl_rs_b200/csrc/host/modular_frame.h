@@ -30,6 +30,7 @@ struct ModularGroupStream {
   std::shared_ptr<ModularTree> local_tree;  // null: global tree
   uint64_t header_bitpos = 0;  // bit offset in the section of the GroupHeader (0 unless the frame has one section)
   uint64_t data_bitpos = 0;    // bit offset in the section of the first entropy-coded bit (ANS state / first symbol)
+  uint32_t dist_multiplier = 0;  // widest channel after the local transforms: LZ77 special distances (bitstream.rs:193-202)
   std::vector<ModularRect> rects;  // in channel order; zero-sized ones keep their index (bitstream.rs:203-206)
 };
 

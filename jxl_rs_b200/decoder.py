@@ -473,6 +473,13 @@ class ModularBatch:
         return {"h2d_bytes": h2d.value, "d2h_bytes": d2h.value, "kernel_launches": launches.value, "device_ms": ms[0],
                 "decode_ms": ms[1]}
 
+    def lz77_stats(self):
+        """Group streams of the added frames that use LZ77, those of them in run-length form (every copy at distance 1),
+        and the device bytes of their symbol windows."""
+        n, rle, win = C.c_uint32(), C.c_uint32(), C.c_uint64()
+        abi.check(self._lib, self._lib.jxg_modular_batch_lz77_stats(self._h, C.byref(n), C.byref(rle), C.byref(win)))
+        return {"lz77_streams": n.value, "rle_streams": rle.value, "window_bytes": win.value}
+
     def read_planes(self, f: int):
         import numpy as np
         fr = self.frames[f]

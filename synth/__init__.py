@@ -34,6 +34,11 @@ def _lib():
         _LIB.jxs_modular_last_error.restype = C.c_char_p
         _LIB.jxs_encode_modular_tokens.restype = C.c_int64
         _LIB.jxs_encode_modular_tokens.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+        _LIB.jxs_encode_modular_lz77.restype = C.c_int64
+        _LIB.jxs_encode_modular_lz77.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                 C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t]
+        _LIB.jxs_modular_lz77_census.argtypes = [C.c_void_p]
+        _LIB.jxs_modular_lz77_census.restype = None
     return _LIB
 
 
@@ -135,12 +140,15 @@ def modular_source(width, height, seed, palette=0):
     return out
 
 
-def encode_modular(width, height, seed, rct=6, squeeze=0, tree_kind=1, source=None, palette=0) -> bytes:
+def encode_modular(width, height, seed, rct=6, squeeze=0, tree_kind=1, source=None, palette=0, lz77=0) -> bytes:
     """One synthetic lossless Modular frame (8-bit RGB, group size 256). rct: 0 or 6 (YCoCg); squeeze: default
     Squeeze transform on/off; tree_kind: 0 single Gradient leaf, 1 property tree, 2 weighted-predictor tree,
     3 tree on properties of the previous channel (17, 19); palette: 1 = global palette transform over the colour
     channels (explicit entries + both implicit colour cubes, no delta entries; rct and squeeze must be 0).
-    source: optional H x W x 3 uint8 array to encode instead of the procedural image."""
+    source: optional H x W x 3 uint8 array to encode instead of the procedural image.
+    lz77: 0 no LZ77; 1 run-length copies in the group streams (every copy at distance 1, the shape libjxl's fastest
+    lossless mode writes); 2 general copies (special distances relative to the stream's widest channel, plain
+    distances, copies across row ends and channels, copies the decoder clamps). lz77_census() describes the copies."""
     lib = _lib()
     src = None
     if source is not None:
@@ -150,13 +158,30 @@ def encode_modular(width, height, seed, rct=6, squeeze=0, tree_kind=1, source=No
         src = source.ctypes.data
     cap = max(1 << 16, width * height * 4)
     buf = C.create_string_buffer(cap)
-    n = lib.jxs_encode_modular_ex(width, height, seed, rct, squeeze, tree_kind, palette, src, buf, cap)
+
+    def run(buf, cap):
+        if lz77:
+            return lib.jxs_encode_modular_lz77(width, height, seed, rct, squeeze, tree_kind, palette, lz77, src, buf, cap)
+        return lib.jxs_encode_modular_ex(width, height, seed, rct, squeeze, tree_kind, palette, src, buf, cap)
+    n = run(buf, cap)
     if n < 0:
         raise RuntimeError("synthetic Modular encode failed: " + lib.jxs_modular_last_error().decode())
     if n > cap:
         buf = C.create_string_buffer(n)
-        n = lib.jxs_encode_modular_ex(width, height, seed, rct, squeeze, tree_kind, palette, src, buf, n)
+        n = run(buf, n)
     return buf.raw[:n]
+
+
+LZ77_CENSUS_KEYS = ("copies", "special", "plain", "cross_channel", "clamped", "max_distance", "max_stream")
+
+
+def lz77_census():
+    """What the last LZ77 encode of this thread wrote (encode_modular with lz77 > 0, encode_modular_tokens with
+    spec["lz77"]): copies, copies with special / plain distances, copies crossing a channel boundary, copies whose
+    distance the decoder clamps to the symbols decoded so far, the longest distance copied from, the longest stream."""
+    out = (C.c_uint64 * 7)()
+    _lib().jxs_modular_lz77_census(out)
+    return dict(zip(LZ77_CENSUS_KEYS, list(out)))
 
 
 def _tree_words(tree):
@@ -197,7 +222,11 @@ def encode_modular_tokens(spec) -> bytes:
       transforms (for the global section: the frame's global transforms) as dicts {"id": 0, "begin", "rct_type"},
       {"id": 1, "begin", "num_c", "num_colors", "num_deltas", "predictor"}, {"id": 2, "squeezes": [(horizontal,
       in_place, begin, num_c), ...]}, and tokens: None (the group header only) or a list of (context, u32 value);
-      with tokens, "tree" is the local tree when use_global_tree is false."""
+      with tokens, "tree" is the local tree when use_global_tree is false.
+    lz77 (optional): a dict with min_symbol (default 224), min_length (3), length (hybrid config of the copy lengths,
+    (0, 0, 0)), mode (1 run-length, 2 general: see encode_modular), multipliers (per section, the widest channel of its
+    stream: the unit of the special distances) and fault (None, or (1, section): that stream starts with a copy,
+    (2, section): its first copy has a length that overflows). The decoded values are those of the token lists."""
     words = [spec["width"], spec["height"], spec.get("group_shift", 1), int(spec.get("grey", 0)),
              spec.get("orientation", 1), int(spec.get("prefix", 0))] + list(spec.get("hybrid", (4, 2, 0)))
     words += _tree_words(spec["tree"])
@@ -217,6 +246,13 @@ def encode_modular_tokens(spec) -> bytes:
             words.append(len(toks))
             for c, v in toks:
                 words += [c, v]
+    lz = spec.get("lz77")
+    if lz:
+        fault = lz.get("fault") or (0, 0)
+        mult = list(lz["multipliers"])
+        assert len(mult) == len(spec["sections"])
+        words += [lz.get("min_symbol", 224), lz.get("min_length", 3)] + list(lz.get("length", (0, 0, 0)))
+        words += [lz["mode"], fault[0], fault[1]] + mult
     lib = _lib()
     arr = (C.c_uint32 * len(words))(*[int(w) & 0xFFFFFFFF for w in words])
     cap = max(1 << 16, 8 * len(words))

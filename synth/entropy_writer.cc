@@ -521,12 +521,24 @@ static AnsCode build_code_syms(size_t num_contexts, const std::vector<uint8_t>& 
   return code;
 }
 
+static const HybridCfg& cluster_cfg(const AnsCode& code, uint32_t c) {
+  return code.lz.enabled && code.lz_dist_own_cfg && c == code.context_map.back() ? code.lz_dist_cfg : code.cfg;
+}
+
 void write_code(BitWriter& bw, const AnsCode& code) {
   if (code.lz.enabled) {  // decode.rs:36-44 + :489-498
     bw.write(1, 1);
-    if (code.lz.min_symbol != 224 || code.lz.min_length != 3) throw std::runtime_error("only min_symbol 224 / min_length 3 are written");
-    bw.u2s_sel(0);  // min_symbol 224
-    bw.u2s_sel(0);  // min_length 3
+    const uint32_t ms = code.lz.min_symbol, ml = code.lz.min_length;
+    if (ms == 224) bw.u2s_sel(0);
+    else if (ms == 512) bw.u2s_sel(1);
+    else if (ms == 4096) bw.u2s_sel(2);
+    else if (ms >= 8 && ms < 8 + (1u << 15)) bw.u2s_sel(3, ms - 8, 15);
+    else throw std::runtime_error("LZ77 min_symbol out of range");
+    if (ml == 3) bw.u2s_sel(0);
+    else if (ml == 4) bw.u2s_sel(1);
+    else if (ml >= 5 && ml < 9) bw.u2s_sel(2, ml - 5, 2);
+    else if (ml >= 9 && ml < 9 + 256) bw.u2s_sel(3, ml - 9, 8);
+    else throw std::runtime_error("LZ77 min_length out of range");
     write_hybrid_cfg(bw, code.lz_len_cfg, 8);
   } else {
     bw.write(0, 1);
@@ -553,7 +565,7 @@ void write_code(BitWriter& bw, const AnsCode& code) {
   }
   if (code.use_prefix) {  // decode.rs:509-524, huffman.rs:466-480
     bw.write(1, 1);
-    for (uint32_t c = 0; c < code.num_clusters; c++) write_hybrid_cfg(bw, code.cfg, 15);
+    for (uint32_t c = 0; c < code.num_clusters; c++) write_hybrid_cfg(bw, cluster_cfg(code, c), 15);
     for (uint32_t c = 0; c < code.num_clusters; c++) write_varint16(bw, uint32_t(code.plen[c].size()) - 1);
     for (uint32_t c = 0; c < code.num_clusters; c++) {
       // a one-symbol code whose symbol is not 0 still needs the simple-code header; plen alone cannot say which
@@ -574,7 +586,7 @@ void write_code(BitWriter& bw, const AnsCode& code) {
   }
   bw.write(0, 1);  // use_prefix_code = 0
   bw.write(code.log_alpha_size - 5, 2);
-  for (uint32_t c = 0; c < code.num_clusters; c++) write_hybrid_cfg(bw, code.cfg, code.log_alpha_size);
+  for (uint32_t c = 0; c < code.num_clusters; c++) write_hybrid_cfg(bw, cluster_cfg(code, c), code.log_alpha_size);
   for (uint32_t c = 0; c < code.num_clusters; c++) write_histogram(bw, code.freqs[c], code.log_alpha_size);
 }
 

@@ -127,6 +127,9 @@ struct AnsCode {
   // as the decoder's table expects them (first bit read = LSB).
   Lz77 lz;
   HybridCfg lz_len_cfg{0, 0, 0};  // hybrid-uint configuration of the copy lengths (8-bit alphabet form, decode.rs:493)
+  // Hybrid-uint configuration of the distance cluster (the last cluster of the context map) when it differs from `cfg`.
+  bool lz_dist_own_cfg = false;
+  HybridCfg lz_dist_cfg{0, 0, 0};
   bool use_prefix = false;
   std::vector<std::vector<uint8_t>> plen;         // [cluster][alphabet]
   std::vector<std::vector<uint16_t>> pbits;       // [cluster][alphabet]

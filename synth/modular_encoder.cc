@@ -4,6 +4,7 @@
 // global transforms RCT (YCoCg) and/or Squeeze (default parameters), and one sub-bitstream per section following
 // the channel -> section rules of modular/mod.rs:353-400. Forward RCT / forward Squeeze are derived here from the
 // decoder definitions (rct.rs:9-40, squeeze.rs:144-195); the round trip "decode == source" is part of the tests.
+#include <algorithm>
 #include <cstring>
 #include <deque>
 #include <stdexcept>
@@ -310,6 +311,123 @@ bool is_meta(const ModularChannel& c) { return c.hshift < 0 || c.vshift < 0; }
 
 }  // namespace
 
+// ---- LZ77 copies in Modular streams ----------------------------------------------------------------------------------
+// A Modular stream reads its copy distances with a multiplier, the widest channel of the stream (bitstream.rs:193-202):
+// a distance symbol k < 120 is the special offset (dx, dy) of entropy_coding/decode.rs:87-101, distance
+// multiplier * dy + dx (at least 1), and k >= 120 the plain distance k - 119. Either is capped at 2^20 and then at the
+// number of symbols decoded so far (decode.rs:107-124). The writer states the rule for the four offsets it uses.
+struct LzCensus {  // what the LZ77 modes wrote (the last encode of this thread): the tests assert reach with it
+  uint64_t copies = 0, special = 0, plain = 0, cross_channel = 0, clamped = 0, max_distance = 0, max_stream = 0;
+};
+thread_local LzCensus g_lz_census;
+
+namespace {
+
+struct SpecialDist {
+  uint32_t sym;
+  int32_t dx, dy;
+};
+constexpr SpecialDist kSpecialUsed[] = {{0, 0, 1}, {1, 1, 0}, {2, 1, 1}, {3, -1, 1}};  // above, left, up-left, up-right
+constexpr uint32_t kWindow = 1u << 20;
+
+struct LzParams {
+  Lz77 lz;
+  HybridCfg cfg, len_cfg{0, 0, 0}, dist_cfg;
+};
+
+Sym literal_sym(const Token& t, const LzParams& P) {
+  Sym s{t.ctx, 0, 0, 0};
+  P.cfg.encode(t.value, s.tok, s.nbits, s.bits);
+  if (s.tok >= P.lz.min_symbol) throw std::runtime_error("literal token collides with the LZ77 range");
+  return s;
+}
+
+// One stream's tokens -> coded symbols with copies. mode 0: literals only; 1: run-length (every copy repeats the
+// previous symbol: special symbol 1, the only symbol of the distance cluster); 2: general (the special offsets above,
+// plain distances 2, 3, 4, 8, 64 and 2^20, copies whose distance the decoder clamps). chan_end: the symbol index where
+// each channel ends. fault 1: the stream starts with a copy; 2: its first copy has a length that overflows u32.
+std::vector<Sym> modular_lz77(const std::vector<Token>& t, const std::vector<size_t>& chan_end, uint32_t mult, uint32_t mode,
+                              const LzParams& P, uint32_t dist_ctx, uint32_t fault, LzCensus& cs) {
+  struct Cand {
+    uint32_t sym, distance;  // distance symbol, distance before the clamp to the decoded count
+    bool special;
+  };
+  std::vector<Cand> cands;
+  if (mode == 1) cands.push_back(Cand{1, 1, true});
+  if (mode == 2) {
+    for (const SpecialDist& sd : kSpecialUsed) {
+      const int64_t d = std::max<int64_t>(int64_t(mult) * sd.dy + sd.dx, 1);
+      cands.push_back(Cand{sd.sym, uint32_t(std::min<int64_t>(d, kWindow)), true});
+    }
+    for (uint32_t d : {2u, 3u, 4u, 8u, 64u, kWindow}) cands.push_back(Cand{120 + d - 1, d, false});
+  }
+  const size_t max_len = mode == 1 ? (size_t(1) << 24) : 4096;
+  const size_t min_len = std::max<size_t>(P.lz.min_length, mode == 1 ? 1 : 4);
+  auto copy = [&](std::vector<Sym>& out, uint32_t ctx, uint64_t len, uint32_t dsym) {
+    Sym l{ctx, 0, 0, 0};
+    P.len_cfg.encode(uint32_t(len - P.lz.min_length), l.tok, l.nbits, l.bits);
+    l.tok += P.lz.min_symbol;
+    out.push_back(l);
+    Sym d{dist_ctx, 0, 0, 0};
+    P.dist_cfg.encode(dsym, d.tok, d.nbits, d.bits);
+    out.push_back(d);
+  };
+  std::vector<Sym> out;
+  out.reserve(t.size());
+  cs.max_stream = std::max<uint64_t>(cs.max_stream, t.size());
+  if (fault == 1 && !t.empty()) copy(out, t[0].ctx, P.lz.min_length, 1);
+  for (size_t i = 0; i < t.size();) {
+    size_t best_len = 0;
+    const Cand* best = nullptr;
+    for (const Cand& c : cands) {
+      const size_t e = std::min<size_t>(c.distance, i);
+      if (e == 0) continue;
+      size_t l = 0;
+      while (i + l < t.size() && l < max_len && t[i + l].value == t[i + l - e].value) l++;
+      if (l > best_len) best_len = l, best = &c;
+    }
+    if (best && best_len >= min_len) {
+      if (fault == 2) {  // the first copy gets a length the decoder must refuse (decode.rs:300-317)
+        fault = 0;
+        Sym l{t[i].ctx, 0, 0, 0};
+        P.len_cfg.encode(0xffffffffu, l.tok, l.nbits, l.bits);
+        l.tok += P.lz.min_symbol;
+        out.push_back(l);
+      }
+      copy(out, t[i].ctx, best_len, best->sym);
+      const size_t e = std::min<size_t>(best->distance, i);
+      cs.copies++;
+      (best->special ? cs.special : cs.plain)++;
+      cs.clamped += best->distance > i;
+      cs.max_distance = std::max<uint64_t>(cs.max_distance, e);
+      const size_t c0 = std::upper_bound(chan_end.begin(), chan_end.end(), i) - chan_end.begin();
+      const size_t c1 = std::upper_bound(chan_end.begin(), chan_end.end(), i + best_len - 1) - chan_end.begin();
+      cs.cross_channel += c0 != c1;
+      i += best_len;
+    } else {
+      out.push_back(literal_sym(t[i], P));
+      i++;
+    }
+  }
+  return out;
+}
+
+// The code of LZ77 streams: contexts [0, nctx) clustered by cmap into nc clusters, then the distance context alone in
+// cluster nc with its own hybrid-uint configuration.
+AnsCode lz_code(std::vector<uint8_t> cmap, uint32_t nc, const std::vector<const std::vector<Sym>*>& streams, bool prefix,
+                const LzParams& P) {
+  if (nc >= 256) throw std::runtime_error("too many clusters for an LZ77 code");
+  cmap.push_back(uint8_t(nc));
+  AnsCode c = build_code_lz77(cmap.size(), cmap, nc + 1, streams, P.lz, prefix);
+  c.cfg = P.cfg;
+  c.lz_len_cfg = P.len_cfg;
+  c.lz_dist_own_cfg = true;
+  c.lz_dist_cfg = P.dist_cfg;
+  return c;
+}
+
+}  // namespace
+
 // Snaps the picture to colours a palette transform without delta entries can carry three ways: the left quarter to the
 // implicit 4x4x4 cube (levels 32, 95, 159, 223), the rest to the levels of the implicit 5x5x5 cube (0, 63, 127, 191, 255).
 void snap_to_palette_colours(uint32_t W, uint32_t H, std::vector<uint8_t>& rgb) {
@@ -323,7 +441,7 @@ void snap_to_palette_colours(uint32_t W, uint32_t H, std::vector<uint8_t>& rgb) 
 }
 
 std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint32_t rct_type, uint32_t squeeze,
-                                    uint32_t tree_kind, const uint8_t* source_rgb, uint32_t palette) {
+                                    uint32_t tree_kind, const uint8_t* source_rgb, uint32_t palette, uint32_t lz77) {
   std::vector<uint8_t> rgb;
   if (source_rgb) rgb.assign(source_rgb, source_rgb + size_t(W) * H * 3);
   else make_image_u8(W, H, seed, rgb);
@@ -452,6 +570,8 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
   };
   std::vector<Token> tok0;
   std::vector<std::vector<Token>> tok_lf(num_lf_groups), tok_hf(num_groups);
+  std::vector<std::vector<size_t>> hf_chan_end(num_groups);
+  std::vector<uint32_t> hf_mult(num_groups, 0);
   {
     std::vector<ModularChannel> c0(ch.begin(), ch.begin() + n0);
     tokenize(c0, 0, tree, uses_wp, tok0);
@@ -467,6 +587,12 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
     for (size_t c = n0; c < ch.size(); c++)
       if (std::min(ch[c].hshift, ch[c].vshift) <= 2) cs.push_back(rect_of(ch[c], group_dim, g % xg, g / xg));
     tokenize(cs, 1 + 3 * uint64_t(num_lf_groups) + 17 + g, tree, uses_wp, tok_hf[g]);
+    size_t end = 0;
+    for (const ModularChannel& c : cs) {
+      hf_mult[g] = std::max(hf_mult[g], c.w);
+      end += size_t(c.w) * c.h;
+      hf_chan_end[g].push_back(end);
+    }
   }
 
   // ---- entropy code over all streams ----
@@ -479,7 +605,33 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
   uint32_t nc;
   HybridCfg cfg;
   std::vector<uint8_t> cmap = cluster_contexts(num_ctx, all, 8, nc, cfg);
-  AnsCode code = build_code(num_ctx, cmap, nc, all);
+  AnsCode code;
+  // lz77 != 0: the group streams carry copies (section 0 and the LF groups only literals, read with the same code)
+  std::vector<Sym> sym0;
+  std::vector<std::vector<Sym>> sym_lf(num_lf_groups), sym_hf(num_groups);
+  if (lz77) {
+    if (lz77 > 2) throw std::runtime_error("lz77 must be 0, 1 or 2");
+    LzParams P;
+    P.lz.enabled = true;
+    P.cfg = cfg;
+    P.dist_cfg = lz77 == 1 ? HybridCfg{0, 0, 0} : cfg;  // run-length: split exponent 0 (Histograms::is_rle)
+    g_lz_census = LzCensus();
+    const uint32_t dctx = uint32_t(num_ctx);
+    sym0 = modular_lz77(tok0, {tok0.size()}, 0, 0, P, dctx, 0, g_lz_census);
+    for (uint32_t g = 0; g < num_lf_groups; g++) sym_lf[g] = modular_lz77(tok_lf[g], {tok_lf[g].size()}, 0, 0, P, dctx, 0, g_lz_census);
+    for (uint32_t g = 0; g < num_groups; g++)
+      sym_hf[g] = modular_lz77(tok_hf[g], hf_chan_end[g], hf_mult[g], lz77, P, dctx, 0, g_lz_census);
+    std::vector<const std::vector<Sym>*> ptrs{&sym0};
+    for (auto& v : sym_lf) ptrs.push_back(&v);
+    for (auto& v : sym_hf) ptrs.push_back(&v);
+    code = lz_code(cmap, nc, ptrs, false, P);
+  } else {
+    code = build_code(num_ctx, cmap, nc, all);
+  }
+  auto write_stream = [&](BitWriter& bw, const std::vector<Token>& toks, const std::vector<Sym>& syms) {
+    if (lz77) write_symbols(bw, code, syms);
+    else write_tokens(bw, code, toks);
+  };
 
   // ---- sections ----
   BitWriter lf_global;
@@ -508,17 +660,17 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
   }
   write_code(lf_global, code);
   write_group_header(lf_global, gh.transforms);
-  if (!tok0.empty()) write_tokens(lf_global, code, tok0);
+  if (!tok0.empty()) write_stream(lf_global, tok0, sym0);
   std::vector<BitWriter> lf_groups(num_lf_groups), hf_groups(num_groups);
   for (uint32_t g = 0; g < num_lf_groups; g++)
     if (!tok_lf[g].empty()) {
       write_group_header(lf_groups[g], {});
-      write_tokens(lf_groups[g], code, tok_lf[g]);
+      write_stream(lf_groups[g], tok_lf[g], sym_lf[g]);
     }
   for (uint32_t g = 0; g < num_groups; g++)
     if (!tok_hf[g].empty()) {
       write_group_header(hf_groups[g], {});
-      write_tokens(hf_groups[g], code, tok_hf[g]);
+      write_stream(hf_groups[g], tok_hf[g], sym_hf[g]);
     }
   BitWriter hf_global;  // empty for Modular frames
 
@@ -755,21 +907,72 @@ std::vector<uint8_t> encode_modular_tokens(const uint32_t* words, size_t nwords)
       s.toks.push_back(Token{ctx, r.next()});
     }
   }
+  // optional LZ77 block: min_symbol, min_length, length hybrid config (3 words), mode, fault kind, fault section, then
+  // one distance multiplier per section
+  const bool lz = r.i != r.n;
+  LzParams P;
+  uint32_t lz_mode = 0, fault = 0, fault_sec = 0;
+  std::vector<uint32_t> mult(nsec, 0);
+  if (lz) {
+    P.lz.enabled = true;
+    P.lz.min_symbol = r.next();
+    P.lz.min_length = r.next();
+    P.len_cfg.split_exponent = r.next();
+    P.len_cfg.msb = r.next();
+    P.len_cfg.lsb = r.next();
+    lz_mode = r.next();
+    fault = r.next();
+    fault_sec = r.next();
+    for (uint32_t& m : mult) m = r.next();
+    if (lz_mode < 1 || lz_mode > 2) throw std::runtime_error("lz77 mode must be 1 or 2");
+    P.cfg = cfg;
+    P.dist_cfg = lz_mode == 1 ? HybridCfg{0, 0, 0} : cfg;
+  }
   if (r.i != r.n) throw std::runtime_error("token description has trailing words");
+  // leaf contexts one cluster each, the distance context after them
+  std::vector<std::vector<Sym>> syms(nsec);
+  auto leaf_map = [](size_t leaves) {
+    if (leaves > 255) throw std::runtime_error("an LZ77 code takes at most 255 leaves");
+    std::vector<uint8_t> m(std::max<size_t>(leaves, 1));
+    for (size_t i = 0; i < m.size(); i++) m[i] = uint8_t(i);
+    return m;
+  };
+  if (lz) {
+    g_lz_census = LzCensus();
+    for (uint32_t i = 0; i < nsec; i++) {
+      if (secs[i].kind != 2) continue;
+      const size_t dctx = std::max<size_t>(secs[i].use_global ? global.leaves : secs[i].local.leaves, 1);
+      syms[i] = modular_lz77(secs[i].toks, {secs[i].toks.size()}, mult[i], lz_mode, P, uint32_t(dctx),
+                             fault && i == fault_sec ? fault : 0, g_lz_census);
+    }
+  }
 
   // the global code covers every section that uses the global tree
   std::vector<const std::vector<Token>*> gstreams;
-  for (const Section& s : secs)
-    if (s.kind == 2 && s.use_global) gstreams.push_back(&s.toks);
-  const AnsCode gcode = leaf_code(global.leaves, gstreams, prefix, cfg);
-  auto section_bits = [&](Section& s, BitWriter& out) {
+  std::vector<const std::vector<Sym>*> gsyms;
+  for (uint32_t i = 0; i < nsec; i++)
+    if (secs[i].kind == 2 && secs[i].use_global) {
+      gstreams.push_back(&secs[i].toks);
+      gsyms.push_back(&syms[i]);
+    }
+  const AnsCode gcode = lz ? lz_code(leaf_map(global.leaves), uint32_t(leaf_map(global.leaves).size()), gsyms, prefix, P)
+                           : leaf_code(global.leaves, gstreams, prefix, cfg);
+  auto section_bits = [&](uint32_t i, BitWriter& out) {
+    Section& s = secs[i];
     if (s.kind == 0) return;
     append_bits(out, s.header);
     if (s.kind < 2) return;
     if (s.use_global) {
-      write_tokens(out, gcode, s.toks);
+      if (lz) write_symbols(out, gcode, syms[i]);
+      else write_tokens(out, gcode, s.toks);
     } else {
       write_tok_tree(out, s.local);
+      if (lz) {
+        const AnsCode lcode = lz_code(leaf_map(s.local.leaves), uint32_t(leaf_map(s.local.leaves).size()), {&syms[i]}, prefix, P);
+        write_code(out, lcode);
+        write_symbols(out, lcode, syms[i]);
+        return;
+      }
       const AnsCode lcode = leaf_code(s.local.leaves, {&s.toks}, prefix, cfg);
       write_code(out, lcode);
       write_tokens(out, lcode, s.toks);
@@ -787,9 +990,9 @@ std::vector<uint8_t> encode_modular_tokens(const uint32_t* words, size_t nwords)
   lf_global.write(1, 1);  // global tree present
   write_tok_tree(lf_global, global);
   write_code(lf_global, gcode);
-  section_bits(secs[0], lf_global);
+  section_bits(0, lf_global);
   std::vector<BitWriter> groups(nsec - 1);
-  for (uint32_t i = 1; i < nsec; i++) section_bits(secs[i], groups[i - 1]);
+  for (uint32_t i = 1; i < nsec; i++) section_bits(i, groups[i - 1]);
 
   BitWriter out;
   out.write(0xff, 8);
@@ -912,7 +1115,7 @@ int jxs_modular_source(uint32_t width, uint32_t height, uint64_t seed, uint8_t* 
 int64_t jxs_encode_modular(uint32_t width, uint32_t height, uint64_t seed, uint32_t rct, uint32_t squeeze,
                            uint32_t tree_kind, const uint8_t* source_rgb, uint8_t* out, size_t cap) {
   try {
-    std::vector<uint8_t> b = jxs::encode_modular(width, height, seed, rct, squeeze, tree_kind, source_rgb, 0);
+    std::vector<uint8_t> b = jxs::encode_modular(width, height, seed, rct, squeeze, tree_kind, source_rgb, 0, 0);
     if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
     return int64_t(b.size());
   } catch (std::exception& e) {
@@ -926,13 +1129,35 @@ int64_t jxs_encode_modular(uint32_t width, uint32_t height, uint64_t seed, uint3
 int64_t jxs_encode_modular_ex(uint32_t width, uint32_t height, uint64_t seed, uint32_t rct, uint32_t squeeze,
                               uint32_t tree_kind, uint32_t palette, const uint8_t* source_rgb, uint8_t* out, size_t cap) {
   try {
-    std::vector<uint8_t> b = jxs::encode_modular(width, height, seed, rct, squeeze, tree_kind, source_rgb, palette);
+    std::vector<uint8_t> b = jxs::encode_modular(width, height, seed, rct, squeeze, tree_kind, source_rgb, palette, 0);
     if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
     return int64_t(b.size());
   } catch (std::exception& e) {
     g_merr = e.what();
     return -1;
   }
+}
+
+// lz77: 1 = run-length copies (distance 1 only, the distance cluster a single symbol), 2 = general copies.
+int64_t jxs_encode_modular_lz77(uint32_t width, uint32_t height, uint64_t seed, uint32_t rct, uint32_t squeeze,
+                                uint32_t tree_kind, uint32_t palette, uint32_t lz77, const uint8_t* source_rgb, uint8_t* out,
+                                size_t cap) {
+  try {
+    std::vector<uint8_t> b = jxs::encode_modular(width, height, seed, rct, squeeze, tree_kind, source_rgb, palette, lz77);
+    if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
+    return int64_t(b.size());
+  } catch (std::exception& e) {
+    g_merr = e.what();
+    return -1;
+  }
+}
+
+// The census of the last LZ77 encode of this thread: copies, special distances, plain distances, copies crossing a
+// channel boundary, copies the decoder clamps, the longest distance, the longest stream (symbols).
+void jxs_modular_lz77_census(uint64_t* out) {
+  const jxs::LzCensus& c = jxs::g_lz_census;
+  const uint64_t v[7] = {c.copies, c.special, c.plain, c.cross_channel, c.clamped, c.max_distance, c.max_stream};
+  memcpy(out, v, sizeof(v));
 }
 
 // The token-level writer (encode_modular_tokens above): `words` is the flat frame description.
