@@ -263,7 +263,10 @@ int jxg_parsed_desc(void* parsed, uint32_t output_format, JxgFrameDesc* desc, co
  * in device memory: min(2^20, pixels) x 4 bytes per LZ77 stream). Delta palettes return JXG_ERR_UNSUPPORTED (no CPU
  * fallback). A group stream that fails (ANS checksum, over-read, an LZ77 copy before any symbol or a copy length
  * overflow: JXG_ERR_LZ77) is reported by jxg_modular_batch_wait; the other streams still decode. Output: interleaved
- * RGB u8 (grey replicated). */
+ * RGB u8 (grey replicated). Frames of one batch must agree on the kind of each inverse-transform step they share: one
+ * frame's step list may be a prefix of another's, in either order of adding. A frame jxg_modular_batch_add refuses
+ * leaves the batch as it was (no stream of it decodes, no statistic counts it); a group-local Squeeze is refused with
+ * JXG_ERR_UNSUPPORTED. */
 int jxg_modular_parse_file(const uint8_t* data, size_t size, void** parsed, JxgImageInfo* info);
 void jxg_modular_parsed_free(void* parsed);
 int jxg_modular_batch_begin(void* ctx, void** batch);

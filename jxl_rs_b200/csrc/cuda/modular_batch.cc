@@ -201,6 +201,44 @@ bool build_walk_table(const jxg::ModularTree& t, uint32_t root, uint32_t ci, uin
   return true;
 }
 
+// Everything add_frame appends to, so that a refused frame leaves the batch as it was (jxg_modular_batch_add).
+struct BatchMark {
+  size_t frames, streams, rct_streams, rects, codes, rcts, refs, levels, store_jobs, blob, blob_pending;
+  std::vector<size_t> level_jobs;
+  uint64_t arena_elems, wp_bytes, out_bytes, lz_window_elems;
+  uint32_t lz77_streams, rle_streams;
+
+  explicit BatchMark(const ModularBatch* b)
+      : frames(b->frames.size()), streams(b->streams.size()), rct_streams(b->rct_streams.size()), rects(b->rects.size()),
+        codes(b->codes.size()), rcts(b->rcts.size()), refs(b->refs.size()), levels(b->levels.size()),
+        store_jobs(b->store_jobs.size()), blob(b->ctx->blob.size), blob_pending(b->ctx->blob.pending.size()),
+        arena_elems(b->arena_elems), wp_bytes(b->wp_bytes), out_bytes(b->out_bytes), lz_window_elems(b->lz_window_elems),
+        lz77_streams(b->lz77_streams), rle_streams(b->rle_streams) {
+    for (const auto& l : b->levels) level_jobs.push_back(l.size());
+  }
+  void restore(ModularBatch* b) const {
+    b->frames.resize(frames);
+    b->streams.resize(streams);
+    b->rct_streams.resize(rct_streams);
+    b->rects.resize(rects);
+    b->codes.resize(codes);
+    b->rcts.resize(rcts);
+    b->refs.resize(refs);
+    b->levels.resize(levels);
+    b->level_kind.resize(levels);
+    for (size_t l = 0; l < levels; l++) b->levels[l].resize(level_jobs[l]);
+    b->store_jobs.resize(store_jobs);
+    b->ctx->blob.size = blob;
+    b->ctx->blob.pending.resize(blob_pending);
+    b->arena_elems = arena_elems;
+    b->wp_bytes = wp_bytes;
+    b->out_bytes = out_bytes;
+    b->lz_window_elems = lz_window_elems;
+    b->lz77_streams = lz77_streams;
+    b->rle_streams = rle_streams;
+  }
+};
+
 void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t stride, bool is_device) {
   if (!ms->device_plan_ok)
     throw jxg::Error(JXG_ERR_UNSUPPORTED, "palette transforms with delta entries or a predictor are not implemented on the device path");
@@ -374,8 +412,8 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t st
     }
     b->levels[si].push_back(j);
   }
-  if (ms->steps.size() < b->levels.size() && !b->frames.empty())
-    throw jxg::Error(JXG_ERR_UNSUPPORTED, "frames of one Modular batch must share the global transform structure");
+  // A frame with fewer steps than the batch has levels has no jobs in the last ones; levels are launched in order and
+  // the store runs after all of them, so only the kinds of the common steps must agree, whatever the order of adding.
   MJobDev sj;
   memset(&sj, 0, sizeof(sj));
   const uint32_t nc = ms->num_color_channels;
@@ -511,10 +549,12 @@ int jxg_modular_batch_add(void* bp, void* parsed, void* out, size_t out_row_stri
   ModularBatch* b = static_cast<ModularBatch*>(bp);
   if (!b || !parsed || !out) return JXG_ERR_ARGUMENT;
   if (b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch already submitted");
+  const BatchMark mark(b);
   try {
     add_frame(b, static_cast<jxg::ModularFrameState*>(parsed), out, out_row_stride, out_is_device != 0);
     return JXG_OK;
   } catch (jxg::Error& e) {
+    mark.restore(b);  // a refused frame leaves nothing behind: no streams decode for it, no stats count it
     return set_error(e.code, e.what());
   }
 }

@@ -865,10 +865,10 @@ void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint3
   if (kind == 0) {
     const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sm_count()) * 16));
     k_modular_rct<<<dim3(max(gx, 1u), num_jobs), 256, 0, stream>>>(jobs, planes);
-  } else if (kind == 1) {
-    k_unsqueeze_h<<<dim3((max_h + 127) / 128, num_jobs), 128, 0, stream>>>(jobs, planes);
+  } else if (kind == 1) {  // a level can hold only empty channels (a squeeze of a zero-height residual): one idle block
+    k_unsqueeze_h<<<dim3(max((max_h + 127) / 128, 1u), num_jobs), 128, 0, stream>>>(jobs, planes);
   } else if (kind == 2) {
-    k_unsqueeze_v<<<dim3((max_w + 127) / 128, num_jobs), 128, 0, stream>>>(jobs, planes);
+    k_unsqueeze_v<<<dim3(max((max_w + 127) / 128, 1u), num_jobs), 128, 0, stream>>>(jobs, planes);
   } else if (kind == 4) {
     const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sm_count()) * 16));
     k_modular_palette<<<dim3(max(gx, 1u), num_jobs), 256, 0, stream>>>(jobs, planes);

@@ -1155,6 +1155,8 @@ void meta_apply_transforms(std::vector<ModularChannel>& ch, uint32_t& nb_meta, G
         for (size_t c = b; c < e; c++) {
           ModularChannel& in = ch[c];
           ModularChannel res;
+          // meta_apply.rs:111-113: a channel shifted by more than 30 in either direction takes no further squeeze
+          if (in.hshift > 30 || in.vshift > 30) fail("too many squeezes");
           if (s.horizontal) {
             uint32_t w = in.w;
             in.w = (w + 1) / 2;

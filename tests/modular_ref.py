@@ -1,7 +1,9 @@
-"""Plain-integer restatement of the reference's Modular decode (jxl/src/frame/modular), for lossless 8-bit frames
-without Squeeze: MA trees, properties, the 14 predictors, the weighted predictor, make_pixel, group-local and global
-RCT, the global palette without delta entries (get_palette_value, with the delta table of
-tests/golden/modular_delta_palette.json), the channel -> section rules and the i32 -> u8 store. Written from the reference text (line numbers
+"""Plain-integer restatement of the reference's Modular decode (jxl/src/frame/modular), for lossless 8-bit frames:
+MA trees, properties, the 14 predictors, the weighted predictor, make_pixel, group-local and global RCT, the global
+palette without delta entries (get_palette_value, with the delta table of tests/golden/modular_delta_palette.json),
+global and group-local Squeeze (default and explicit steps, meta channels; the scalar unsqueeze, and separately the
+i32 lane form), the channel -> section rules for any channel list (global section, ModularLF and ModularHF streams)
+and the i32 -> u8 store. Written from the reference text (line numbers
 below) with Python ints and explicit wrap32 / wrap64; it shares no code with the front-end (csrc/host/modular.cc)
 or the synthetic writer.
 
@@ -88,8 +90,11 @@ def link_tree(tree, check=True):
 
 
 def _refuse(check, what):
-    if check:
+    """check: True raises, a list (a frame written with check=False) collects the refusal, False ignores it."""
+    if check is True:
         raise TreeRefused(what)
+    if isinstance(check, list):
+        check.append(what)
 
 
 def validate_tree(nodes, num_properties):
@@ -280,9 +285,18 @@ def make_pixel(dec, mul, guess):
 # ---------------------------------------------------------------------------------------------------------------------
 class Coverage:
     """What a run reached: pixels per predictor, (property, branch) pairs, offset / multiplier leaves, wrapped
-    make_pixel results, RCT types."""
+    make_pixel results, RCT types; for Squeeze: (tendency branch, clamp, fired) triples, tail columns / rows ("h" /
+    "v"), zero-width / zero-height residuals, in_place = false and meta squeezes, the default rules that fired,
+    (section kind, shift) pairs of the coded channels, and outputs the `as i32` of unsqueeze wrapped."""
+
+    SQUEEZE_SETS = ("tendency", "tails", "empty_residuals", "default_rules", "sections")
 
     def __init__(self):
+        for k in self.SQUEEZE_SETS:
+            setattr(self, k, set())
+        self.not_in_place = 0
+        self.meta_squeezes = 0
+        self.squeeze_wrapped = 0
         self.predictors = set()
         self.branches = set()
         self.offset_leaves = 0
@@ -305,6 +319,11 @@ class Coverage:
         self.ref_slots |= o.ref_slots
         self.palette |= o.palette
         self.wrapped_props |= o.wrapped_props
+        for k in self.SQUEEZE_SETS:
+            getattr(self, k).update(getattr(o, k))
+        self.not_in_place += o.not_in_place
+        self.meta_squeezes += o.meta_squeezes
+        self.squeeze_wrapped += o.squeeze_wrapped
 
 
 def decode_channels(chans, stream_id, tree, wp_hdr, chooser, cov, faults=()):
@@ -328,7 +347,8 @@ def decode_channels(chans, stream_id, tree, wp_hdr, chooser, cov, faults=()):
         props[0], props[1] = ci, stream_id
         # precompute_references (common.rs:40-82): earlier channels of the same size and shift, nearest first
         order = range(ci - 1, -1, -1) if "refs_farthest_first" not in faults else range(ci)
-        refs = [chans[j] for j in order if (chans[j]["w"], chans[j]["h"], chans[j]["shift"]) == (w, h, ch["shift"])]
+        key = (lambda o: (o["w"], o["h"])) if "refs_size_only" in faults else (lambda o: (o["w"], o["h"], o["shift"]))
+        refs = [chans[j] for j in order if key(chans[j]) == key(ch)]
         refs = refs[:num_ref // 4]
         for y in range(h):
             row, top, toptop = ch["data"][y], ch["data"][y - 1] if y else None, ch["data"][y - 2] if y > 1 else None
@@ -499,6 +519,211 @@ def inverse_palette(pal, index_plane, num_colors, num_c, cov, faults=()):
     return out
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# Squeeze (transforms/squeeze.rs, the squeeze arm of meta_apply.rs:90-180)
+# ---------------------------------------------------------------------------------------------------------------------
+MAX_FIRST_PREVIEW_SIZE = 8
+
+
+def is_meta(ch):
+    return ch["shift"] is None
+
+
+def default_squeeze(chans, cov, faults=()):
+    """squeeze.rs:39-105: the 4:2:0 preview steps when the two channels after the first non-meta one have its size,
+    a vertical step first on tall images, then alternating steps until the first channel is at most 8 x 8."""
+    nm = 0
+    while nm < len(chans) and is_meta(chans[nm]):
+        nm += 1
+    w, h = chans[nm]["w"], chans[nm]["h"]
+    nc = len(chans) - nm
+    params = []
+    preview = nc >= 2 if "preview_nc2" in faults else nc > 2
+    if preview and (chans[nm + 1]["w"], chans[nm + 1]["h"]) == (w, h):
+        cov.default_rules.add("preview420")
+        if w > 1:
+            params.append((True, False, nm + 1, 2))
+        if h > 1:
+            params.append((False, False, nm + 1, 2))
+    if w <= h and h > MAX_FIRST_PREVIEW_SIZE and "no_vertical_first" not in faults:
+        cov.default_rules.add("vertical_first")
+        params.append((False, True, nm, nc))
+        h = -(-h // 2)
+    while w > MAX_FIRST_PREVIEW_SIZE or h > MAX_FIRST_PREVIEW_SIZE:
+        cov.default_rules.add("alternating")
+        if w > MAX_FIRST_PREVIEW_SIZE:
+            params.append((True, True, nm, nc))
+            w = -(-w // 2)
+        if h > MAX_FIRST_PREVIEW_SIZE:
+            params.append((False, True, nm, nc))
+            h = -(-h // 2)
+    return params
+
+
+def meta_apply_squeeze(chans, steps, cov, check=True, faults=()):
+    """The squeeze arm of meta_apply_single_transform on a channel list ({"w", "h", "shift": (hshift, vshift) or None
+    for meta channels}), in place: check_squeeze_params (squeeze.rs:17-37), TooManySqueezes (meta_apply.rs:111-113),
+    the averages in place of their channels and the residuals after the range (in_place) or at the end. Returns the
+    steps applied (default_squeeze's list for an empty one). check=False applies what it can of a refused step, so that
+    the frame can still be written."""
+    if not steps:
+        steps = default_squeeze(chans, cov, faults)
+    applied = []
+    for hz, in_place, b, n in steps:
+        e = b + n
+        if n == 0 or e > len(chans):
+            _refuse(check, "InvalidChannelRange")
+            continue
+        if is_meta(chans[b]) != is_meta(chans[e - 1]):
+            _refuse(check, "MixingDifferentChannels")
+        if is_meta(chans[b]) and not in_place:
+            _refuse(check, "MetaSqueezeRequiresInPlace")
+        if is_meta(chans[b]):
+            cov.meta_squeezes += 1
+        if not in_place:
+            cov.not_in_place += 1
+        off = e if in_place else len(chans)
+        for ic in range(n):
+            ch = chans[b + ic]
+            sh = ch["shift"]
+            if sh is not None and (sh[0] > 30 or sh[1] > 30):
+                _refuse(check, "TooManySqueezes")
+            new = None if sh is None else (sh[0] + 1, sh[1]) if hz else (sh[0], sh[1] + 1)
+            w, h = ch["w"], ch["h"]
+            if hz:
+                avg, res = (-(-w // 2), h), (w - -(-w // 2), h)
+            else:
+                avg, res = (w, -(-h // 2)), (w, h - -(-h // 2))
+            chans[b + ic] = {"w": avg[0], "h": avg[1], "shift": new}
+            rshift = sh if "residual_shift_kept" in faults else new
+            chans.insert(off + ic, {"w": res[0], "h": res[1], "shift": rshift})
+        applied.append((hz, in_place, b, n))
+    return applied
+
+
+def smooth_tendency(b, a, n, cov=None, faults=()):
+    """smooth_tendency_scalar (squeeze.rs:143-168) in exact integers: b the output left of / above the pair, a its
+    average, n the next average. Records (branch, clamp, fired) in cov.tendency."""
+    if b >= a >= n:
+        branch = "increasing"
+        diff = tdiv(4 * b - 3 * n - a + (5 if "tendency_plus5" in faults else 6), 12)
+        clamps = ((lambda d: d - (d & 1) > 2 * (b - a), 2 * (b - a) + 1), (lambda d: d + (d & 1) > 2 * (a - n), 2 * (a - n)))
+    elif b <= a <= n:
+        branch = "decreasing"
+        diff = tdiv(4 * b - 3 * n - a - 6, 12)
+        clamps = ((lambda d: d + (d & 1) < 2 * (b - a), 2 * (b - a) - 1), (lambda d: d - (d & 1) < 2 * (a - n), 2 * (a - n)))
+    else:
+        if cov is not None:
+            cov.tendency.add(("none", None, None))
+        return 0
+    order = (1, 0) if "clamps_swapped" in faults else (0, 1)
+    for k in order:
+        fired = clamps[k][0](diff)
+        if cov is not None:
+            cov.tendency.add((branch, k, fired))
+        if fired:
+            diff = clamps[k][1]
+    return diff
+
+
+def unsqueeze(avg, res, nxt, prev, cov=None, faults=()):
+    """unsqueeze_scalar (squeeze.rs:187-194): i64 arithmetic, `diff / 2` truncating toward zero, `as i32` at the end."""
+    diff = res + smooth_tendency(prev, avg, nxt, cov, faults)
+    a = avg + (diff // 2 if "diff_floor" in faults else tdiv(diff, 2))
+    b = a - diff
+    wa, wb = wrap32(a), wrap32(b)
+    if cov is not None and (wa != a or wb != b):
+        cov.squeeze_wrapped += 1
+    return wa, wb
+
+
+def unsqueeze_line(avg, res, cov=None, faults=()):
+    """One row of hsqueeze_scalar (squeeze.rs:389-439) or one column of vsqueeze_scalar (576-644) over a whole channel:
+    pairs from (avg[x], res[x]) with the next average avg[x + 1] (its own average at the end) and the previous output,
+    then the tail avg[-1] when the output length is odd; a channel without residuals is its average
+    (do_hsqueeze_step / do_vsqueeze_step shortcuts)."""
+    n = len(avg) + len(res)
+    if n == 0:
+        return []
+    if not res:
+        return [avg[0]]
+    out = [0] * n
+    prev = avg[0]
+    for x in range(len(res)):
+        a, prev = unsqueeze(avg[x], res[x], avg[x + 1] if x + 1 < len(avg) else avg[x], prev, cov, faults)
+        out[2 * x], out[2 * x + 1] = a, prev
+    if n & 1:
+        out[n - 1] = avg[-1]
+    return out
+
+
+def inverse_squeeze(avg, res, horizontal, cov, faults=()):
+    """avg, res: lists of rows. Returns the output rows."""
+    h, aw = len(avg), len(avg[0]) if avg else 0
+    if horizontal:
+        rw = len(res[0]) if res else 0
+        if rw == 0:
+            cov.empty_residuals.add("h")
+        out = [unsqueeze_line(avg[y], res[y] if rw else [], cov, faults) for y in range(h)]
+        if (aw + rw) & 1 and rw:
+            cov.tails.add("h")
+            if "tail_wrong_row" in faults:
+                for y in range(1, h):
+                    out[y][-1] = avg[y - 1][-1]
+        return out
+    rh = len(res)
+    if rh == 0:
+        cov.empty_residuals.add("v")
+    cols = [unsqueeze_line([r[x] for r in avg], [r[x] for r in res], cov, faults) for x in range(aw)]
+    out = [[c[y] for c in cols] for y in range(h + rh)]
+    if (h + rh) & 1 and rh:
+        cov.tails.add("v")
+        if "tail_wrong_row" in faults and h >= 2:
+            out[-1] = list(avg[h - 2])
+    return out
+
+
+def undo_squeeze(data, steps, cov, faults=()):
+    """The inverse of meta_apply_squeeze on a list of channel planes (lists of rows), last step first."""
+    for hz, in_place, b, n in reversed(steps):
+        e = b + n
+        off = e if in_place else len(data) - n
+        for ic in range(n):
+            r = off + (n - 1 - ic if "late_offset" in faults and not in_place else ic)
+            data[b + ic] = inverse_squeeze(data[b + ic], data[r], hz, cov, faults)
+        del data[off:off + n]
+
+
+def smooth_tendency_lane(a, b, c):
+    """smooth_tendency_impl (squeeze.rs:107-141) on one Wrapping<i32> lane (jxl_simd scalar.rs): a the previous
+    output, b the average, c the next average; mul_wide_take_high(x, 0x55555556) is (x * 0x55555556) >> 32 in i64,
+    abs wraps at i32::MIN, shr! is arithmetic."""
+    a_b, b_c, a_c = wrap32(a - b), wrap32(b - c), wrap32(a - c)
+    abs_a_b, abs_b_c, abs_a_c = wrap32(abs(a_b)), wrap32(abs(b_c)), wrap32(abs(a_c))
+    non_monotonic = (a_b ^ b_c) < 0
+    skip = a_b != 0 and non_monotonic
+    skip = b_c != 0 and skip
+    abs_a_b_3 = wrap32((abs_a_b * 0x55555556) >> 32)
+    x = wrap32(2 + abs_a_c + abs_a_b_3) >> 2
+    abs_a_b_2_add_x = wrap32(wrap32(abs_a_b << 1) + (x & 1))
+    if x > abs_a_b_2_add_x:
+        x = wrap32(wrap32(abs_a_b << 1) + 1)
+    abs_b_c_2 = wrap32(abs_b_c << 1)
+    if wrap32(x + (x & 1)) > abs_b_c_2:
+        x = abs_b_c_2
+    if skip:
+        x = 0
+    return wrap32(-x) if a_c < 0 else x
+
+
+def unsqueeze_lane(avg, res, nxt, prev):
+    """unsqueeze_impl (squeeze.rs:170-185) on one lane, every operation wrapping."""
+    diff = wrap32(res + smooth_tendency_lane(prev, avg, nxt))
+    sign = (diff & 0xFFFFFFFF) >> 31
+    a = wrap32(avg + (wrap32(diff + sign) >> 1))
+    return a, wrap32(a - diff)
+
+
 def store_u8(planes):
     """convert.rs ConvertI32ToU8 at bit depth 8: clamp to [0, 255]; grey is replicated into R, G and B."""
     p = np.array(planes, dtype=np.int64)
@@ -526,105 +751,199 @@ def section_layout(w, h, group_shift, nc):
     return n0, rects, n_lf
 
 
+def grid_rect(ch, dim, gx, gy):
+    """get_grid_rect (mod.rs:150-190) of a coded channel in the grid of `dim` image pixels: cells of
+    (dim >> hshift) x (dim >> vshift) channel pixels; (x0, y0, w, h), empty past the channel's edge."""
+    gw, gh = dim >> ch["shift"][0], dim >> ch["shift"][1]
+    bx, by = gx * gw, gy * gh
+    if gw == 0 or gh == 0 or bx >= ch["w"] or by >= ch["h"]:
+        return (0, 0, 0, 0)
+    return (bx, by, min(ch["w"] - bx, gw), min(ch["h"] - by, gh))
+
+
+def channel_sections(chans, w, h, group_shift, faults=()):
+    """The channel -> section rules (mod.rs:341-407, one pass) for any coded channel list: the leading "meta or small"
+    channels go to the global section; of the rest, channels with min(hshift, vshift) >= 3 to the ModularLF stream of
+    each LF group (stream id 1 + num_lf_groups + g, rects of lf_group_dim >> shift), channels with shift 0..2 to the
+    ModularHF stream of each group (rects of group_dim >> shift); meta channels after the first big one go nowhere.
+    Returns (n0, [(stream id, [(channel, rect)])] per LF group, the same per HF group)."""
+    gd = 128 << group_shift
+    lfd = gd * 8
+    n0 = 0
+    while n0 < len(chans) and (is_meta(chans[n0]) or (chans[n0]["w"] <= gd and chans[n0]["h"] <= gd)):
+        n0 += 1
+    rest = [i for i in range(n0, len(chans)) if not is_meta(chans[i])]
+    xl, yl = -(-w // lfd), -(-h // lfd)
+    xg, yg = -(-w // gd), -(-h // gd)
+    n_lf = xl * yl
+    lf = []
+    for g in range(n_lf):
+        sid = 1 + n_lf + g + (1 if "lf_stream_id_plus1" in faults else 0)
+        lf.append((sid, [(i, grid_rect(chans[i], lfd, g % xl, g // xl)) for i in rest if min(chans[i]["shift"]) >= 3]))
+    hf = []
+    for g in range(xg * yg):
+        hf.append((1 + 3 * n_lf + 17 + g,
+                   [(i, grid_rect(chans[i], gd, g % xg, g // xg)) for i in rest if min(chans[i]["shift"]) <= 2]))
+    return n0, lf, hf
+
+
 class Frame:
     """A token-level frame: geometry, global tree and transforms, one description per HF group (WeightedHeader, local
-    RCTs, local tree). `decode(chooser)` decodes forward and fills .spec (for synth.encode_modular_tokens), .planes
-    (the i32 planes before the u8 store, as coded), .u8 (oriented) and .cov.
-    palette: None or (num_colors, index_chooser[, begin, num_c]): a global palette transform without delta entries
-    and with the Zero predictor (the form the device decodes); the palette meta channel takes `chooser`, the index
-    channel `index_chooser`."""
+    transforms, local tree). `decode(chooser)` decodes forward and fills .spec (for synth.encode_modular_tokens),
+    .planes (the i32 planes before the u8 store, as coded), .u8 (oriented), .cov and .stream_widths (per section, the
+    widest channel of its stream: the LZ77 distance multiplier).
+    transforms: the global transforms in header order, ("rct", begin, type), ("palette", begin, num_c, num_colors)
+    (no delta entries, the Zero predictor: the form the device decodes) or ("squeeze", [(horizontal, in_place, begin,
+    num_c), ...]) with [] for the default steps. Without it: `palette` then `global_rct` [(begin, type)].
+    palette: None or (num_colors, index_chooser[, begin, num_c]): meta channels take `chooser`, the other channels
+    `index_chooser`. groups: group index -> {"wp", "rct": [(begin, type)] or "transforms" (RCT and Squeeze, as above),
+    "tree" (local tree or None)}."""
 
     def __init__(self, w, h, tree, group_shift=1, grey=False, orientation=1, prefix=False, hybrid=(4, 2, 0),
-                 global_rct=(), global_wp=None, groups=None, faults=(), check=True, palette=None):
+                 global_rct=(), global_wp=None, groups=None, faults=(), check=True, palette=None, transforms=None):
         self.w, self.h, self.tree, self.group_shift, self.grey = w, h, tree, group_shift, grey
         self.orientation, self.prefix, self.hybrid = orientation, prefix, hybrid
-        self.global_rct = list(global_rct)  # [(begin, type)], applied after the palette
+        self.global_rct = list(global_rct)
         self.global_wp = global_wp
-        self.groups = groups or {}  # group index -> {"wp", "rct": [(begin, type)], "tree" (local tree or None)}
+        self.groups = groups or {}
         self.faults = faults
         self.check = check  # False: write what a decoder must refuse (trees, transform ranges) instead of raising
         self.palette = palette
+        self.transforms = transforms
+
+    def _global_transforms(self, nc):
+        if self.transforms is not None:
+            return list(self.transforms)
+        out = []
+        if self.palette:
+            pb, pn = (self.palette[2], self.palette[3]) if len(self.palette) > 2 else (0, nc)
+            out.append(("palette", pb, pn, self.palette[0]))
+        return out + [("rct", b, t) for b, t in self.global_rct]
+
+    def _meta_apply(self, chans, transforms, cov):
+        """meta_apply_single_transform for each transform; returns (applied transforms, spec dicts)."""
+        applied, spec = [], []
+        for t in transforms:
+            if t[0] == "rct":
+                spec.append({"id": 0, "begin": t[1], "rct_type": t[2]})
+                if t[2] >= 42:  # headers/modular.rs: rct_type < 42
+                    _refuse(self._chk, "InvalidRct")
+                _check_equal_channels(chans, t[1], 3, self._chk)
+                applied.append(t)
+            elif t[0] == "palette":
+                _, b, n, ncol = t
+                spec.append({"id": 1, "begin": b, "num_c": n, "num_colors": ncol, "num_deltas": 0, "predictor": 0})
+                _check_equal_channels(chans, b, n, self._chk)
+                info = chans[min(b, len(chans) - 1)]
+                del chans[b + 1:b + n]
+                chans.insert(0, {"w": ncol, "h": n, "shift": None})
+                if b + 1 < len(chans):
+                    chans[b + 1] = dict(info)
+                applied.append(t)
+            else:
+                spec.append({"id": 2, "squeezes": list(t[1])})
+                applied.append(("squeeze", meta_apply_squeeze(chans, list(t[1]), cov, self._chk, self.faults)))
+        return applied, spec
 
     def decode(self, chooser):
         nc = 1 if self.grey else 3
         gtree = link_tree(self.tree, self.check)
-        gd = 128 << self.group_shift
-        small = self.w <= gd and self.h <= gd
-        _, rects, n_lf = section_layout(self.w, self.h, self.group_shift, nc)
         cov = Coverage()
-        gtr, n_img, bad = [], nc, False
-        if self.palette:
-            num_colors, index_chooser = self.palette[0], self.palette[1]
-            pb, pn = (self.palette[2], self.palette[3]) if len(self.palette) > 2 else (0, nc)
-            gtr.append({"id": 1, "begin": pb, "num_c": pn, "num_colors": num_colors, "num_deltas": 0, "predictor": 0})
-            bad |= pb + pn > nc  # check_equal_channels (meta_apply.rs:188)
-            n_img = max(nc - pn + 1, 1)
-        gtr += [{"id": 0, "begin": b, "rct_type": t} for b, t in self.global_rct]
-        bad |= any(b + 3 > n_img or t >= 42 for b, t in self.global_rct)  # rct_type < 42, meta_apply.rs:62
-        if bad and self.check:
-            raise TreeRefused("transform")
-        # the global channel list after meta_apply: [palette meta channel] + n_img image channels. Section 0 takes the
-        # leading "meta or small" channels (mod.rs:353-365), the HF groups the rest.
-        meta = [{"w": self.palette[0], "h": pn, "shift": -1}] if self.palette else []
-        planes = [[[0] * self.w for _ in range(self.h)] for _ in range(n_img)]
-        sections = [None] * (1 + n_lf + len(rects))
-        s0 = {"use_global_tree": True, "wp": self.global_wp, "transforms": gtr, "tokens": None}
-        n0_img = n_img if small else 0
-        route = chooser
-        if self.palette:
-            route = lambda g, m, x, y, c: (chooser if c == 0 else index_chooser)(g, m, x, y, c)  # noqa: E731
-        chans = meta + [{"w": self.w, "h": self.h, "shift": 0} for _ in range(n0_img)]
-        pal_data = None
-        if chans:
-            s0["tokens"] = decode_channels(chans, 0, gtree, self.global_wp, route, cov, self.faults)
-            if self.palette:
-                pal_data = chans[0]["data"]
-            for c in range(n0_img):
-                planes[c] = chans[len(meta) + c]["data"]
-        sections[0] = s0
-        for g, (x0, y0, rw, rh) in enumerate(rects):
-            if n0_img == n_img:  # every image channel went to section 0: the HF groups hold nothing and have no bytes
-                break
-            desc = self.groups.get(g, {})
-            use_global = desc.get("tree") is None
-            tree = gtree if use_global else link_tree(desc["tree"], self.check)
-            chans = [{"w": rw, "h": rh, "shift": 0} for _ in range(n_img)]
-            sid = 1 + 3 * n_lf + 17 + g
-            gch = _offset_chooser(index_chooser if self.palette else chooser, x0, y0)
-            toks = decode_channels(chans, sid, tree, desc.get("wp"), gch, cov, self.faults)
-            data = [c["data"] for c in chans]
-            sections[1 + n_lf + g] = {"use_global_tree": use_global, "wp": desc.get("wp"),
-                                      "transforms": [{"id": 0, "begin": b, "rct_type": t} for b, t in desc.get("rct", ())],
-                                      "tree": desc.get("tree"), "tokens": toks}
-            if any(b + 3 > n_img or t >= 42 for b, t in desc.get("rct", ())):
-                bad = True
-                if self.check:
-                    raise TreeRefused("transform")
-                continue
-            for b, t in reversed(desc.get("rct", ())):  # local transforms are undone at the end of the section
-                inverse_rct(data, b, t, self.faults)
-                cov.local_rct.add(t)
-            for c in range(n_img):
-                for yy in range(rh):
-                    planes[c][y0 + yy][x0:x0 + rw] = data[c][yy]
+        self._log = []  # refusals met with check=False
+        self._chk = True if self.check else self._log
+        chans = [{"w": self.w, "h": self.h, "shift": (0, 0)} for _ in range(nc)]
+        applied, gspec = self._meta_apply(chans, self._global_transforms(nc), cov)
+        n0, lf, hf = channel_sections(chans, self.w, self.h, self.group_shift, self.faults)
+        index_chooser = self.palette[1] if self.palette else chooser
+        route = lambda g, m, x, y, c, meta: (chooser if meta else index_chooser)(g, m, x, y, c)  # noqa: E731
+        data = [None] * len(chans)
+        for i in range(n0):
+            cov.sections.add(("global", chans[i]["shift"]))
+        s0 = {"use_global_tree": True, "wp": self.global_wp, "transforms": gspec, "tokens": None}
+        sc = [dict(chans[i]) for i in range(n0)]
+        toks = decode_channels(sc, 0, gtree, self.global_wp,
+                               lambda g, m, x, y, c: route(g, m, x, y, c, is_meta(sc[c])), cov, self.faults)
+        if any(c["w"] and c["h"] for c in sc):
+            s0["tokens"] = toks
+        self.stream_widths = [max([c["w"] for c in sc], default=0)]
+        for i in range(n0):
+            data[i] = sc[i]["data"]
+        for i in range(n0, len(chans)):
+            data[i] = [[0] * chans[i]["w"] for _ in range(chans[i]["h"])]
+        sections = [s0]
+        for kind, streams in (("lf", lf), ("hf", hf)):
+            for g, (sid, items) in enumerate(streams):
+                sections.append(self._group(kind, g, sid, items, chans, data, gtree, route, cov))
+                self.stream_widths.append(self._width)
+        bad = bool(self._log)
+        planes = None
         if not bad:
-            for b, t in reversed(self.global_rct):
-                inverse_rct(planes, b, t, self.faults)
-                cov.rct.add(t)
-            if self.palette:
-                planes = inverse_palette(pal_data, planes[0], num_colors, nc, cov, self.faults)
+            for t in reversed(applied):
+                if t[0] == "rct":
+                    inverse_rct(data, t[1], t[2], self.faults)
+                    cov.rct.add(t[2])
+                elif t[0] == "palette":
+                    _, b, n, ncol = t
+                    outs = inverse_palette(data[0], data[b + 1], ncol, n, cov, self.faults)
+                    data = data[1:b + 1] + outs + data[b + 2:]
+                else:
+                    undo_squeeze(data, t[1], cov, self.faults)
+            planes = data[:nc]
         self.spec = {"width": self.w, "height": self.h, "group_shift": self.group_shift, "grey": self.grey,
                      "orientation": self.orientation, "prefix": self.prefix, "hybrid": self.hybrid,
                      "tree": self.tree, "sections": sections}
-        self.planes = np.array(planes, dtype=np.int64)
+        self.bad = bad
+        self.planes = np.array(planes, dtype=np.int64) if planes is not None else None
         from tests.f64_pipeline import orient
-        self.u8 = np.ascontiguousarray(orient(store_u8(planes), self.orientation)) if not bad else None
+        self.u8 = np.ascontiguousarray(orient(store_u8(planes), self.orientation)) if planes is not None else None
         self.cov = cov
         return self
 
+    def _group(self, kind, g, sid, items, chans, data, gtree, route, cov):
+        """One ModularLF / ModularHF stream: its rects of the coded channels, the group's local transforms (undone at
+        the end of the section, bitstream.rs:230), the symbols; the decoded rects go back into `data`."""
+        self._width = 0
+        if not any(r[2] and r[3] for _, r in items):
+            return None  # bitstream.rs:143-150: no channel with samples, no bytes
+        desc = self.groups.get(g, {}) if kind == "hf" else {}
+        for i, _ in items:
+            cov.sections.add((kind, chans[i]["shift"]))
+        local = desc.get("transforms")
+        if local is None:
+            local = [("rct", b, t) for b, t in desc.get("rct", ())]
+        use_global = desc.get("tree") is None
+        tree = gtree if use_global else link_tree(desc["tree"], self.check)
+        sc = [{"w": r[2], "h": r[3], "shift": chans[i]["shift"]} for i, r in items]
+        before = len(self._log)
+        applied, lspec = self._meta_apply(sc, local, cov)
+        x0s = {k: items[k][1][:2] for k in range(len(items))}
+        ch = lambda gg, m, x, y, c: route(gg, m, x + x0s.get(c, (0, 0))[0], y + x0s.get(c, (0, 0))[1], c, False)  # noqa: E731
+        toks = decode_channels(sc, sid, tree, desc.get("wp"), ch, cov, self.faults)
+        self._width = max(c["w"] for c in sc)
+        sec = {"use_global_tree": use_global, "wp": desc.get("wp"), "transforms": lspec, "tree": desc.get("tree"),
+               "tokens": toks}
+        if len(self._log) > before:
+            return sec
+        ld = [c["data"] for c in sc]
+        for t in reversed(applied):
+            if t[0] == "rct":
+                inverse_rct(ld, t[1], t[2], self.faults)
+                cov.local_rct.add(t[2])
+            else:
+                undo_squeeze(ld, t[1], cov, self.faults)
+        for k, (i, (x0, y0, rw, rh)) in enumerate(items):
+            for yy in range(rh):
+                data[i][y0 + yy][x0:x0 + rw] = ld[k][yy]
+        return sec
 
-def _offset_chooser(chooser, x0, y0):
-    return lambda guess, mul, x, y, c: chooser(guess, mul, x + x0, y + y0, c)
+
+def _check_equal_channels(chans, b, n, check):  # meta_apply.rs:26-47
+    if b + n > len(chans):
+        _refuse(check, "InvalidChannelRange")
+        return
+    for i in range(1, n):
+        if (chans[b + i]["w"], chans[b + i]["h"], chans[b + i]["shift"]) != (chans[b]["w"], chans[b]["h"], chans[b]["shift"]):
+            _refuse(check, "MixingDifferentChannels")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
