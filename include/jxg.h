@@ -220,6 +220,14 @@ int jxg_batch_stage_marks(void* batch, float* ms, int n);
 int jxg_batch_stats(void* batch, uint64_t* kernel_launches, uint64_t* h2d_bytes, uint64_t* d2h_bytes,
                     float* last_device_ms);
 
+/* Which entropy kernel instances the batch's streams go to: the streams of k_entropy_lean (ANS, one pass, no shift,
+ * no LZ77), k_entropy_fast (prefix codes or a shifted single pass) and k_entropy (several passes or LZ77);
+ * lean_all_420: the lean kernel's instance that assumes hybrid-uint configuration (4, 2, 0) in every cluster;
+ * lean_ctx_smem: the instance that stages the context maps in shared memory; lean_S: lanes per warp of the lean
+ * schedule (4 or 8), 0 before jxg_batch_run or without lean streams. Any pointer may be NULL. */
+int jxg_batch_entropy_stats(void* batch, uint32_t* n_lean, uint32_t* n_fast, uint32_t* n_slow, int* lean_all_420,
+                            int* lean_ctx_smem, uint32_t* lean_S);
+
 /* ---------------- convenience front-end (host parse + batch) ----------------
  * Parses complete .jxl files (container or bare codestream) on the host with
  * the in-tree C++ front-end (the stand-in for the Rust host: headers, TOC,

@@ -903,6 +903,19 @@ int jxg_batch_stats(void* bp, uint64_t* kernel_launches, uint64_t* h2d_bytes, ui
   return JXG_OK;
 }
 
+int jxg_batch_entropy_stats(void* bp, uint32_t* n_lean, uint32_t* n_fast, uint32_t* n_slow, int* lean_all_420,
+                            int* lean_ctx_smem, uint32_t* lean_S) {
+  Batch* b = static_cast<Batch*>(bp);
+  if (!b) return JXG_ERR_ARGUMENT;
+  if (n_lean) *n_lean = uint32_t(b->streams_lean.size());
+  if (n_fast) *n_fast = uint32_t(b->streams_fast.size());
+  if (n_slow) *n_slow = uint32_t(b->streams_slow.size());
+  if (lean_all_420) *lean_all_420 = b->lean_all_420 ? 1 : 0;
+  if (lean_ctx_smem) *lean_ctx_smem = b->lean_ctx_smem ? 1 : 0;
+  if (lean_S) *lean_S = b->lean_ctas ? b->lean_S : 0;
+  return JXG_OK;
+}
+
 int jxg_batch_read_coeffs(void* bp, uint32_t f, int32_t* out, size_t out_len) {
   Batch* b = static_cast<Batch*>(bp);
   if (!b || f >= b->frames.size() || !b->uploaded) return JXG_ERR_ARGUMENT;

@@ -144,6 +144,17 @@ class Batch:
         self._lib.jxg_batch_stats(self._h, C.byref(k), C.byref(h), C.byref(d), C.byref(ms))
         return {"kernel_launches": k.value, "h2d_bytes": h.value, "d2h_bytes": d.value, "device_ms": ms.value}
 
+    def entropy_stats(self):
+        """Which entropy kernel instances decode this batch (jxg_batch_entropy_stats): stream counts of k_entropy_lean,
+        k_entropy_fast and k_entropy, the lean kernel's (4, 2, 0) and shared-memory context map forms, and its lanes
+        per warp (0 before run() or without lean streams)."""
+        nl, nf, ns, s = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()
+        a420, smem = C.c_int(), C.c_int()
+        abi.check(self._lib, self._lib.jxg_batch_entropy_stats(self._h, C.byref(nl), C.byref(nf), C.byref(ns),
+                                                               C.byref(a420), C.byref(smem), C.byref(s)))
+        return {"lean": nl.value, "fast": nf.value, "slow": ns.value, "lean_all_420": bool(a420.value),
+                "lean_ctx_smem": bool(smem.value), "lean_S": s.value}
+
     def read_coeffs(self, f: int):
         n = self.frames[f].info.num_groups * 3 * 65536
         out = np.empty(n, np.int32)

@@ -39,6 +39,8 @@ def _lib():
                                                  C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t]
         _LIB.jxs_modular_lz77_census.argtypes = [C.c_void_p]
         _LIB.jxs_modular_lz77_census.restype = None
+        _LIB.jxs_encode_vardct_tokens.restype = C.c_int64
+        _LIB.jxs_encode_vardct_tokens.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
     return _LIB
 
 
@@ -263,4 +265,61 @@ def encode_modular_tokens(spec) -> bytes:
     if n > cap:
         buf = C.create_string_buffer(n)
         n = lib.jxs_encode_modular_tokens(arr, len(words), buf, n)
+    return buf.raw[:n]
+
+
+def encode_vardct_tokens(spec) -> bytes:
+    """One VarDCT frame whose AC coefficient streams hold exactly the given tokens; the writer predicts nothing and checks
+    nothing (frames a decoder must refuse can be written). The image metadata, the LF quantisation, the dequantisation
+    matrices, the colour correlation and the filters are the defaults. `spec` is a dict:
+      width, height; shifts: one per pass (1..11 passes), the last one 0;
+      bcm: None (the default BlockContextMap) or {"lf": [X, Y, B threshold lists], "qf": [thresholds as decoded, >= 1],
+      "map": block context per (channel, order, qf bucket, LF bucket)};
+      lf: (3, yb, xb) quantised LF integers of the channels X, Y, B; varblocks: (bx, by, transform, raw_quant) tiling
+      the frame; num_histograms;
+      passes: per pass {"selector": 0..3, "used_orders": the 13 bits of selector 3, "perms": {(order, channel):
+      permutation of 64 * num_blocks entries, the first num_blocks fixed}, "cmap": context -> cluster, "cfgs": hybrid
+      (split_exponent, msb, lsb) per cluster, "log_alpha": the smallest ANS alphabet (log2), "prefix": prefix codes,
+      "lz77": None or (min_symbol, min_length)};
+      sections: per pass, per group: (histogram index, [(context, u32 value), ...])."""
+    import numpy as np
+    words = [spec["width"], spec["height"], len(spec["shifts"])] + list(spec["shifts"][:-1])
+    bcm = spec.get("bcm")
+    if bcm is None:
+        words.append(0)
+    else:
+        words.append(1)
+        for thr in bcm["lf"]:
+            words += [len(thr)] + list(thr)
+        words += [len(bcm["qf"])] + list(bcm["qf"])
+        words += [len(bcm["map"])] + list(bcm["map"])
+    lf = np.asarray(spec["lf"], np.int64)
+    words += lf.transpose(1, 2, 0).reshape(-1).tolist()
+    words.append(len(spec["varblocks"]))
+    for vb in spec["varblocks"]:
+        words += list(vb)
+    words.append(spec["num_histograms"])
+    for p in spec["passes"]:
+        words += [p.get("selector", 2), p.get("used_orders", 0), len(p.get("perms", {}))]
+        for (o, c), perm in p.get("perms", {}).items():
+            words += [o, c, len(perm)] + list(perm)
+        words += [len(p["cmap"])] + list(p["cmap"]) + [len(p["cfgs"])]
+        for cfg in p["cfgs"]:
+            words += list(cfg)
+        lz = p.get("lz77")
+        words += [p.get("log_alpha", 5), int(p.get("prefix", 0)), int(lz is not None)] + list(lz or (224, 3))
+    for hist, toks in spec["sections"]:
+        words += [hist, len(toks)]
+        for c, v in toks:
+            words += [c, v]
+    lib = _lib()
+    arr = np.asarray([int(w) & 0xFFFFFFFF for w in words], np.uint32)
+    cap = max(1 << 16, 8 * len(words))
+    buf = C.create_string_buffer(cap)
+    n = lib.jxs_encode_vardct_tokens(arr.ctypes.data, len(words), buf, cap)
+    if n < 0:
+        raise RuntimeError("token-level VarDCT encode failed: " + lib.jxs_last_error().decode())
+    if n > cap:
+        buf = C.create_string_buffer(n)
+        n = lib.jxs_encode_vardct_tokens(arr.ctypes.data, len(words), buf, n)
     return buf.raw[:n]

@@ -1079,6 +1079,362 @@ std::vector<uint8_t> encode(const Params& p) {
   return bytes;
 }
 
+// ---------------------------------------------------------------------------
+// Token-level VarDCT writer (jxs_encode_vardct_tokens): every symbol of the AC coefficient streams is given by the
+// caller, together with the BlockContextMap, the LF integers, the varblocks, the coefficient orders and the entropy
+// codes. Nothing is predicted or checked, so frames a decoder must refuse can be written too.
+// ---------------------------------------------------------------------------
+struct TokenPassSpec {
+  uint32_t selector = 2, used_orders = 0;
+  struct Perm {
+    uint32_t ord, c;
+    std::vector<uint32_t> perm;
+  };
+  std::vector<Perm> perms;
+  std::vector<uint8_t> context_map;
+  uint32_t num_clusters = 1;
+  std::vector<HybridCfg> cfgs;
+  uint32_t log_alpha = 5;
+  bool prefix = false, lz77 = false;
+  uint32_t lz_min_symbol = 224, lz_min_length = 3;
+};
+
+// coeff_order.rs / permutation.rs:27-90 inverted: the Lehmer code of perm[skip..] over the values skip..size-1, as
+// tokens of the 8 permutation contexts (get_context = min(7, ceil_log2(x + 1))); trailing zero codes are not written.
+static void permutation_tokens(const std::vector<uint32_t>& perm, uint32_t skip, std::vector<Token>& out) {
+  const uint32_t size = uint32_t(perm.size());
+  const uint32_t n = size - skip;
+  std::vector<uint32_t> fen(n + 1, 0);  // Fenwick tree over the values still unused
+  auto add = [&](uint32_t i, int d) {
+    for (i++; i <= n; i += i & (0u - i)) fen[i] += uint32_t(d);
+  };
+  auto below = [&](uint32_t i) {  // unused values < i
+    uint32_t s = 0;
+    for (; i; i -= i & (0u - i)) s += fen[i];
+    return s;
+  };
+  for (uint32_t i = 0; i < n; i++) add(i, 1);
+  std::vector<uint32_t> lehmer(n);
+  for (uint32_t i = 0; i < n; i++) {
+    const uint32_t v = perm[skip + i];
+    if (v < skip || v >= size) throw std::runtime_error("permutation entry outside its range");
+    lehmer[i] = below(v - skip);
+    add(v - skip, -1);
+  }
+  uint32_t end = n;
+  while (end && lehmer[end - 1] == 0) end--;
+  auto ctx = [](uint32_t x) { return std::min<uint32_t>(7, ceil_log2(uint64_t(x) + 1)); };
+  out.push_back(Token{ctx(size), end});
+  uint32_t prev = 0;
+  for (uint32_t i = 0; i < end; i++) {
+    out.push_back(Token{ctx(prev), lehmer[i]});
+    prev = lehmer[i];
+  }
+}
+
+std::vector<uint8_t> encode_vardct_tokens(const uint32_t* w, size_t len) {
+  size_t pos = 0;
+  auto next = [&]() -> uint32_t {
+    if (pos >= len) throw std::runtime_error("VarDCT token spec too short");
+    return w[pos++];
+  };
+  const uint32_t W = next(), H = next(), num_passes = next();
+  if (!W || !H || num_passes < 1 || num_passes > 11) throw std::runtime_error("bad size or pass count");
+  std::vector<uint32_t> shifts(num_passes - 1);
+  for (auto& s : shifts) s = next();
+  const uint32_t xb = (W + 7) / 8, yb = (H + 7) / 8, xg = (W + 255) / 256, yg = (H + 255) / 256, num_groups = xg * yg;
+  const uint32_t xlfg = (xb + 255) / 256, ylfg = (yb + 255) / 256, num_lf_groups = xlfg * ylfg;
+  BitWriter lf_global;
+  lf_global.write(1, 1);                // LfQuantFactors default
+  lf_global.u2s_sel(0, 1024 - 1, 11);   // global_scale 1024
+  lf_global.write(0, 2);                // quant_lf = 16
+  if (next() == 0) {
+    lf_global.write(1, 1);  // default BlockContextMap
+  } else {                  // block_context_map.rs:61-126
+    lf_global.write(0, 1);
+    for (int c = 0; c < 3; c++) {
+      const uint32_t n = next();
+      lf_global.write(n, 4);
+      for (uint32_t i = 0; i < n; i++) {
+        const uint32_t u = pack_signed(int32_t(next()));
+        if (u < 16) lf_global.u2s_sel(0, u, 4);
+        else if (u < 272) lf_global.u2s_sel(1, u - 16, 8);
+        else if (u < 65808) lf_global.u2s_sel(2, u - 272, 16);
+        else lf_global.u2s_sel(3, u - 65808, 32);
+      }
+    }
+    const uint32_t nq = next();
+    lf_global.write(nq, 4);
+    for (uint32_t i = 0; i < nq; i++) {
+      const uint32_t v = next() - 1;  // stored minus one
+      if (v < 4) lf_global.u2s_sel(0, v, 2);
+      else if (v < 12) lf_global.u2s_sel(1, v - 4, 3);
+      else if (v < 44) lf_global.u2s_sel(2, v - 12, 5);
+      else lf_global.u2s_sel(3, v - 44, 8);
+    }
+    std::vector<uint8_t> map(next());
+    uint32_t nc = 0;
+    for (auto& m : map) {
+      m = uint8_t(next());
+      nc = std::max<uint32_t>(nc, m + 1u);
+    }
+    write_context_map(lf_global, map, nc);
+  }
+  lf_global.write(1, 1);  // default ColorCorrelationParams
+  lf_global.write(0, 1);  // no global tree
+  // quantised LF integers, X / Y / B per block in raster order
+  std::vector<int32_t> lfq[3];
+  for (auto& q : lfq) q.resize(size_t(xb) * yb);
+  for (size_t i = 0; i < size_t(xb) * yb; i++)
+    for (int c = 0; c < 3; c++) lfq[c][i] = int32_t(next());
+  // varblocks
+  std::vector<uint8_t> tmap(size_t(xb) * yb, 255);
+  std::vector<int32_t> rq(size_t(xb) * yb, 0);
+  const uint32_t nvb = next();
+  for (uint32_t i = 0; i < nvb; i++) {
+    const uint32_t bx = next(), by = next(), t = next(), q = next();
+    if (t >= 27) throw std::runtime_error("transform type above 26");
+    const uint32_t cx = kCoveredBlocksX[t], cy = kCoveredBlocksY[t];
+    if (bx + cx > xb || by + cy > yb) throw std::runtime_error("varblock outside the frame");
+    for (uint32_t y = 0; y < cy; y++)
+      for (uint32_t x = 0; x < cx; x++) {
+        uint8_t& m = tmap[size_t(by + y) * xb + bx + x];
+        if (m != 255) throw std::runtime_error("overlapping varblocks");
+        m = uint8_t(t) | ((x | y) ? 0 : 128);
+      }
+    rq[size_t(by) * xb + bx] = int32_t(q);
+  }
+  for (uint8_t m : tmap)
+    if (m == 255) throw std::runtime_error("block not covered by a varblock");
+  std::vector<BitWriter> lf_groups(num_lf_groups);
+  for (uint32_t g = 0; g < num_lf_groups; g++) {
+    BitWriter& bw = lf_groups[g];
+    const uint32_t x0 = (g % xlfg) * 256, y0 = (g / xlfg) * 256;
+    const uint32_t gw = std::min(256u, xb - x0), gh = std::min(256u, yb - y0);
+    bw.write(0, 2);  // extra_precision
+    std::vector<Chan> ch(3);
+    const int order[3] = {1, 0, 2};  // stored Y, X, B
+    for (int i = 0; i < 3; i++) {
+      ch[i].w = gw;
+      ch[i].h = gh;
+      for (uint32_t y = 0; y < gh; y++)
+        for (uint32_t x = 0; x < gw; x++) ch[i].d.push_back(lfq[order[i]][size_t(y0 + y) * xb + x0 + x]);
+    }
+    write_modular(bw, ch, 5);
+    std::vector<int32_t> types, quants;
+    for (uint32_t y = 0; y < gh; y++)
+      for (uint32_t x = 0; x < gw; x++) {
+        const size_t o = size_t(y0 + y) * xb + x0 + x;
+        if (tmap[o] & 128) {
+          types.push_back(tmap[o] & 127);
+          quants.push_back(rq[o] - 1);
+        }
+      }
+    const uint32_t count = uint32_t(types.size());
+    bw.write(count - 1, ceil_log2(uint64_t(gw) * gh));
+    const uint32_t cw = (gw + 7) / 8, chh = (gh + 7) / 8;
+    std::vector<Chan> mc(4);
+    mc[0].w = mc[1].w = cw;
+    mc[0].h = mc[1].h = chh;
+    mc[0].d.assign(size_t(cw) * chh, 0);
+    mc[1].d.assign(size_t(cw) * chh, 0);
+    mc[2].w = count;
+    mc[2].h = 2;
+    mc[2].d = types;
+    mc[2].d.insert(mc[2].d.end(), quants.begin(), quants.end());
+    mc[3].w = gw;
+    mc[3].h = gh;
+    mc[3].d.assign(size_t(gw) * gh, 0);
+    write_modular(bw, mc, 1);
+  }
+  // HfGlobal (frame/decode.rs:506-566)
+  BitWriter hf_global;
+  hf_global.write(1, 1);  // DequantMatrices all_default
+  const uint32_t num_histograms = next();
+  hf_global.write(num_histograms - 1, ceil_log2(num_groups));
+  std::vector<AnsCode> codes(num_passes);
+  std::vector<BitWriter> order_bits(num_passes);  // per pass: used_orders and the permutations (before its AC code)
+  for (uint32_t p = 0; p < num_passes; p++) {
+    TokenPassSpec ps;
+    ps.selector = next();
+    ps.used_orders = next();
+    order_bits[p].write(ps.selector, 2);
+    if (ps.selector == 3) order_bits[p].write(ps.used_orders, 13);
+    const uint32_t used = ps.selector == 0 ? 0x5f : ps.selector == 1 ? 0x13 : ps.selector == 2 ? 0 : ps.used_orders;
+    const uint32_t nperm = next();
+    for (uint32_t i = 0; i < nperm; i++) {
+      TokenPassSpec::Perm pm;
+      pm.ord = next();
+      pm.c = next();
+      pm.perm.resize(next());
+      for (auto& v : pm.perm) v = next();
+      ps.perms.push_back(std::move(pm));
+    }
+    if (used) {  // coeff_order.rs:122-148: one stream over 8 contexts for every (used order, channel) in turn
+      static const int kOrderTransform[13] = {0, 1, 4, 5, 7, 9, 11, 18, 20, 21, 23, 24, 26};  // TRANSFORM_TYPE_LUT
+      std::vector<Token> toks;
+      for (uint32_t ord = 0; ord < 13; ord++) {
+        if (!(used & (1u << ord))) continue;
+        const uint32_t nb = uint32_t(kCoveredBlocksX[kOrderTransform[ord]]) * kCoveredBlocksY[kOrderTransform[ord]];
+        for (uint32_t c = 0; c < 3; c++) {
+          std::vector<uint32_t> perm(nb * 64);
+          for (uint32_t i = 0; i < perm.size(); i++) perm[i] = i;
+          for (auto& pm : ps.perms)
+            if (pm.ord == ord && pm.c == c) {
+              if (pm.perm.size() != perm.size()) throw std::runtime_error("permutation of the wrong size");
+              perm = pm.perm;
+            }
+          permutation_tokens(perm, nb, toks);
+        }
+      }
+      std::vector<uint8_t> one(8, 0);
+      AnsCode oc = build_code(8, one, 1, {&toks}, 6);
+      write_code(order_bits[p], oc);
+      write_tokens(order_bits[p], oc, toks);
+    }
+    ps.context_map.resize(next());
+    for (auto& m : ps.context_map) m = uint8_t(next());
+    ps.num_clusters = next();
+    for (uint32_t i = 0; i < ps.num_clusters; i++) {
+      HybridCfg h;
+      h.split_exponent = next();
+      h.msb = next();
+      h.lsb = next();
+      ps.cfgs.push_back(h);
+    }
+    ps.log_alpha = next();
+    ps.prefix = next() != 0;
+    ps.lz77 = next() != 0;
+    ps.lz_min_symbol = next();
+    ps.lz_min_length = next();
+    // the sections' tokens of this pass come later in the spec; the code is built once they are read
+    codes[p].num_contexts = uint32_t(ps.context_map.size());
+    codes[p].context_map = ps.context_map;
+    codes[p].num_clusters = ps.num_clusters;
+    codes[p].cluster_cfgs = ps.cfgs;
+    codes[p].log_alpha_size = ps.log_alpha;
+    codes[p].use_prefix = ps.prefix;
+    codes[p].lz.enabled = ps.lz77;
+    codes[p].lz.min_symbol = ps.lz_min_symbol;
+    codes[p].lz.min_length = ps.lz_min_length;
+  }
+  std::vector<uint32_t> hist(size_t(num_passes) * num_groups);
+  std::vector<std::vector<Token>> toks(size_t(num_passes) * num_groups);
+  for (size_t s = 0; s < toks.size(); s++) {
+    hist[s] = next();
+    toks[s].resize(next());
+    for (auto& t : toks[s]) {
+      t.ctx = next();
+      t.value = next();
+    }
+  }
+  if (pos != len) throw std::runtime_error("VarDCT token spec too long");
+  std::vector<std::vector<Sym>> syms(toks.size());
+  for (uint32_t p = 0; p < num_passes; p++) {
+    const AnsCode spec = codes[p];
+    std::vector<const std::vector<Token>*> tp;
+    for (uint32_t g = 0; g < num_groups; g++) tp.push_back(&toks[size_t(p) * num_groups + g]);
+    if (spec.lz.enabled) {  // one hybrid-uint configuration for the literals; the distance context gets its own cluster
+      for (auto& h : spec.cluster_cfgs)
+        if (h.split_exponent != spec.cluster_cfgs[0].split_exponent || h.msb != spec.cluster_cfgs[0].msb ||
+            h.lsb != spec.cluster_cfgs[0].lsb)
+          throw std::runtime_error("an LZ77 pass takes one hybrid-uint configuration");
+      const HybridCfg len_cfg{0, 0, 0};
+      std::vector<const std::vector<Sym>*> sp;
+      for (uint32_t g = 0; g < num_groups; g++) {
+        syms[size_t(p) * num_groups + g] = lz77_symbols(*tp[g], spec.cluster_cfgs[0], spec.lz, len_cfg, spec.num_contexts);
+        sp.push_back(&syms[size_t(p) * num_groups + g]);
+      }
+      std::vector<uint8_t> map = spec.context_map;
+      map.push_back(uint8_t(spec.num_clusters));
+      codes[p] = build_code_lz77(spec.num_contexts + 1, map, spec.num_clusters + 1, sp, spec.lz, spec.use_prefix);
+      codes[p].cfg = spec.cluster_cfgs[0];
+      codes[p].lz_len_cfg = len_cfg;
+    } else {
+      codes[p] = build_code_cfgs(spec.num_contexts, spec.context_map, spec.num_clusters, tp, spec.log_alpha_size,
+                                 spec.use_prefix, spec.cluster_cfgs);
+    }
+  }
+  for (uint32_t p = 0; p < num_passes; p++) {
+    append_bits(hf_global, order_bits[p]);
+    write_code(hf_global, codes[p]);
+  }
+  std::vector<BitWriter> hf_groups(toks.size());
+  for (size_t s = 0; s < toks.size(); s++) {
+    hf_groups[s].write(hist[s], ceil_log2(num_histograms));  // group.rs:333-341
+    const AnsCode& code = codes[s / num_groups];
+    if (code.lz.enabled) write_symbols(hf_groups[s], code, syms[s]);
+    else write_tokens(hf_groups[s], code, toks[s]);
+  }
+
+  BitWriter out;
+  out.write(0xff, 8);
+  out.write(0x0a, 8);
+  auto write_dim = [&](uint32_t v) {  // size.rs:31-47
+    const uint32_t m = v - 1;
+    if (m < (1u << 9)) out.u2s_sel(0, m, 9);
+    else if (m < (1u << 13)) out.u2s_sel(1, m, 13);
+    else if (m < (1u << 18)) out.u2s_sel(2, m, 18);
+    else out.u2s_sel(3, m, 30);
+  };
+  out.write(0, 1);  // small = false
+  write_dim(H);
+  out.write(0, 3);  // explicit xsize
+  write_dim(W);
+  out.write(1, 1);  // ImageMetadata all_default
+  out.write(1, 1);  // CustomTransformData all_default
+  out.zero_pad_to_byte();
+  // FrameHeader (frame_header.rs:267-444) with the default filters and qm scales
+  out.write(0, 1);  // all_default
+  out.write(0, 2);  // RegularFrame
+  out.write(0, 1);  // VarDCT
+  out.write_u64(0);  // flags
+  out.write(0, 2);  // upsampling = 1
+  out.write(3, 3);  // x_qm_scale
+  out.write(2, 3);  // b_qm_scale
+  if (num_passes == 1) out.u2s_sel(0);  // Passes (frame_header.rs:46-75)
+  else if (num_passes <= 3) out.u2s_sel(num_passes - 1);
+  else out.u2s_sel(3, num_passes - 4, 3);
+  if (num_passes != 1) {
+    out.u2s_sel(0);  // num_ds = 0
+    for (uint32_t s : shifts) out.write(s, 2);
+  }
+  out.write(0, 1);  // have_crop
+  out.write(0, 2);  // blending mode Replace
+  out.write(1, 1);  // is_last
+  out.write(0, 2);  // name length 0
+  out.write(0, 1);  // RestorationFilter all_default = 0
+  out.write(1, 1);  // gab
+  out.write(0, 1);  // gab_custom
+  out.write(2, 2);  // epf_iters
+  out.write(0, 1);  // epf_sharp_custom
+  out.write(0, 1);  // epf_weight_custom
+  out.write(0, 1);  // epf_sigma_custom
+  out.write_u64(0);  // restoration filter extensions
+  out.write_u64(0);  // frame header extensions
+  std::vector<std::vector<uint8_t>> sections;
+  if (num_groups == 1 && num_passes == 1) {  // single TOC entry: sections concatenated bitwise
+    BitWriter all;
+    append_bits(all, lf_global);
+    append_bits(all, lf_groups[0]);
+    append_bits(all, hf_global);
+    append_bits(all, hf_groups[0]);
+    sections.push_back(all.finish());
+  } else {
+    sections.push_back(lf_global.finish());
+    for (auto& b : lf_groups) sections.push_back(b.finish());
+    sections.push_back(hf_global.finish());
+    for (auto& b : hf_groups) sections.push_back(b.finish());
+  }
+  out.write(0, 1);  // TOC not permuted
+  out.zero_pad_to_byte();
+  for (auto& s : sections) write_toc_entry(out, uint32_t(s.size()));
+  out.zero_pad_to_byte();
+  std::vector<uint8_t> bytes = out.finish();
+  for (auto& s : sections) bytes.insert(bytes.end(), s.begin(), s.end());
+  return bytes;
+}
+
 // 8-bit RGB rendering of the same procedural image (source of the synthetic Modular frames).
 void make_image_u8(uint32_t width, uint32_t height, uint64_t seed, std::vector<uint8_t>& rgb) {
   Params p{width, height, seed, 1.0f, 0, 0, 0, 0, 0};
@@ -1158,6 +1514,19 @@ int64_t jxs_encode_synthetic_ex(uint32_t width, uint32_t height, uint64_t seed, 
       if (pos != dequant_len) throw std::runtime_error("dequant array too long");
     }
     std::vector<uint8_t> b = jxs::encode(p);
+    if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
+    return int64_t(b.size());
+  } catch (std::exception& e) {
+    g_err = e.what();
+    return -1;
+  }
+}
+
+// One VarDCT frame written exactly as described by `spec` (synth/__init__.py encode_vardct_tokens gives the layout).
+// Returns the number of bytes written (or the needed size when `cap` is too small), negative on error.
+int64_t jxs_encode_vardct_tokens(const uint32_t* spec, size_t len, uint8_t* out, size_t cap) {
+  try {
+    std::vector<uint8_t> b = jxs::encode_vardct_tokens(spec, len);
     if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
     return int64_t(b.size());
   } catch (std::exception& e) {

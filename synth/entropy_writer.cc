@@ -383,6 +383,18 @@ static std::vector<Sym> plain_symbols(const std::vector<Token>& tokens, const Hy
   }
   return out;
 }
+// Each token with the configuration of its context's cluster.
+static std::vector<Sym> plain_symbols(const std::vector<Token>& tokens, const std::vector<uint8_t>& cluster_of_ctx,
+                                      const std::vector<HybridCfg>& cfgs) {
+  std::vector<Sym> out;
+  out.reserve(tokens.size());
+  for (const Token& t : tokens) {
+    Sym s{t.ctx, 0, 0, 0};
+    cfgs.at(cluster_of_ctx.at(t.ctx)).encode(t.value, s.tok, s.nbits, s.bits);
+    out.push_back(s);
+  }
+  return out;
+}
 
 std::vector<Sym> lz77_symbols(const std::vector<Token>& tokens, const HybridCfg& cfg, const Lz77& lz, const HybridCfg& len_cfg,
                               uint32_t dist_ctx) {
@@ -429,6 +441,20 @@ AnsCode build_code(size_t num_contexts, const std::vector<uint8_t>& cluster_of_c
   for (auto& v : syms) ptrs.push_back(&v);
   AnsCode code = build_code_syms(num_contexts, cluster_of_ctx, num_clusters, ptrs, min_log_alpha, use_prefix);
   code.cfg = cfg;
+  return code;
+}
+
+AnsCode build_code_cfgs(size_t num_contexts, const std::vector<uint8_t>& cluster_of_ctx, uint32_t num_clusters,
+                        const std::vector<const std::vector<Token>*>& streams, uint32_t min_log_alpha, bool use_prefix,
+                        const std::vector<HybridCfg>& cfgs) {
+  if (cfgs.size() != num_clusters) throw std::runtime_error("one hybrid-uint configuration per cluster expected");
+  std::vector<std::vector<Sym>> syms;
+  for (auto* s : streams) syms.push_back(plain_symbols(*s, cluster_of_ctx, cfgs));
+  std::vector<const std::vector<Sym>*> ptrs;
+  for (auto& v : syms) ptrs.push_back(&v);
+  AnsCode code = build_code_syms(num_contexts, cluster_of_ctx, num_clusters, ptrs, min_log_alpha, use_prefix);
+  code.cfg = cfgs[0];
+  code.cluster_cfgs = cfgs;
   return code;
 }
 
@@ -522,7 +548,29 @@ static AnsCode build_code_syms(size_t num_contexts, const std::vector<uint8_t>& 
 }
 
 static const HybridCfg& cluster_cfg(const AnsCode& code, uint32_t c) {
+  if (!code.cluster_cfgs.empty()) return code.cluster_cfgs[c];
   return code.lz.enabled && code.lz_dist_own_cfg && c == code.context_map.back() ? code.lz_dist_cfg : code.cfg;
+}
+
+void write_context_map(BitWriter& bw, const std::vector<uint8_t>& map, uint32_t num_clusters) {
+  // context map (context_map.rs:43-76)
+  uint32_t bits_needed = ceil_log2(num_clusters);
+  if (bits_needed <= 3 && uint32_t(map.size()) * bits_needed < 2048) {
+    bw.write(1, 1);  // is_simple
+    bw.write(bits_needed, 2);
+    if (bits_needed)
+      for (uint8_t m : map) bw.write(m, bits_needed);
+  } else {
+    bw.write(0, 1);  // not simple
+    bw.write(0, 1);  // no MTF
+    std::vector<Token> toks;
+    toks.reserve(map.size());
+    for (uint8_t m : map) toks.push_back(Token{0, m});
+    std::vector<uint8_t> one(1, 0);
+    AnsCode sub = build_code(1, one, 1, {&toks});
+    write_code(bw, sub);
+    write_tokens(bw, sub, toks);
+  }
 }
 
 void write_code(BitWriter& bw, const AnsCode& code) {
@@ -543,26 +591,7 @@ void write_code(BitWriter& bw, const AnsCode& code) {
   } else {
     bw.write(0, 1);
   }
-  if (code.num_contexts > 1) {
-    // context map (context_map.rs:43-76)
-    uint32_t bits_needed = ceil_log2(code.num_clusters);
-    if (bits_needed <= 3 && code.num_contexts * bits_needed < 2048) {
-      bw.write(1, 1);  // is_simple
-      bw.write(bits_needed, 2);
-      if (bits_needed)
-        for (uint8_t m : code.context_map) bw.write(m, bits_needed);
-    } else {
-      bw.write(0, 1);  // not simple
-      bw.write(0, 1);  // no MTF
-      std::vector<Token> toks;
-      toks.reserve(code.context_map.size());
-      for (uint8_t m : code.context_map) toks.push_back(Token{0, m});
-      std::vector<uint8_t> one(1, 0);
-      AnsCode sub = build_code(1, one, 1, {&toks});
-      write_code(bw, sub);
-      write_tokens(bw, sub, toks);
-    }
-  }
+  if (code.num_contexts > 1) write_context_map(bw, code.context_map, code.num_clusters);
   if (code.use_prefix) {  // decode.rs:509-524, huffman.rs:466-480
     bw.write(1, 1);
     for (uint32_t c = 0; c < code.num_clusters; c++) write_hybrid_cfg(bw, cluster_cfg(code, c), 15);
@@ -591,6 +620,7 @@ void write_code(BitWriter& bw, const AnsCode& code) {
 }
 
 void write_tokens(BitWriter& bw, const AnsCode& code, const std::vector<Token>& tokens) {
+  if (!code.cluster_cfgs.empty()) return write_symbols(bw, code, plain_symbols(tokens, code.context_map, code.cluster_cfgs));
   write_symbols(bw, code, plain_symbols(tokens, code.cfg));
 }
 

@@ -120,6 +120,7 @@ struct AnsCode {
   uint32_t num_clusters = 0;
   uint32_t log_alpha_size = 6;
   HybridCfg cfg;
+  std::vector<HybridCfg> cluster_cfgs;            // empty: every cluster uses `cfg`; else one configuration per cluster
   std::vector<std::vector<uint16_t>> freqs;       // [cluster][alphabet] sums to 4096
   std::vector<std::vector<uint16_t>> inv;         // [cluster] start index per symbol into slots
   std::vector<std::vector<uint16_t>> slots;       // [cluster] concatenated idx lists per symbol (offset -> idx)
@@ -142,9 +143,15 @@ std::vector<uint16_t> normalize_counts(const std::vector<uint64_t>& counts, size
 AnsCode build_code(size_t num_contexts, const std::vector<uint8_t>& cluster_of_ctx, uint32_t num_clusters,
                    const std::vector<const std::vector<Token>*>& streams, uint32_t min_log_alpha = 5, bool use_prefix = false,
                    const HybridCfg& cfg = HybridCfg());
+// build_code with one hybrid-uint configuration per cluster (cfgs[cluster]).
+AnsCode build_code_cfgs(size_t num_contexts, const std::vector<uint8_t>& cluster_of_ctx, uint32_t num_clusters,
+                        const std::vector<const std::vector<Token>*>& streams, uint32_t min_log_alpha, bool use_prefix,
+                        const std::vector<HybridCfg>& cfgs);
 // Convenience: one cluster per context when num_contexts <= 8, else quantile clustering into <= max_clusters.
 std::vector<uint8_t> cluster_contexts(size_t num_contexts, const std::vector<const std::vector<Token>*>& streams,
                                       uint32_t max_clusters, uint32_t& num_clusters, const HybridCfg& cfg);
+// Serialises a context map (context_map.rs:43-76): the simple form when it fits, else entropy coded without MTF.
+void write_context_map(BitWriter& bw, const std::vector<uint8_t>& map, uint32_t num_clusters);
 // Serialises the LZ77 parameters, context map, ANS flag, log_alpha, uint configs, histograms (decode.rs:487-545).
 void write_code(BitWriter& bw, const AnsCode& code);
 // Writes initial state + symbols so that decoding ends in 0x130000.
