@@ -185,12 +185,14 @@ int jxg_batch_run(void* batch, void* cuda_stream);
 /* Blocks until the batch finished; returns the first error (per-stream status
  * words written by the entropy kernel, check_final_state decode.rs:400). */
 int jxg_batch_wait(void* batch, uint32_t* first_bad_frame, uint32_t* first_bad_group);
-/* Re-run the same batch (inputs already resident in HBM): device-only timing. */
+/* Re-run the same batch (inputs already resident in HBM): device-only timing. Ordered after the batch's own last
+ * run, whichever stream that ran on. */
 int jxg_batch_rerun_device(void* batch, void* cuda_stream);
 void jxg_batch_end(void* batch);
 
-/* Parity taps: copy intermediate planes of frame `f` of a finished batch to
- * host. coeffs: 3 planes of i32, dense per group in decode order (group.rs:53).
+/* Parity taps: copy intermediate planes of frame `f` of a batch to host, after
+ * waiting for the batch's own last run on whichever stream it ran.
+ * coeffs: 3 planes of i32, dense per group in decode order (group.rs:53).
  * xyb: the 3 padded XYB planes (f32) after dequant + IDCT; `stage` must be 0
  * (JXG_ERR_ARGUMENT otherwise). Meaningful after a run stopped with debug stop 2. */
 int jxg_batch_read_coeffs(void* batch, uint32_t f, int32_t* out, size_t out_len);
@@ -284,8 +286,10 @@ int jxg_modular_batch_add(void* batch, void* parsed, void* out, size_t out_row_s
 int jxg_modular_batch_set_lanes(void* batch, int lanes_per_warp);
 int jxg_modular_batch_run(void* batch, void* cuda_stream);
 int jxg_modular_batch_wait(void* batch, uint32_t* first_bad_frame, uint32_t* first_bad_group);
+/* Ordered after the batch's own last run, whichever stream that ran on. */
 int jxg_modular_batch_rerun_device(void* batch, void* cuda_stream);
-/* Parity tap: final colour planes of frame f (3 x H x W i32, before the u8 conversion). */
+/* Parity tap: final colour planes of frame f (3 x H x W i32, before the u8 conversion), after waiting for the
+ * batch's own last run on whichever stream it ran. */
 int jxg_modular_batch_read_planes(void* batch, uint32_t f, int32_t* out, size_t out_len);
 /* ms[0]: whole batch on the device, ms[1]: group-stream decode kernel (+ local RCT). */
 int jxg_modular_batch_stats(void* batch, uint64_t* h2d_bytes, uint64_t* d2h_bytes, uint64_t* kernel_launches, float* ms);

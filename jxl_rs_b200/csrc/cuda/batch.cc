@@ -59,11 +59,10 @@ struct FrameOut {
   size_t stage_off, stage_stride;
 };
 
-struct Batch {
-  Context* ctx;
+struct Batch : BatchCore {
   PinnedArena& blob;
   explicit Batch(Context* c)
-      : ctx(c), blob(c->blob), d_blob(c->d_blob), d_coeffs(c->d_coeffs), d_block_off(c->d_block_off), d_nz(c->d_nz),
+      : blob(c->blob), d_blob(c->d_blob), d_coeffs(c->d_coeffs), d_block_off(c->d_block_off), d_nz(c->d_nz),
         d_planes_a(c->d_planes_a), d_status(c->d_status), d_out(c->d_out) {}
   std::vector<FrameDev> frames;
   std::vector<SectionDev> sections;
@@ -82,7 +81,6 @@ struct Batch {
   int debug_stop = 0;
   // device
   DevBuf &d_blob, &d_coeffs, &d_block_off, &d_nz, &d_planes_a, &d_status, &d_out;
-  bool uploaded = false;
   // byte offsets of the batch tables inside the blob (they ride on the one pinned H2D copy: a cudaMemcpyAsync from
   // pageable std::vector storage blocks the calling thread until earlier device work drains, which takes long with
   // other batches in flight)
@@ -90,13 +88,9 @@ struct Batch {
     uint64_t frames = 0, sections = 0, streams = 0, lean_cta = 0, lean_warp = 0, streams_lean = 0, streams_fast = 0, streams_slow = 0,
              nz_base = 0, ftiles = 0;
   } tab;
-  int32_t* status_host = nullptr;  // pinned (context-owned): a D2H copy into pageable memory would block jxg_batch_run
-  size_t status_n = 0;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_handoff = nullptr;
-  cudaStream_t last_stream = nullptr;  // stream of the last run / rerun (the context's or the caller's)
+  cudaEvent_t ev_handoff = nullptr;
   bool profile = false;
   cudaEvent_t stage_ev[kNumStages + 1] = {nullptr};
-  uint64_t launches = 0, h2d = 0, d2h = 0;
   float last_ms = 0;
 };
 
@@ -240,10 +234,10 @@ int jxg_init(int device, void** out_ctx) {
     no_off[i] = uint32_t(no.size());
     no.insert(no.end(), o.begin(), o.end());
   }
-  if (int r = upload(ctx->dequant_default, dq, ctx->stream, nullptr)) return r;
-  if (int r = upload(ctx->dequant_default_off, dq_off, ctx->stream, nullptr)) return r;
-  if (int r = upload(ctx->natural_orders, no, ctx->stream, nullptr)) return r;
-  if (int r = upload(ctx->natural_order_off, no_off, ctx->stream, nullptr)) return r;
+  if (int r = upload(ctx->dequant_default, dq, ctx->stream)) return r;
+  if (int r = upload(ctx->dequant_default_off, dq_off, ctx->stream)) return r;
+  if (int r = upload(ctx->natural_orders, no, ctx->stream)) return r;
+  if (int r = upload(ctx->natural_order_off, no_off, ctx->stream)) return r;
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   g_live_contexts[device & 63].fetch_add(1);
   *out_ctx = ctx.release();
@@ -266,24 +260,9 @@ void jxg_shutdown(void* c) {
 int jxg_batch_begin(void* c, uint32_t n_frames_hint, void** out_batch) {
   if (!c || !out_batch) return JXG_ERR_ARGUMENT;
   Context* cx = static_cast<Context*>(c);
-  if (cx->batch_live) return set_error(JXG_ERR_ARGUMENT, "one live batch per context: call jxg_batch_end first");
   auto b = std::make_unique<Batch>(cx);
-  CUDA_TRY(cudaSetDevice(b->ctx->device));
-  cx->blob.size = 0;
-  cx->blob.pending.clear();
-  cx->blob.deferred_threads = 0;
+  if (int r = batch_begin(*b, cx, &b->ev_handoff, cudaEventDisableTiming)) return r;
   b->frames.reserve(n_frames_hint);
-  CUDA_TRY(cudaEventCreate(&b->ev0));
-  if (cudaError_t e = cudaEventCreate(&b->ev1); e != cudaSuccess) {
-    cudaEventDestroy(b->ev0);
-    return set_error(JXG_ERR_CUDA, std::string("cudaEventCreate: ") + cudaGetErrorString(e));
-  }
-  if (cudaError_t e = cudaEventCreateWithFlags(&b->ev_handoff, cudaEventDisableTiming); e != cudaSuccess) {
-    cudaEventDestroy(b->ev0);
-    cudaEventDestroy(b->ev1);
-    return set_error(JXG_ERR_CUDA, std::string("cudaEventCreate: ") + cudaGetErrorString(e));
-  }
-  cx->batch_live = true;  // only once nothing can fail any more
   *out_batch = b.release();
   return JXG_OK;
 }
@@ -291,14 +270,10 @@ int jxg_batch_begin(void* c, uint32_t n_frames_hint, void** out_batch) {
 void jxg_batch_end(void* bp) {
   Batch* b = static_cast<Batch*>(bp);
   if (!b) return;
-  cudaSetDevice(b->ctx->device);
-  if (b->uploaded && b->ev1) cudaEventSynchronize(b->ev1);
-  if (b->ev0) cudaEventDestroy(b->ev0);
-  if (b->ev1) cudaEventDestroy(b->ev1);
-  if (b->ev_handoff) cudaEventDestroy(b->ev_handoff);
+  batch_end(*b);
+  cudaEventDestroy(b->ev_handoff);
   for (auto& e : b->stage_ev)
     if (e) cudaEventDestroy(e);
-  b->ctx->batch_live = false;
   delete b;
 }
 
@@ -730,11 +705,6 @@ static int launch(Batch* b, cudaStream_t se, cudaStream_t s, bool copy_to_host) 
   return 0;
 }
 
-static int copy_status(Batch* b, cudaStream_t s) {
-  CUDA_TRY(cudaMemcpyAsync(b->status_host, b->d_status.p, b->status_n * 4, cudaMemcpyDeviceToHost, s));
-  return 0;
-}
-
 // JXG_TRACE_RUN=1: host-side phase times of jxg_batch_run on stderr (which call blocks, and for how long).
 struct RunTrace {
   bool on = getenv("JXG_TRACE_RUN") != nullptr;
@@ -785,34 +755,13 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
     if (fo.orientation != 1) b->frames[f].out_ptr = static_cast<uint8_t*>(b->ctx->d_orient.p) + fo.stage_off;
     else b->frames[f].out_ptr = fo.is_device ? fo.user_ptr : static_cast<uint8_t*>(b->d_out.p) + fo.dev_off;
   }
-  b->status_n = b->streams.size();
-  if (b->status_n > b->ctx->status_cap) {
-    if (b->ctx->status_host) cudaFreeHost(b->ctx->status_host);
-    size_t cap = std::max<size_t>(b->status_n * 2, 1 << 16);
-    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&b->ctx->status_host), cap * 4, cudaHostAllocDefault));
-    b->ctx->status_cap = cap;
-  }
-  b->status_host = b->ctx->status_host;
-  memset(b->status_host, 0, b->status_n * 4);
-  {  // batch tables behind the frames' data in the pinned blob: they travel with the one H2D copy below
-    auto put = [&](const void* p, size_t bytes, uint64_t& off) {
-      const int64_t o = b->blob.append(bytes ? p : nullptr, bytes, 16, 16);
-      if (o < 0) return false;
-      off = uint64_t(o);
-      return true;
-    };
-    bool ok = put(b->frames.data(), b->frames.size() * sizeof(FrameDev), b->tab.frames) &&
-              put(b->sections.data(), b->sections.size() * sizeof(SectionDev), b->tab.sections) &&
-              put(b->streams.data(), b->streams.size() * sizeof(StreamDev), b->tab.streams) &&
-              put(b->lean_cta_first.data(), b->lean_cta_first.size() * 4, b->tab.lean_cta) &&
-              put(b->lean_warps.data(), b->lean_warps.size() * sizeof(uint2), b->tab.lean_warp) &&
-              put(b->streams_lean.data(), b->streams_lean.size() * sizeof(StreamDev), b->tab.streams_lean) &&
-              put(b->streams_fast.data(), b->streams_fast.size() * sizeof(StreamDev), b->tab.streams_fast) &&
-              put(b->streams_slow.data(), b->streams_slow.size() * sizeof(StreamDev), b->tab.streams_slow) &&
-              put(b->nz_base.data(), b->nz_base.size() * 8, b->tab.nz_base) &&
-              put(b->fused_prefix.data(), b->fused_prefix.size() * 4, b->tab.ftiles);
-    if (!ok) return set_error(JXG_ERR_CUDA, "pinned staging allocation failed");
-  }
+  if (int r = batch_status(*b, b->streams.size())) return r;
+  if (!batch_table(b->blob, b->frames, b->tab.frames) || !batch_table(b->blob, b->sections, b->tab.sections) ||
+      !batch_table(b->blob, b->streams, b->tab.streams) || !batch_table(b->blob, b->lean_cta_first, b->tab.lean_cta) ||
+      !batch_table(b->blob, b->lean_warps, b->tab.lean_warp) || !batch_table(b->blob, b->streams_lean, b->tab.streams_lean) ||
+      !batch_table(b->blob, b->streams_fast, b->tab.streams_fast) || !batch_table(b->blob, b->streams_slow, b->tab.streams_slow) ||
+      !batch_table(b->blob, b->nz_base, b->tab.nz_base) || !batch_table(b->blob, b->fused_prefix, b->tab.ftiles))
+    return set_error(JXG_ERR_CUDA, "pinned staging allocation failed");
   if (int r = b->d_blob.ensure(b->blob.size + 64)) return r;
   trace.mark("alloc");
   b->blob.flush();
@@ -834,7 +783,7 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
   trace.mark("uploads");
   if (int r = launch(b, se, s, true)) return r;
   trace.mark("launch");
-  if (int r = copy_status(b, s)) return r;
+  CUDA_TRY(cudaMemcpyAsync(b->status_host, b->d_status.p, b->status_n * 4, cudaMemcpyDeviceToHost, s));
   // ev1 = everything of this batch done. The D2H stream joins the post stream and carries ev1 when it holds the output
   // copies (no debug stop): the post stream itself must not wait for them (the next batch's transforms follow on it).
   if (b->debug_stop == 0) {
@@ -883,14 +832,7 @@ int jxg_batch_wait(void* bp, uint32_t* first_bad_frame, uint32_t* first_bad_grou
   }
   CUDA_TRY(cudaGetLastError());
   cudaEventElapsedTime(&b->last_ms, b->ev0, b->ev1);
-  for (size_t i = 0; i < b->status_n; i++)
-    if (b->status_host[i] != 0) {
-      if (first_bad_frame) *first_bad_frame = b->streams[i].frame;
-      if (first_bad_group) *first_bad_group = b->streams[i].group;
-      return set_error(b->status_host[i], "entropy decode failed in frame " + std::to_string(b->streams[i].frame) +
-                                              " group " + std::to_string(b->streams[i].group));
-    }
-  return JXG_OK;
+  return batch_first_failure(*b, b->streams, "entropy decode failed in frame ", first_bad_frame, first_bad_group);
 }
 
 int jxg_batch_stats(void* bp, uint64_t* kernel_launches, uint64_t* h2d_bytes, uint64_t* d2h_bytes, float* last_device_ms) {
@@ -941,8 +883,7 @@ int jxg_batch_read_xyb(void* bp, uint32_t f, int stage, float* out, size_t out_l
   const FrameDev& F = b->frames[f];
   size_t n = 3 * F.plane_size;
   if (out_len < n) return JXG_ERR_ARGUMENT;
-  CUDA_TRY(cudaSetDevice(b->ctx->device));
-  CUDA_TRY(cudaStreamSynchronize(b->ctx->stream));
+  if (int r = batch_wait_last_run(*b)) return r;
   CUDA_TRY(cudaMemcpy(out, static_cast<const float*>(b->d_planes_a.p) + F.plane_base, n * 4, cudaMemcpyDeviceToHost));
   return JXG_OK;
 }

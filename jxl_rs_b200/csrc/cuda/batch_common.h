@@ -137,7 +137,7 @@ struct Context {
   // steady-state decode loop does no cudaMalloc / cudaHostAlloc.
   PinnedArena blob;
   DevBuf d_blob, d_coeffs, d_block_off, d_nz, d_planes_a, d_status, d_out, d_lean_desc, d_lean_nblk, d_orient, d_lzwin,
-      d_modular_lzwin;
+      d_modular_lzwin, d_modular_wp;
   bool batch_live = false;
   // pinned status readback buffer, owned by the context: cudaHostAlloc / cudaFreeHost synchronise the whole
   // device, so they must not happen per batch when batches of several contexts are in flight
@@ -145,12 +145,94 @@ struct Context {
   size_t status_cap = 0;
 };
 
+// What a batch of either engine holds besides its frames. ev0: before the upload; ev1: behind everything of the last run.
+struct BatchCore {
+  Context* ctx = nullptr;
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  bool uploaded = false;
+  cudaStream_t last_stream = nullptr;  // stream of the last run / rerun (the context's or the caller's)
+  int32_t* status_host = nullptr;      // pinned (context-owned): a D2H copy into pageable memory would block the run
+  size_t status_n = 0;
+  uint64_t launches = 0, h2d = 0, d2h = 0;
+};
+
+// One live batch per context. Creates ev0, ev1 and the engine's own event `extra`; on failure the context stays free.
+inline int batch_begin(BatchCore& b, Context* cx, cudaEvent_t* extra, unsigned extra_flags) {
+  if (cx->batch_live) return set_error(JXG_ERR_ARGUMENT, "one live batch per context: end the previous batch first");
+  CUDA_TRY(cudaSetDevice(cx->device));
+  b.ctx = cx;
+  cx->blob.size = 0;
+  cx->blob.pending.clear();
+  cx->blob.deferred_threads = 0;
+  cudaError_t e = cudaEventCreate(&b.ev0);
+  if (e == cudaSuccess) e = cudaEventCreate(&b.ev1);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(extra, extra_flags);
+  if (e != cudaSuccess) {
+    for (cudaEvent_t ev : {b.ev0, b.ev1, *extra})
+      if (ev) cudaEventDestroy(ev);
+    return set_error(JXG_ERR_CUDA, std::string("cudaEventCreate: ") + cudaGetErrorString(e));
+  }
+  cx->batch_live = true;  // only once nothing can fail any more
+  return 0;
+}
+
+// Waits for the last run (the context's pools are then free for the next batch); the engine destroys its own events.
+inline void batch_end(BatchCore& b) {
+  cudaSetDevice(b.ctx->device);
+  if (b.uploaded) cudaEventSynchronize(b.ev1);
+  cudaEventDestroy(b.ev0);
+  cudaEventDestroy(b.ev1);
+  b.ctx->batch_live = false;
+}
+
+// The batch's status words: the first n of the context's pinned status buffer (grown if needed), zeroed.
+inline int batch_status(BatchCore& b, size_t n) {
+  Context* cx = b.ctx;
+  if (n > cx->status_cap) {
+    if (cx->status_host) cudaFreeHost(cx->status_host);
+    cx->status_host = nullptr;
+    cx->status_cap = 0;
+    const size_t cap = std::max<size_t>(n * 2, 1 << 16);
+    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&cx->status_host), cap * 4, cudaHostAllocDefault));
+    cx->status_cap = cap;
+  }
+  b.status_host = cx->status_host;
+  b.status_n = n;
+  memset(b.status_host, 0, n * 4);
+  return 0;
+}
+
+// The first non-zero status word as the batch's error: "<what><frame> group <group>" of the stream it belongs to.
+template <typename Stream>
+int batch_first_failure(const BatchCore& b, const std::vector<Stream>& streams, const char* what, uint32_t* frame, uint32_t* group) {
+  for (size_t i = 0; i < b.status_n; i++)
+    if (b.status_host[i] != 0) {
+      if (frame) *frame = streams[i].frame;
+      if (group) *group = streams[i].group;
+      return set_error(b.status_host[i], what + std::to_string(streams[i].frame) + " group " + std::to_string(streams[i].group));
+    }
+  return 0;
+}
+
+// Appends a batch table to the pinned blob, so that it travels with the one H2D copy; `off`: its offset in the blob.
+template <typename T>
+bool batch_table(PinnedArena& blob, const std::vector<T>& v, uint64_t& off) {
+  const int64_t o = blob.append(v.empty() ? nullptr : v.data(), v.size() * sizeof(T), 16, 16);
+  off = uint64_t(o);
+  return o >= 0;
+}
+
+// Read taps copy device buffers of the last run, which may have run on a caller's stream: they wait for its ev1.
+inline int batch_wait_last_run(const BatchCore& b) {
+  CUDA_TRY(cudaSetDevice(b.ctx->device));
+  CUDA_TRY(cudaEventSynchronize(b.ev1));
+  return 0;
+}
 
 template <typename T>
-int upload(DevBuf& b, const std::vector<T>& v, cudaStream_t s, uint64_t* counter) {
+int upload(DevBuf& b, const std::vector<T>& v, cudaStream_t s) {
   if (int r = b.ensure(std::max<size_t>(v.size() * sizeof(T), 16))) return r;
   if (!v.empty()) CUDA_TRY(cudaMemcpyAsync(b.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, s));
-  if (counter) *counter += v.size() * sizeof(T);
   return 0;
 }
 

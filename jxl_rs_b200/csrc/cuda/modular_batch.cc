@@ -32,11 +32,10 @@ struct MFrame {
   uint64_t host_planes_blob = 0;   // blob offset of the packed host-decoded planes
   uint64_t host_planes_elems = 0;
   size_t dev_out_off = 0;
-  uint32_t first_stream = 0, num_streams = 0;
 };
 
-struct ModularBatch {
-  Context* ctx;
+// Device buffers: the context's pools; tables: in its pinned blob. A steady-state loop of batches allocates nothing.
+struct ModularBatch : BatchCore {
   std::vector<MFrame> frames;
   std::vector<MStreamDev> streams;
   std::vector<uint32_t> order, rct_streams;
@@ -45,20 +44,17 @@ struct ModularBatch {
   std::vector<MRctDev> rcts;
   std::vector<uint32_t> refs;
   std::vector<std::vector<MJobDev>> levels;  // jobs grouped by plan step index
-  std::vector<int> level_kind;
+  std::vector<jxg::ModularJobKind> level_kind;
   std::vector<MJobDev> store_jobs;
   uint64_t arena_elems = 0, wp_bytes = 0, out_bytes = 0;
   uint64_t lz_window_elems = 0;             // symbol windows of the LZ77 streams, one per stream
   uint32_t lz77_streams = 0, rle_streams = 0;  // streams with LZ77; of those, streams whose copies all have distance 1
   uint32_t num_plain = 0;                   // streams without LZ77: the first ones of `order`
-  std::vector<uint32_t> stream_frame_group;  // for error reports
-  bool uploaded = false;
-  uint64_t launches = 0, h2d = 0, d2h = 0;
   uint32_t lanes_per_warp = 1;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_decode = nullptr;
-  int32_t* status_host = nullptr;
-  // device pools (context-owned buffers are reused where the meaning matches)
-  DevBuf d_streams, d_order, d_rct_streams, d_rects, d_codes, d_rcts, d_refs, d_jobs, d_wp;
+  cudaEvent_t ev_decode = nullptr;
+  struct {  // byte offsets of the batch tables in the blob
+    uint64_t streams = 0, order = 0, rct_streams = 0, rects = 0, codes = 0, rcts = 0, refs = 0, jobs = 0;
+  } tab;
 };
 
 uint64_t blob_append(ModularBatch* b, const void* p, size_t bytes, size_t align = 16, size_t tail = 0) {
@@ -239,24 +235,12 @@ struct BatchMark {
   }
 };
 
-void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t stride, bool is_device) {
-  if (!ms->device_plan_ok)
-    throw jxg::Error(JXG_ERR_UNSUPPORTED, "palette transforms with delta entries or a predictor are not implemented on the device path");
-  if (ms->toc.offsets.size() == 1 && !ms->hf[0].empty)
-    throw jxg::Error(JXG_ERR_UNSUPPORTED, "single-section Modular frames with a coded group are not on the device path");
-  MFrame f;
-  f.ms = ms;
-  f.out = out;
-  f.out_stride = stride;
-  f.out_is_device = is_device;
-  const uint32_t W = ms->header.xsize(), H = ms->header.ysize();
-  const uint32_t orient = ms->file.orientation;  // applied by the store kernel (render/save.rs)
-  if (stride < size_t(orient >= 5 ? H : W) * 3) throw jxg::Error(JXG_ERR_INVALID_OUTPUT, "output row stride too small");
-  // ---- plane arena: host-decoded coded channels first (one contiguous upload), then the rest ----
+// Plane arena: host-decoded coded channels first (one contiguous copy from the blob), then the rest.
+void add_arena(ModularBatch* b, MFrame& f) {
+  const jxg::ModularFrameState* ms = f.ms;
   f.arena_base = b->arena_elems;
   f.buf_off.assign(ms->bufs.size(), 0);
   uint64_t cursor = f.arena_base;
-  std::vector<int32_t> packed;
   for (size_t c = 0; c < ms->coded.size(); c++)
     if (ms->host_decoded[c]) {
       f.buf_off[c] = cursor;
@@ -271,18 +255,20 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t st
     }
   b->arena_elems = (cursor + 63) & ~uint64_t(63);
   if (f.host_planes_elems) {
-    f.host_planes_blob = uint64_t(b->ctx->blob.append(nullptr, 0, 16, 0));
+    f.host_planes_blob = blob_append(b, nullptr, 0, 16);
     for (size_t c = 0; c < ms->coded.size(); c++)
       if (ms->host_decoded[c] && !ms->coded[c].data.empty()) blob_append(b, ms->coded[c].data.data(), ms->coded[c].data.size() * 4, 4);
   }
-  // ---- codes / trees ----
+}
+
+// Codes / trees, and per coded group stream its MStreamDev, rects, reference channels, local RCTs and LZ77 window.
+void add_streams(ModularBatch* b, MFrame& f) {
+  const jxg::ModularFrameState* ms = f.ms;
   uint32_t global_code = 0;
   uint64_t global_tree = 0;
   bool have_global = false;
-  static const bool walk_tables = !(getenv("JXG_MODULAR_WALK_TABLES") && atoi(getenv("JXG_MODULAR_WALK_TABLES")) == 0);
   std::map<WalkKey, WalkInfo> walk_cache;
   std::map<uint64_t, bool> inner_static;
-  f.first_stream = uint32_t(b->streams.size());
   for (const jxg::ModularGroupStream& st : ms->hf) {
     if (st.empty) continue;
     const jxg::ModularTree* tree = st.local_tree ? st.local_tree.get() : &ms->global_tree;
@@ -322,7 +308,7 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t st
       rd.h = r.h;
       rd.walk = kWalkGeneric;
       rd.lut_off = 0;
-      if (walk_tables && r.w && r.h) {
+      if (r.w && r.h) {
         const uint32_t root = static_root(*tree, uint32_t(ri), st.stream_id);
         // channel / stream decisions below another split make the table specific to this channel of this stream
         auto is_it = inner_static.find(d.tree_off);
@@ -380,15 +366,20 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t st
     }
     b->streams.push_back(d);
   }
-  f.num_streams = uint32_t(b->streams.size()) - f.first_stream;
-  // ---- global inverse plan -> jobs per level ----
+}
+
+// Global inverse plan -> jobs per level. A frame with fewer steps than the batch has levels has no jobs in the last
+// ones; levels are launched in order and the store runs after all of them, so only the kinds of the common steps must
+// agree, whatever the order of adding.
+void add_plan(ModularBatch* b, const MFrame& f) {
+  const jxg::ModularFrameState* ms = f.ms;
   for (size_t si = 0; si < ms->steps.size(); si++) {
     const jxg::ModularStep& s = ms->steps[si];
     if (b->levels.size() <= si) {
       b->levels.emplace_back();
-      b->level_kind.push_back(int(s.kind));
+      b->level_kind.push_back(s.kind);
     }
-    if (b->level_kind[si] != int(s.kind))
+    if (b->level_kind[si] != s.kind)
       throw jxg::Error(JXG_ERR_UNSUPPORTED, "frames of one Modular batch must share the global transform structure");
     MJobDev j;
     memset(&j, 0, sizeof(j));
@@ -397,9 +388,9 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t st
     j.c = f.buf_off[s.c];
     j.w = ms->bufs[s.a].w;
     j.h = ms->bufs[s.a].h;
-    j.rw = s.kind == 1 ? ms->bufs[s.b].w : (s.kind == 2 ? ms->bufs[s.b].h : 0);
+    j.rw = s.kind == jxg::kJobHSqueeze ? ms->bufs[s.b].w : (s.kind == jxg::kJobVSqueeze ? ms->bufs[s.b].h : 0);
     j.op = s.rct_op;
-    if (s.kind == 3) {  // one job per colour channel: a index plane, b palette plane (row c = component c), c output
+    if (s.kind == jxg::kJobPalette) {  // one job per colour channel: a index plane, b palette plane (row c = component c), c output
       if (ms->bufs[s.b].h < s.n || ms->bufs[s.b].w < s.num_colors) throw jxg::Error(jxg::kErrBitstream, "palette channel smaller than its header says");
       for (uint32_t c = 0; c < s.n; c++) {
         j.c = f.buf_off[s.c + c];
@@ -412,8 +403,12 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t st
     }
     b->levels[si].push_back(j);
   }
-  // A frame with fewer steps than the batch has levels has no jobs in the last ones; levels are launched in order and
-  // the store runs after all of them, so only the kinds of the common steps must agree, whatever the order of adding.
+}
+
+// Store job: the final colour planes -> the u8 output, in the file's orientation (render/save.rs).
+void add_store(ModularBatch* b, MFrame& f) {
+  const jxg::ModularFrameState* ms = f.ms;
+  const uint32_t W = ms->header.xsize(), H = ms->header.ysize();
   MJobDev sj;
   memset(&sj, 0, sizeof(sj));
   const uint32_t nc = ms->num_color_channels;
@@ -422,15 +417,33 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t st
   sj.c = f.buf_off[ms->out_buf[nc > 2 ? 2 : 0]];
   sj.w = W;
   sj.h = H;
-  sj.op = orient;
+  sj.op = ms->file.orientation;
   for (uint32_t c = 0; c < nc; c++)
     if (ms->bufs[ms->out_buf[c]].w != W || ms->bufs[ms->out_buf[c]].h != H)
       throw jxg::Error(jxg::kErrBitstream, "unexpected output channel size");
-  if (!is_device) {
+  if (!f.out_is_device) {
     f.dev_out_off = b->out_bytes;
     b->out_bytes += (size_t(W) * H * 3 + 255) & ~size_t(255);
   }
   b->store_jobs.push_back(sj);
+}
+
+void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t stride, bool is_device) {
+  if (!ms->device_plan_ok)
+    throw jxg::Error(JXG_ERR_UNSUPPORTED, "palette transforms with delta entries or a predictor are not implemented on the device path");
+  if (ms->toc.offsets.size() == 1 && !ms->hf[0].empty)
+    throw jxg::Error(JXG_ERR_UNSUPPORTED, "single-section Modular frames with a coded group are not on the device path");
+  const uint32_t W = ms->header.xsize(), H = ms->header.ysize();
+  if (stride < size_t(ms->file.orientation >= 5 ? H : W) * 3) throw jxg::Error(JXG_ERR_INVALID_OUTPUT, "output row stride too small");
+  MFrame f;
+  f.ms = ms;
+  f.out = out;
+  f.out_stride = stride;
+  f.out_is_device = is_device;
+  add_arena(b, f);
+  add_streams(b, f);
+  add_plan(b, f);
+  add_store(b, f);
   b->frames.push_back(std::move(f));
 }
 
@@ -439,15 +452,15 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
   MBatchDev B;
   memset(&B, 0, sizeof(B));
   B.blob = static_cast<const uint8_t*>(cx->d_blob.p);
-  B.streams = static_cast<const MStreamDev*>(b->d_streams.p);
-  B.order = static_cast<const uint32_t*>(b->d_order.p);
-  B.rct_streams = static_cast<const uint32_t*>(b->d_rct_streams.p);
-  B.rects = static_cast<const MRectDev*>(b->d_rects.p);
-  B.codes = static_cast<const MCodeDev*>(b->d_codes.p);
-  B.rcts = static_cast<const MRctDev*>(b->d_rcts.p);
-  B.refs = static_cast<const uint32_t*>(b->d_refs.p);
+  B.streams = reinterpret_cast<const MStreamDev*>(B.blob + b->tab.streams);
+  B.order = reinterpret_cast<const uint32_t*>(B.blob + b->tab.order);
+  B.rct_streams = reinterpret_cast<const uint32_t*>(B.blob + b->tab.rct_streams);
+  B.rects = reinterpret_cast<const MRectDev*>(B.blob + b->tab.rects);
+  B.codes = reinterpret_cast<const MCodeDev*>(B.blob + b->tab.codes);
+  B.rcts = reinterpret_cast<const MRctDev*>(B.blob + b->tab.rcts);
+  B.refs = reinterpret_cast<const uint32_t*>(B.blob + b->tab.refs);
   B.planes = static_cast<int32_t*>(cx->d_planes_a.p);
-  B.wp_scratch = static_cast<uint8_t*>(b->d_wp.p);
+  B.wp_scratch = static_cast<uint8_t*>(cx->d_modular_wp.p);
   B.status = static_cast<int32_t*>(cx->d_status.p);
   B.queue = reinterpret_cast<uint32_t*>(B.status + b->streams.size());
   B.num_streams = uint32_t(b->streams.size());
@@ -457,30 +470,21 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
     if (f.host_planes_elems)
       CUDA_TRY(cudaMemcpyAsync(B.planes + f.arena_base, B.blob + f.host_planes_blob, f.host_planes_elems * 4,
                                cudaMemcpyDeviceToDevice, s));
-  uint64_t launches = uint64_t(launch_modular_decode(B, b->num_plain, b->lanes_per_warp, uint32_t(b->rct_streams.size()), s));
-  if (b->ev_decode) CUDA_TRY(cudaEventRecord(b->ev_decode, s));
-  const MJobDev* jobs = static_cast<const MJobDev*>(b->d_jobs.p);
-  size_t job_cursor = 0;
-  for (size_t l = 0; l < b->levels.size(); l++) {
+  b->launches = uint64_t(launch_modular_decode(B, b->num_plain, b->lanes_per_warp, uint32_t(b->rct_streams.size()), s));
+  CUDA_TRY(cudaEventRecord(b->ev_decode, s));
+  const MJobDev* jobs = reinterpret_cast<const MJobDev*>(B.blob + b->tab.jobs);  // the levels in order, then the stores
+  auto launch_jobs = [&](jxg::ModularJobKind kind, const std::vector<MJobDev>& level) {
     uint32_t mw = 0, mh = 0;
-    for (const MJobDev& j : b->levels[l]) {
+    for (const MJobDev& j : level) {
       mw = std::max(mw, j.w);
       mh = std::max(mh, j.h);
     }
-    launch_modular_jobs(b->level_kind[l] == 3 ? 4 : b->level_kind[l], jobs + job_cursor, uint32_t(b->levels[l].size()), mw, mh, B.planes, s);
-    job_cursor += b->levels[l].size();
-    launches++;
-  }
-  {
-    uint32_t mw = 0, mh = 0;
-    for (const MJobDev& j : b->store_jobs) {
-      mw = std::max(mw, j.w);
-      mh = std::max(mh, j.h);
-    }
-    launch_modular_jobs(3, jobs + job_cursor, uint32_t(b->store_jobs.size()), mw, mh, B.planes, s);
-    launches++;
-  }
-  b->launches = launches;
+    launch_modular_jobs(kind, jobs, uint32_t(level.size()), mw, mh, B.planes, s);
+    jobs += level.size();
+    b->launches++;
+  };
+  for (size_t l = 0; l < b->levels.size(); l++) launch_jobs(b->level_kind[l], b->levels[l]);
+  launch_jobs(jxg::kJobStore, b->store_jobs);
   if (copy_to_host) {
     for (const MFrame& f : b->frames)
       if (!f.out_is_device) {
@@ -491,7 +495,7 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
         b->d2h += size_t(W) * 3 * H;
       }
   }
-  CUDA_TRY(cudaMemcpyAsync(b->status_host, cx->d_status.p, b->streams.size() * 4, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(b->status_host, cx->d_status.p, b->status_n * 4, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -529,18 +533,8 @@ void jxg_modular_parsed_free(void* parsed) { delete static_cast<jxg::ModularFram
 
 int jxg_modular_batch_begin(void* c, void** out_batch) {
   if (!c || !out_batch) return JXG_ERR_ARGUMENT;
-  Context* cx = static_cast<Context*>(c);
-  if (cx->batch_live) return set_error(JXG_ERR_ARGUMENT, "one live batch per context: end the previous batch first");
-  CUDA_TRY(cudaSetDevice(cx->device));
   auto b = std::make_unique<ModularBatch>();
-  b->ctx = cx;
-  cx->blob.size = 0;
-  cx->blob.pending.clear();
-  cx->blob.deferred_threads = 0;
-  cx->batch_live = true;
-  CUDA_TRY(cudaEventCreate(&b->ev0));
-  CUDA_TRY(cudaEventCreate(&b->ev1));
-  CUDA_TRY(cudaEventCreate(&b->ev_decode));
+  if (int r = batch_begin(*b, static_cast<Context*>(c), &b->ev_decode, cudaEventDefault)) return r;
   *out_batch = b.release();
   return JXG_OK;
 }
@@ -572,6 +566,7 @@ int jxg_modular_batch_run(void* bp, void* cuda_stream) {
   Context* cx = b->ctx;
   CUDA_TRY(cudaSetDevice(cx->device));
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : cx->stream;
+  b->last_stream = s;
   b->h2d = b->d2h = 0;
   // streams without LZ77, then those with it (each group has its own decode launch); longest section first within
   // each (the decode kernel's queue is a longest-processing-time schedule)
@@ -582,11 +577,10 @@ int jxg_modular_batch_run(void* bp, void* cuda_stream) {
     return lz(x) != lz(y) ? lz(y) : b->streams[x].sec_len > b->streams[y].sec_len;
   });
   b->num_plain = uint32_t(b->streams.size()) - b->lz77_streams;
-  if (int r = cx->d_blob.ensure(cx->blob.size + 64)) return r;
   if (int r = cx->d_planes_a.ensure(std::max<size_t>(b->arena_elems * 4, 16))) return r;
   if (int r = cx->d_status.ensure((b->streams.size() + 8) * 4)) return r;
   if (int r = cx->d_out.ensure(std::max<size_t>(b->out_bytes, 16))) return r;
-  if (int r = b->d_wp.ensure(std::max<size_t>(b->wp_bytes, 16))) return r;
+  if (int r = cx->d_modular_wp.ensure(std::max<size_t>(b->wp_bytes, 16))) return r;
   if (b->lz_window_elems && cx->d_modular_lzwin.ensure(b->lz_window_elems * 4)) {
     cudaGetLastError();
     return set_error(JXG_ERR_UNSUPPORTED, "no device memory for the LZ77 windows of the batch (" +
@@ -598,28 +592,20 @@ int jxg_modular_batch_run(void* bp, void* cuda_stream) {
     b->store_jobs[i].out_stride =
         f.out_is_device ? f.out_stride : size_t(f.ms->file.orientation >= 5 ? f.ms->header.ysize() : f.ms->header.xsize()) * 3;
   }
-  if (b->streams.size() > cx->status_cap) {
-    if (cx->status_host) cudaFreeHost(cx->status_host);
-    size_t cap = std::max<size_t>(b->streams.size() * 2, 1 << 16);
-    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&cx->status_host), cap * 4, cudaHostAllocDefault));
-    cx->status_cap = cap;
-  }
-  b->status_host = cx->status_host;
-  memset(b->status_host, 0, b->streams.size() * 4);
+  if (int r = batch_status(*b, b->streams.size())) return r;
   std::vector<MJobDev> all_jobs;
   for (auto& l : b->levels) all_jobs.insert(all_jobs.end(), l.begin(), l.end());
   all_jobs.insert(all_jobs.end(), b->store_jobs.begin(), b->store_jobs.end());
+  PinnedArena& blob = cx->blob;
+  if (!batch_table(blob, b->streams, b->tab.streams) || !batch_table(blob, b->order, b->tab.order) ||
+      !batch_table(blob, b->rct_streams, b->tab.rct_streams) || !batch_table(blob, b->rects, b->tab.rects) ||
+      !batch_table(blob, b->codes, b->tab.codes) || !batch_table(blob, b->rcts, b->tab.rcts) ||
+      !batch_table(blob, b->refs, b->tab.refs) || !batch_table(blob, all_jobs, b->tab.jobs))
+    return set_error(JXG_ERR_CUDA, "pinned staging allocation failed");
+  if (int r = cx->d_blob.ensure(blob.size + 64)) return r;
   CUDA_TRY(cudaEventRecord(b->ev0, s));
-  CUDA_TRY(cudaMemcpyAsync(cx->d_blob.p, cx->blob.p, cx->blob.size, cudaMemcpyHostToDevice, s));
-  b->h2d += cx->blob.size;
-  if (int r = upload(b->d_streams, b->streams, s, &b->h2d)) return r;
-  if (int r = upload(b->d_order, b->order, s, &b->h2d)) return r;
-  if (int r = upload(b->d_rct_streams, b->rct_streams, s, &b->h2d)) return r;
-  if (int r = upload(b->d_rects, b->rects, s, &b->h2d)) return r;
-  if (int r = upload(b->d_codes, b->codes, s, &b->h2d)) return r;
-  if (int r = upload(b->d_rcts, b->rcts, s, &b->h2d)) return r;
-  if (int r = upload(b->d_refs, b->refs, s, &b->h2d)) return r;
-  if (int r = upload(b->d_jobs, all_jobs, s, &b->h2d)) return r;
+  CUDA_TRY(cudaMemcpyAsync(cx->d_blob.p, blob.p, blob.size, cudaMemcpyHostToDevice, s));
+  b->h2d += blob.size;
   b->uploaded = true;
   if (int r = launch_all(b, s, true)) return r;
   CUDA_TRY(cudaEventRecord(b->ev1, s));
@@ -631,6 +617,8 @@ int jxg_modular_batch_rerun_device(void* bp, void* cuda_stream) {
   if (!b || !b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch was never submitted");
   CUDA_TRY(cudaSetDevice(b->ctx->device));
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : b->ctx->stream;
+  b->last_stream = s;
+  CUDA_TRY(cudaStreamWaitEvent(s, b->ev1, 0));  // the previous run of this batch still owns its device buffers
   CUDA_TRY(cudaEventRecord(b->ev0, s));
   if (int r = launch_all(b, s, false)) return r;
   CUDA_TRY(cudaEventRecord(b->ev1, s));
@@ -640,24 +628,16 @@ int jxg_modular_batch_rerun_device(void* bp, void* cuda_stream) {
 int jxg_modular_batch_wait(void* bp, uint32_t* bad_frame, uint32_t* bad_group) {
   ModularBatch* b = static_cast<ModularBatch*>(bp);
   if (!b || !b->uploaded) return JXG_ERR_ARGUMENT;
-  CUDA_TRY(cudaSetDevice(b->ctx->device));
-  CUDA_TRY(cudaEventSynchronize(b->ev1));
-  for (size_t i = 0; i < b->streams.size(); i++)
-    if (b->status_host[i] != 0) {
-      if (bad_frame) *bad_frame = b->streams[i].frame;
-      if (bad_group) *bad_group = b->streams[i].group;
-      return set_error(b->status_host[i], "Modular group stream failed: frame " + std::to_string(b->streams[i].frame) + " group " +
-                                              std::to_string(b->streams[i].group));
-    }
-  return JXG_OK;
+  if (int r = batch_wait_last_run(*b)) return r;
+  CUDA_TRY(cudaGetLastError());
+  return batch_first_failure(*b, b->streams, "Modular group stream failed: frame ", bad_frame, bad_group);
 }
 
 // Parity tap: the final colour planes (3 x H x W i32, before the u8 conversion) of frame f.
 int jxg_modular_batch_read_planes(void* bp, uint32_t f, int32_t* out, size_t out_len) {
   ModularBatch* b = static_cast<ModularBatch*>(bp);
   if (!b || !b->uploaded || f >= b->frames.size() || !out) return JXG_ERR_ARGUMENT;
-  CUDA_TRY(cudaSetDevice(b->ctx->device));
-  CUDA_TRY(cudaStreamSynchronize(b->ctx->stream));
+  if (int r = batch_wait_last_run(*b)) return r;
   const MJobDev& j = b->store_jobs[f];
   const size_t n = size_t(j.w) * j.h;
   if (out_len < 3 * n) return set_error(JXG_ERR_ARGUMENT, "plane buffer too small");
@@ -672,8 +652,7 @@ int jxg_modular_batch_read_planes(void* bp, uint32_t f, int32_t* out, size_t out
 int jxg_modular_batch_stats(void* bp, uint64_t* h2d, uint64_t* d2h, uint64_t* launches, float* ms) {
   ModularBatch* b = static_cast<ModularBatch*>(bp);
   if (!b || !b->uploaded) return JXG_ERR_ARGUMENT;
-  CUDA_TRY(cudaSetDevice(b->ctx->device));
-  CUDA_TRY(cudaEventSynchronize(b->ev1));
+  if (int r = batch_wait_last_run(*b)) return r;
   if (h2d) *h2d = b->h2d;
   if (d2h) *d2h = b->d2h;
   if (launches) *launches = b->launches;
@@ -724,11 +703,8 @@ int jxg_modular_walk_table(const int32_t* nodes, uint32_t n_nodes, const uint8_t
 void jxg_modular_batch_end(void* bp) {
   ModularBatch* b = static_cast<ModularBatch*>(bp);
   if (!b) return;
-  cudaSetDevice(b->ctx->device);
-  cudaStreamSynchronize(b->ctx->stream);
-  for (cudaEvent_t e : {b->ev0, b->ev1, b->ev_decode})
-    if (e) cudaEventDestroy(e);
-  b->ctx->batch_live = false;
+  batch_end(*b);
+  cudaEventDestroy(b->ev_decode);
   delete b;
 }
 

@@ -169,7 +169,7 @@ void build_inverse_plan(ModularFrameState& ms) {
     if (t.id == 0) {
       const uint32_t perm = t.rct_type / 7, b = t.begin_channel;
       ModularStep s;
-      s.kind = 0;
+      s.kind = kJobRct;
       s.a = cur[b];
       s.b = cur[b + 1];
       s.c = cur[b + 2];
@@ -188,7 +188,7 @@ void build_inverse_plan(ModularFrameState& ms) {
         return;
       }
       ModularStep s;
-      s.kind = 3;
+      s.kind = kJobPalette;
       s.a = cur[bi];
       s.b = cur[0];
       s.c = uint32_t(ms.bufs.size());
@@ -207,7 +207,7 @@ void build_inverse_plan(ModularFrameState& ms) {
         for (size_t c = b; c < e; c++) {
           const uint32_t avg = cur[c], res = cur[offset + (c - b)];
           ModularStep s;
-          s.kind = sq.horizontal ? 1 : 2;
+          s.kind = sq.horizontal ? kJobHSqueeze : kJobVSqueeze;
           s.a = avg;
           s.b = res;
           s.c = uint32_t(ms.bufs.size());

@@ -39,9 +39,17 @@ struct ModularGroupStream {
 struct ModularBuf {
   uint32_t w = 0, h = 0;
 };
+// Kinds of the plan steps and of the device jobs that carry them out (the `kind` of launch_modular_jobs in
+// cuda/modular_device.h): one numbering. It lives here because the front-end also builds without the CUDA headers.
+enum ModularJobKind : uint32_t {
+  kJobRct = 0,       // in place on a, b, c
+  kJobHSqueeze = 1,  // horizontal unsqueeze: a avg, b residual -> c
+  kJobVSqueeze = 2,  // vertical unsqueeze
+  kJobStore = 3,     // final colour planes -> u8 output (device job only, no plan step)
+  kJobPalette = 4,   // palette without delta entries: a index channel, b palette, c .. c + n - 1 the colour channels
+};
 struct ModularStep {
-  uint32_t kind = 0;  // 0 RCT (in place on a,b,c), 1 horizontal unsqueeze (a avg, b residual -> c), 2 vertical,
-                      // 3 palette without delta entries (a index channel, b palette, c .. c + n - 1 the colour channels)
+  ModularJobKind kind = kJobRct;
   uint32_t a = 0, b = 0, c = 0;
   uint32_t rct_op = 0;
   uint32_t n = 0, num_colors = 0;  // palette: colour channels, explicit palette entries

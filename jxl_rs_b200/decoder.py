@@ -85,16 +85,44 @@ class JxgContext:
             pass
 
 
-class Batch:
+class _BatchHandle:
+    """The handle of either batch kind (C functions `<_PREFIX>begin / run / rerun_device / end`): one live batch per
+    context; run and rerun_device take a raw cudaStream_t, 0 for the context's own stream."""
+    _PREFIX = ""
+
+    def __init__(self, ctx: JxgContext, *begin_args):
+        self._lib = ctx._lib
+        self._ctx = ctx
+        self._h = C.c_void_p()
+        abi.check(self._lib, getattr(self._lib, self._PREFIX + "begin")(ctx._h, *begin_args, C.byref(self._h)))
+
+    def run(self, stream_ptr: int = 0):
+        abi.check(self._lib, getattr(self._lib, self._PREFIX + "run")(self._h, C.c_void_p(stream_ptr)))
+
+    def rerun_device(self, stream_ptr: int = 0):
+        abi.check(self._lib, getattr(self._lib, self._PREFIX + "rerun_device")(self._h, C.c_void_p(stream_ptr)))
+
+    def close(self):
+        if self._h.value:
+            if self._ctx._h.value:  # a batch that outlives its context is abandoned, not freed through it
+                getattr(self._lib, self._PREFIX + "end")(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Batch(_BatchHandle):
     """jxg_batch_*: frames decoded together by one kernel pipeline."""
+    _PREFIX = "jxg_batch_"
 
     def __init__(self, ctx: JxgContext, n_hint: int = 0, staging_threads: int = 0):
         """staging_threads > 0: large input copies are deferred to run() and done by that many host threads
         (jxg_batch_set_deferred_copy); the ParsedFrames added are kept alive by this object."""
-        self._lib = ctx._lib
-        self._ctx = ctx
-        self._h = C.c_void_p()
-        abi.check(self._lib, self._lib.jxg_batch_begin(ctx._h, n_hint, C.byref(self._h)))
+        super().__init__(ctx, n_hint)
         self._keep = []
         self.frames = []
         if staging_threads > 0:
@@ -129,12 +157,6 @@ class Batch:
         abi.check(self._lib, self._lib.jxg_batch_stage_marks(self._h, ms, 11))
         return [float(v) for v in ms]
 
-    def run(self, stream_ptr: int = 0):
-        abi.check(self._lib, self._lib.jxg_batch_run(self._h, C.c_void_p(stream_ptr)))
-
-    def rerun_device(self, stream_ptr: int = 0):
-        abi.check(self._lib, self._lib.jxg_batch_rerun_device(self._h, C.c_void_p(stream_ptr)))
-
     def wait(self):
         f, g = C.c_uint32(), C.c_uint32()
         abi.check(self._lib, self._lib.jxg_batch_wait(self._h, C.byref(f), C.byref(g)))
@@ -167,18 +189,6 @@ class Batch:
         out = np.empty(3 * ps * pr, np.float32)
         abi.check(self._lib, self._lib.jxg_batch_read_xyb(self._h, f, stage, out.ctypes.data_as(C.c_void_p), out.size))
         return out.reshape(3, pr, ps)
-
-    def close(self):
-        if self._h.value:
-            if self._ctx._h.value:  # a batch that outlives its context is abandoned, not freed through it
-                self._lib.jxg_batch_end(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def decode_files(ctx: JxgContext, files, pixel_format: JxlPixelFormat = JxlPixelFormat(), to_host: bool = True):
@@ -451,14 +461,12 @@ class ModularParsedFrame:
             self._h = C.c_void_p()
 
 
-class ModularBatch:
+class ModularBatch(_BatchHandle):
     """jxg_modular_batch_*: Modular frames whose group streams are decoded together on the GPU."""
+    _PREFIX = "jxg_modular_batch_"
 
     def __init__(self, ctx: JxgContext, lanes_per_warp: int = 1):
-        self._lib = ctx._lib
-        self._ctx = ctx
-        self._h = C.c_void_p()
-        abi.check(self._lib, self._lib.jxg_modular_batch_begin(ctx._h, C.byref(self._h)))
+        super().__init__(ctx)
         abi.check(self._lib, self._lib.jxg_modular_batch_set_lanes(self._h, lanes_per_warp))
         self.frames = []
 
@@ -466,12 +474,6 @@ class ModularBatch:
         abi.check(self._lib, self._lib.jxg_modular_batch_add(self._h, frame._h, C.c_void_p(out_ptr), row_stride,
                                                              1 if out_is_device else 0))
         self.frames.append(frame)
-
-    def run(self, stream_ptr: int = 0):
-        abi.check(self._lib, self._lib.jxg_modular_batch_run(self._h, C.c_void_p(stream_ptr)))
-
-    def rerun_device(self, stream_ptr: int = 0):
-        abi.check(self._lib, self._lib.jxg_modular_batch_rerun_device(self._h, C.c_void_p(stream_ptr)))
 
     def wait(self):
         bf, bg = C.c_uint32(), C.c_uint32()
@@ -497,18 +499,6 @@ class ModularBatch:
         out = np.zeros((3, fr.info.coded_height, fr.info.coded_width), np.int32)
         abi.check(self._lib, self._lib.jxg_modular_batch_read_planes(self._h, f, out.ctypes.data, out.size))
         return out
-
-    def close(self):
-        if self._h and self._h.value:
-            if self._ctx._h.value:  # a batch that outlives its context is abandoned, not freed through it
-                self._lib.jxg_modular_batch_end(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def decode_modular_files(ctx: JxgContext, files, to_host: bool = True, lanes_per_warp: int = 1):

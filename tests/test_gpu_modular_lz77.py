@@ -7,6 +7,7 @@ import pytest
 
 from jxl_rs_b200 import abi
 from tests import test_modular_lz77 as L
+from tests.gpu_modular import gpu_decode
 
 pytestmark = pytest.mark.gpu
 
@@ -17,31 +18,6 @@ def ctx():
     c = j.JxgContext(0)
     yield c
     c.close()
-
-
-def gpu_decode(ctx, files, lanes=1, expect_error=False):
-    """(u8 outputs, i32 planes, lz77_stats, the JxgError of wait() or None)."""
-    import torch
-    import jxl_rs_b200 as j
-    frames = [j.ModularParsedFrame(f) for f in files]
-    outs = [torch.empty((fr.height, fr.width, 3), dtype=torch.uint8).pin_memory() for fr in frames]
-    b = j.ModularBatch(ctx, lanes)
-    err = None
-    try:
-        for fr, o in zip(frames, outs):
-            b.add(fr, o.data_ptr(), fr.width * 3, False)
-        stats = b.lz77_stats()
-        b.run()
-        try:
-            b.wait()
-        except abi.JxgError as e:
-            if not expect_error:
-                raise
-            err = e
-        planes = [b.read_planes(i) for i in range(len(frames))]
-    finally:
-        b.close()
-    return [o.numpy().copy() for o in outs], planes, stats, err
 
 
 @pytest.mark.parametrize("lz", [1, 2])
@@ -55,7 +31,7 @@ def test_writer_frames_equal_the_oracle(ctx, kw, lz):
     data = synth.encode_modular(w, h, 7, source=src, lz77=lz, **kw)
     ref_out, ref_planes = L.oracle(data)
     for lanes in (1, 2, 4):
-        (out,), (planes,), st, _ = gpu_decode(ctx, [data], lanes)
+        (out,), (planes,), st = gpu_decode(ctx, [data], lanes, lz77_stats=True)
         assert np.array_equal(planes, ref_planes) and np.array_equal(out, ref_out) and np.array_equal(out, src)
         assert st["lz77_streams"] == 9 and st["rle_streams"] == (9 if lz == 1 else 0), st
         assert st["window_bytes"] > 0
@@ -66,7 +42,7 @@ def test_writer_frames_equal_the_oracle(ctx, kw, lz):
 def test_token_frames_equal_the_model(ctx, name, mode):
     frame, data, _ = L.token_frame(name, mode)
     for lanes in (1, 2, 4):
-        (out,), (planes,), st, _ = gpu_decode(ctx, [data], lanes)
+        (out,), (planes,), st = gpu_decode(ctx, [data], lanes, lz77_stats=True)
         assert np.array_equal(np.asarray(planes).reshape(-1), L.model_planes(frame).reshape(-1).astype(np.int32))
         assert np.array_equal(out, frame.u8)
         assert st["lz77_streams"] > 0
@@ -75,7 +51,7 @@ def test_token_frames_equal_the_model(ctx, name, mode):
 def test_copy_at_distance_two_to_the_twenty(ctx):
     planes, data, _ = L.long_stream_frame()
     for lanes in (1, 4):
-        _, (got,), st, _ = gpu_decode(ctx, [data], lanes)
+        _, (got,), st = gpu_decode(ctx, [data], lanes, lz77_stats=True)
         assert np.array_equal(got, planes.astype(np.int32))
         assert st["lz77_streams"] == 2 and st["window_bytes"] == 2 * 4 << 20
 
@@ -89,11 +65,11 @@ def test_mixed_batch(ctx):
     files = [synth.encode_modular(w, h, 7, source=src, lz77=1), synth.encode_modular(w, h, 7, source=src, lz77=0),
              synth.encode_modular(w, h, 7, source=src, tree_kind=2, lz77=2)]
     for lanes in (1, 2, 4):
-        outs, planes, st, _ = gpu_decode(ctx, files, lanes)
+        outs, planes, st = gpu_decode(ctx, files, lanes, lz77_stats=True)
         assert st["lz77_streams"] == 18 and st["rle_streams"] == 9, st
         for o in outs:
             assert np.array_equal(o, src)
-        (alone_out,), (alone_planes,), st0, _ = gpu_decode(ctx, files[1:2], lanes)
+        (alone_out,), (alone_planes,), st0 = gpu_decode(ctx, files[1:2], lanes, lz77_stats=True)
         assert st0["lz77_streams"] == 0
         assert np.array_equal(alone_planes, planes[1]) and np.array_equal(alone_out, outs[1])
 
@@ -104,7 +80,7 @@ def test_lz77_errors_are_reported(ctx, fault):
     good_frame, good, _ = L.token_frame("ans_tree", 2, lz=L.ERROR_LZ)
     _, bad, _ = L.token_frame("ans_tree", 2, fault=(fault, 4), lz=L.ERROR_LZ)
     for lanes in (1, 4):
-        (out, _), (planes, _), _, err = gpu_decode(ctx, [good, bad], lanes, expect_error=True)
+        (out, _), (planes, _), err = gpu_decode(ctx, [good, bad], lanes, expect_error=True)
         assert err is not None and err.code == -10 and "frame 1 group 2" in str(err), err
         assert np.array_equal(np.asarray(planes).reshape(-1), L.model_planes(good_frame).reshape(-1).astype(np.int32))
         assert np.array_equal(out, good_frame.u8)
@@ -115,6 +91,6 @@ def test_large_run_length_frame(ctx):
     w = h = 4096
     src = L.flat_picture(w, h, 2)
     data = synth.encode_modular(w, h, 1, source=src, lz77=1)
-    (out,), _, st, _ = gpu_decode(ctx, [data], 4)
+    (out,), _, st = gpu_decode(ctx, [data], 4, lz77_stats=True)
     assert np.array_equal(out, src)
     assert st["lz77_streams"] == 256 and st["rle_streams"] == 256

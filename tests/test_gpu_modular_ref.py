@@ -8,6 +8,7 @@ import pytest
 from jxl_rs_b200 import abi
 from tests import modular_ref as M
 from tests import test_modular_ref as T
+from tests.gpu_modular import gpu_decode
 
 pytestmark = pytest.mark.gpu
 
@@ -18,23 +19,6 @@ def ctx():
     c = j.JxgContext(0)
     yield c
     c.close()
-
-
-def gpu_decode(ctx, files, lanes=1):
-    import torch
-    import jxl_rs_b200 as j
-    frames = [j.ModularParsedFrame(f) for f in files]
-    outs = [torch.empty((fr.height, fr.width, 3), dtype=torch.uint8).pin_memory() for fr in frames]
-    b = j.ModularBatch(ctx, lanes)
-    try:
-        for fr, o in zip(frames, outs):
-            b.add(fr, o.data_ptr(), fr.width * 3, False)
-        b.run()
-        b.wait()
-        planes = [b.read_planes(i) for i in range(len(frames))]
-    finally:
-        b.close()
-    return [o.numpy().copy() for o in outs], planes
 
 
 def _check(frame, out, planes):

@@ -9,6 +9,7 @@ import pytest
 from jxl_rs_b200 import abi
 from tests import modular_ref as M
 from tests import test_gpu_modular_ref as G
+from tests.gpu_modular import gpu_decode
 from tests import test_modular_squeeze as S
 
 pytestmark = pytest.mark.gpu
@@ -26,14 +27,14 @@ def _check(frame, out, planes):
 def test_device_equals_model(ctx, name):
     frame, data = S.model(name)
     for lanes in (1, 2, 4):
-        (out,), (planes,) = G.gpu_decode(ctx, [data], lanes)
+        (out,), (planes,) = gpu_decode(ctx, [data], lanes)
         _check(frame, out, planes)
 
 
 def test_local_squeeze_is_unsupported(ctx):
     _, data = S.model("local_squeeze")
     with pytest.raises(abi.JxgError) as e:
-        G.gpu_decode(ctx, [data])
+        gpu_decode(ctx, [data])
     assert e.value.code == -2, e.value  # JXG_ERR_UNSUPPORTED
 
 
@@ -42,7 +43,7 @@ def test_squeeze_refusals_on_device(ctx, name, size, bad, good):
     import synth
     G._refused_on_device(ctx, synth.encode_modular_tokens(S.refusal_frame(size, bad, False).spec))
     f = S.refusal_frame(size, good, True)
-    (out,), (planes,) = G.gpu_decode(ctx, [synth.encode_modular_tokens(f.spec)])
+    (out,), (planes,) = gpu_decode(ctx, [synth.encode_modular_tokens(f.spec)])
     _check(f, out, planes)
 
 
@@ -67,7 +68,7 @@ def test_batch_of_different_sizes(ctx):
     frames = [_steps_frame(w, h, STEPS, 40 + i) for i, (w, h) in enumerate([(300, 150), (9, 5), (64, 64), (131, 20),
                                                                             (50, 37)])]
     for lanes in (1, 4):
-        outs, planes = G.gpu_decode(ctx, [d for _, d in frames], lanes)
+        outs, planes = gpu_decode(ctx, [d for _, d in frames], lanes)
         for (f, _), o, p in zip(frames, outs, planes):
             _check(f, o, p)
 
@@ -78,33 +79,9 @@ def test_step_lists_that_are_prefixes_in_either_order(ctx):
     short = _steps_frame(70, 50, STEPS[2:], 50)  # its plan is the first four levels of the long one's
     long_ = _steps_frame(80, 40, STEPS, 51)
     for pair in ((short, long_), (long_, short)):
-        outs, planes = G.gpu_decode(ctx, [d for _, d in pair], 2)
+        outs, planes = gpu_decode(ctx, [d for _, d in pair], 2)
         for (f, _), o, p in zip(pair, outs, planes):
             _check(f, o, p)
-
-
-def _rollback_run(ctx, files, refused):
-    import torch
-    import jxl_rs_b200 as j
-    frames = [j.ModularParsedFrame(f) for f in files]
-    outs = [torch.empty((fr.height, fr.width, 3), dtype=torch.uint8).pin_memory() for fr in frames]
-    b = j.ModularBatch(ctx, 2)
-    try:
-        kept = []
-        for i, (fr, o) in enumerate(zip(frames, outs)):
-            if i == refused:
-                with pytest.raises(abi.JxgError):
-                    b.add(fr, o.data_ptr(), fr.width * 3, False)
-            else:
-                b.add(fr, o.data_ptr(), fr.width * 3, False)
-                kept.append(i)
-        stats = b.lz77_stats()
-        b.run()
-        b.wait()
-        planes = [b.read_planes(k) for k in range(len(kept))]
-    finally:
-        b.close()
-    return [outs[i].numpy().copy() for i in kept], planes, stats
 
 
 def test_refused_frame_leaves_the_batch_unchanged(ctx):
@@ -114,10 +91,10 @@ def test_refused_frame_leaves_the_batch_unchanged(ctx):
     a = _steps_frame(140, 60, STEPS, 60, lz={})
     c = _steps_frame(96, 70, STEPS, 61, lz={})
     b = _steps_frame(140, 60, [(False, True, 0, 3), (True, True, 0, 3)], 62, lz={"fault": (1, 2)})
-    _, alone, alone_stats = _rollback_run(ctx, [a[1], c[1]], None)
+    _, alone, alone_stats = gpu_decode(ctx, [a[1], c[1]], 2, lz77_stats=True)
     assert alone_stats["lz77_streams"] > 0
     for first, last in ((a, c), (c, a)):
-        outs, planes, stats = _rollback_run(ctx, [first[1], b[1], last[1]], 1)
+        outs, planes, stats = gpu_decode(ctx, [first[1], b[1], last[1]], 2, lz77_stats=True, refused=(1,))
         assert stats == alone_stats, (stats, alone_stats)
         for (f, _), o, p in zip((first, last), outs, planes):
             _check(f, o, p)
