@@ -2310,12 +2310,15 @@ __device__ __forceinline__ uint16_t sample16(const FrameDev& F, float v) {
 //   stage evaluates out-of-image cells at the mirrored coordinate, so halo
 //   cells hold exactly what the reference's mirror-padded rows hold
 //   (render/simple_pipeline/run_stage.rs:127-134) and stages chain in the tile.
-// * EPF sums of absolute differences are built from channel-combined difference
-//   maps D_o(c) = sum_ch scale_ch * |I_ch(c) - I_ch(c + o)| shared by all pixels
-//   (epf0.rs:157-168 / epf1.rs:98-101 evaluate the same sums per pixel).
+// * EPF sums of absolute differences are built from channel-combined differences
+//   D_o(c) = sum_ch scale_ch * |I_ch(c) - I_ch(c + o)| (epf0.rs:157-168 /
+//   epf1.rs:98-101 evaluate the same sums per pixel). EPF stage 0 stores its six
+//   difference maps in shared memory; stages 1 and 2 need only D_(1,0) and
+//   D_(0,1) and recompute them from the source cells, which keeps the Gaborish +
+//   EPF 2 tile at two plane buffers (69 KB) and spares each stage a barrier.
 // * HBM traffic: one read of the IDCT planes (+ halo) and one write of the output.
 // ===========================================================================
-constexpr int kTW = 64, kTH = 32, kFilterThreads = 512;
+constexpr int kTW = 64, kTH = 32;
 
 struct FusedTiles {
   const uint32_t* tile_prefix;  // [num_frames + 1], kTW x kTH tiles
@@ -2328,9 +2331,15 @@ template <bool GAB, int EPF>
 struct FCfg {
   static constexpr int H = (GAB ? 1 : 0) + (EPF >= 3 ? 3 : 0) + (EPF >= 1 ? 2 : 0) + (EPF >= 2 ? 1 : 0);
   static constexpr int WW = kTW + 2 * H, WH = kTH + 2 * H, NC = WW * WH;
-  static constexpr int NMAPS = EPF >= 3 ? 6 : (EPF >= 1 ? 2 : 0);
+  static constexpr int NMAPS = EPF >= 3 ? 6 : 0;  // only EPF stage 0 reads stored maps; stages 1 and 2 recompute theirs
   static constexpr int SBW = WW / 8 + 2, SBH = WH / 8 + 2;  // sigma blocks covering the window
   static constexpr size_t kSmemBytes = sizeof(float) * (size_t(6 + NMAPS) * NC + SBW * SBH);
+  // EPF <= 2 tiles (<= 69 KB): 384 threads at <= 56 registers, 3 CTAs per SM. At 512 threads the same 3 CTAs need <= 40
+  // registers, where the vector path spills (176 B stored / 232 B loaded per thread) and filters a 4K batch 22 % slower
+  // (DESIGN §7). The EPF 3 tile (172 KB) fits one CTA per SM at any size, so it keeps 512 threads: at 384 it has a
+  // quarter fewer warps per SM, and config 4 then measured 8 % slower than with stored maps at 512 threads.
+  static constexpr int kThreads = EPF >= 3 ? 512 : 384;
+  static constexpr int kMinCtas = EPF >= 3 ? 1 : 3;
 };
 
 // Cell -> source position. INTERIOR tiles (window fully inside the image) skip every range / mirror computation.
@@ -2350,18 +2359,17 @@ __device__ __forceinline__ bool cell_source(int lx, int ly, int wx0, int wy0, in
   return true;
 }
 
-// One EPF stage. src/dst: [3][NC]; maps: [NMAPS][NC]; M = margin of the output region (compile time).
+// One EPF stage. src/dst: [3][NC]; maps: [6][NC], stage 0 only; M = margin of the output region (compile time).
 template <int STAGE, int WW, int WH, int H, int SBW, int M, bool INTERIOR>
 __device__ __forceinline__ void epf_stage(const FrameDev& F, const float* src, float* dst, float* maps, const float* sig,
                                           int wx0, int wy0, int sbx0, int sby0) {
   constexpr int NC = WW * WH;
   const int w = int(F.width), h = int(F.height);
   const float s0 = F.epf_channel_scale[0], s1 = F.epf_channel_scale[1], s2 = F.epf_channel_scale[2];
-  constexpr int B = STAGE == 0 ? 3 : (STAGE == 1 ? 2 : 1);  // border of this stage
-  constexpr int MP = M - B;                                   // margin of valid source cells
-  // ---- phase A: difference maps over the source-valid area ----
-  {
-    constexpr int NO = STAGE == 0 ? 6 : 2;
+  // ---- phase A (stage 0): difference maps over the source-valid area ----
+  if (STAGE == 0) {
+    constexpr int NO = 6;
+    constexpr int MP = M - 3;  // margin of valid source cells
     constexpr int ox[6] = {1, 0, 2, 0, 1, 1}, oy[6] = {0, 1, 0, 2, 1, -1};  // (1,0) (0,1) (2,0) (0,2) (1,1) (1,-1)
     constexpr int aw = WW - 2 * MP, ah = WH - 2 * MP;
     for (int idx = threadIdx.x; idx < aw * ah; idx += blockDim.x) {
@@ -2376,16 +2384,20 @@ __device__ __forceinline__ void epf_stage(const FrameDev& F, const float* src, f
         maps[k * NC + o] = fmaf(fabsf(src[on] - c0), s0, fmaf(fabsf(src[NC + on] - c1), s1, fabsf(src[2 * NC + on] - c2) * s2));
       }
     }
+    __syncthreads();
   }
-  __syncthreads();
   // ---- phase B ----
   const float kMinSigma = -3.90524291751269967465540850526868f;
   const float sigma_scale = STAGE == 0 ? F.epf_pass0_sigma_scale : (STAGE == 1 ? 1.0f : F.epf_pass2_sigma_scale);
   const float sm = sigma_scale * 1.65f, bsm = sm * F.epf_border_sad_mul;
   constexpr int R = H - M;  // halo still needed after this stage
   constexpr int bw_ = kTW + 2 * R, bh_ = kTH + 2 * R;
-  const float* Dh = maps;       // (1,0)
-  const float* Dv = maps + NC;  // (0,1)
+  // D_(1,0) and D_(0,1) at cell c, summed as phase A sums them
+  auto diff = [&](int a, int b) {
+    return fmaf(fabsf(src[b] - src[a]), s0, fmaf(fabsf(src[NC + b] - src[NC + a]), s1, fabsf(src[2 * NC + b] - src[2 * NC + a]) * s2));
+  };
+  auto Dh = [&](int c) { return STAGE == 0 ? maps[c] : diff(c, c + 1); };
+  auto Dv = [&](int c) { return STAGE == 0 ? maps[NC + c] : diff(c, c + WW); };
   for (int idx = threadIdx.x; idx < bw_ * bh_; idx += blockDim.x) {
     const int lx = M + idx % bw_, ly = M + idx / bw_;
     int o, mx, my;
@@ -2401,7 +2413,7 @@ __device__ __forceinline__ void epf_stage(const FrameDev& F, const float* src, f
     const float inv_s = inv_sigma_px * (border ? bsm : sm);
     if (STAGE == 2) {
       // neighbours in the reference's order: up, left, right, down (epf2.rs:83)
-      const float sad[4] = {Dv[o - WW], Dh[o - 1], Dh[o], Dv[o]};
+      const float sad[4] = {Dv(o - WW), Dh(o - 1), Dh(o), Dv(o)};
       const int offs[4] = {-WW, -1, 1, WW};
       float wacc = 1.0f, acc[3] = {src[o], src[NC + o], src[2 * NC + o]};
 #pragma unroll
@@ -2416,9 +2428,7 @@ __device__ __forceinline__ void epf_stage(const FrameDev& F, const float* src, f
       for (int c = 0; c < 3; c++) dst[c * NC + od] = acc[c] * inv_w;
       continue;
     }
-    auto plus_sum = [&](const float* Mp, int base) {
-      return Mp[base - WW] + Mp[base - 1] + Mp[base] + Mp[base + 1] + Mp[base + WW];
-    };
+    auto plus_sum = [&](auto D, int base) { return D(base - WW) + D(base - 1) + D(base) + D(base + 1) + D(base + WW); };
     if (STAGE == 1) {
       const float sad[4] = {plus_sum(Dv, o - WW), plus_sum(Dh, o - 1), plus_sum(Dh, o), plus_sum(Dv, o)};
       const int offs[4] = {-WW, -1, 1, WW};
@@ -2440,10 +2450,10 @@ __device__ __forceinline__ void epf_stage(const FrameDev& F, const float* src, f
       continue;
     }
     // STAGE 0: 12 neighbours (epf0.rs:182-195 order)
-    const float* MB = maps + 2 * NC;  // (2,0)
-    const float* MD = maps + 3 * NC;  // (0,2)
-    const float* ME = maps + 4 * NC;  // (1,1)
-    const float* MF = maps + 5 * NC;  // (1,-1)
+    auto MB = [&](int c) { return maps[2 * NC + c]; };  // (2,0)
+    auto MD = [&](int c) { return maps[3 * NC + c]; };  // (0,2)
+    auto ME = [&](int c) { return maps[4 * NC + c]; };  // (1,1)
+    auto MF = [&](int c) { return maps[5 * NC + c]; };  // (1,-1)
     const int offs[12] = {-2 * WW, -WW - 1, -WW, -WW + 1, -2, -1, 1, 2, WW - 1, WW, WW + 1, 2 * WW};
     const float sad[12] = {
         plus_sum(MD, o - 2 * WW), plus_sum(ME, o - WW - 1), plus_sum(Dv, o - WW), plus_sum(MF, o),
@@ -2620,8 +2630,9 @@ __device__ __forceinline__ void filter_tile(const BatchDev& B, const FrameDev& F
 
 // ---------------------------------------------------------------------------
 // Vectorised interior path of the default filter configuration (Gaborish + EPF iters 2, halo 4): every thread owns
-// quads of 4 horizontally adjacent cells, loads rows with 16-byte shared-memory accesses, shares the 3-tap sums of
-// the difference maps between the four cells, and converts / stores its four pixels straight from registers.
+// quads of 4 horizontally adjacent cells, loads rows with 16-byte shared-memory accesses, computes the EPF differences
+// of its quad and their plus-shaped sums once for the four cells, and converts / stores its four pixels straight from
+// registers.
 // Same arithmetic as the scalar path except for the association of a few float sums and the approximate
 // sqrt / divide of the sRGB curve (<= 3 ulp), both far inside the 1e-3 / 1 LSB parity tolerances.
 // ---------------------------------------------------------------------------
@@ -2644,31 +2655,15 @@ __device__ __forceinline__ float linear_to_srgb_fast(float v) {  // color/tf.rs:
   return copysignf(r, v);
 }
 
-// EPF difference maps (channel-combined |a - right|, |a - below|) for the rows [r0, r1) of `src`, all quads.
-template <int WW, int NC>
-__device__ __forceinline__ void epf_maps_v4(const float* src, float* maps, int r0, int r1, float s0, float s1, float s2) {
-  constexpr int QW = WW / 4;
-  for (int q = threadIdx.x; q < QW * (r1 - r0); q += blockDim.x) {
-    const int ly = r0 + q / QW, o = ly * WW + (q % QW) * 4;
-    float dh[4] = {0, 0, 0, 0}, dv[4] = {0, 0, 0, 0};
+// Channel-combined EPF differences of one row segment, accumulated one channel at a time (channel 0, 1, 2, each
+// term fmaf(|a - b|, scale, sum) from 0): dh[i] = D_(1,0) of cell a[i], dv[i] = D_(0,1) of cell a[i + DA] whose lower
+// neighbour is b[i + DB].
+template <int NH, int NV, int DA, int DB>
+__device__ __forceinline__ void acc_diffs(float* dh, float* dv, const float* a, const float* b, float sc) {
 #pragma unroll
-    for (int c = 0; c < 3; c++) {
-      const float sc = c == 0 ? s0 : (c == 1 ? s1 : s2);
-      const float* p = src + c * NC + o;
-      const float4 m = ld4(p), d = ld4(p + WW);
-      const float r = p[4];
-      dh[0] = fmaf(fabsf(m.x - m.y), sc, dh[0]);
-      dh[1] = fmaf(fabsf(m.y - m.z), sc, dh[1]);
-      dh[2] = fmaf(fabsf(m.z - m.w), sc, dh[2]);
-      dh[3] = fmaf(fabsf(m.w - r), sc, dh[3]);
-      dv[0] = fmaf(fabsf(m.x - d.x), sc, dv[0]);
-      dv[1] = fmaf(fabsf(m.y - d.y), sc, dv[1]);
-      dv[2] = fmaf(fabsf(m.z - d.z), sc, dv[2]);
-      dv[3] = fmaf(fabsf(m.w - d.w), sc, dv[3]);
-    }
-    st4(maps + o, make_float4(dh[0], dh[1], dh[2], dh[3]));
-    st4(maps + NC + o, make_float4(dv[0], dv[1], dv[2], dv[3]));
-  }
+  for (int i = 0; i < NH; i++) dh[i] = fmaf(fabsf(a[i] - a[i + 1]), sc, dh[i]);
+#pragma unroll
+  for (int i = 0; i < NV; i++) dv[i] = fmaf(fabsf(a[i + DA] - b[i + DB]), sc, dv[i]);
 }
 
 // Sigma of every 8x8 block touched by a tile's window (features/epf.rs:54-79).
@@ -2697,9 +2692,9 @@ struct TileRef {
 };
 
 // Gaborish + EPF iters 2 on an interior tile, four pixels per thread: bufA receives the tile's window, bufB is the
-// second plane buffer.
+// second plane buffer. Three barriers: after the load, after Gaborish and after EPF stage 1.
 __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev& F, const float* src_planes, float* bufA,
-                                               float* bufB, float* maps, float* sig, int x0, int y0) {
+                                               float* bufB, float* sig, int x0, int y0) {
   using C = FCfg<true, 2>;
   constexpr int H = 4, WW = C::WW, WH = C::WH, NC = C::NC, QW = WW / 4;
   static_assert(C::H == H && WW == 72 && WH == 40, "vector path is written for the halo-4 configuration");
@@ -2734,14 +2729,9 @@ __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev
     }
   }
   __syncthreads();
-  const float cs0 = F.epf_channel_scale[0], cs1 = F.epf_channel_scale[1], cs2 = F.epf_channel_scale[2];
   const float kMinSigma = -3.90524291751269967465540850526868f;
-  // ---- EPF stage 1 (epf1.rs): maps of bufB rows 1..38, then rows 3..36 -> bufA ----
-  epf_maps_v4<WW, NC>(bufB, maps, 1, WH - 1, cs0, cs1, cs2);
-  __syncthreads();
+  // ---- EPF stage 1 (epf1.rs): bufB rows 3..36 -> bufA ----
   {
-    const float* Dh = maps;
-    const float* Dv = maps + NC;
     const float sm = 1.65f, bsm = sm * F.epf_border_sad_mul;
     for (int q = threadIdx.x; q < QW * (WH - 6); q += blockDim.x) {
       const int ly = 3 + q / QW, lx = (q % QW) * 4, o = ly * WW + lx;
@@ -2756,34 +2746,79 @@ __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev
       const float is_n = inv_sigma_px * (rowb ? bsm : sm), is_b = inv_sigma_px * bsm;
       const bool lo4 = (mx & 4) == 0;  // quad covers columns 0..3 (border at cell 0) or 4..7 (border at cell 3)
       const float isg[4] = {lo4 ? is_b : is_n, is_n, is_n, lo4 ? is_n : is_b};
-      // plus-shaped sums of Dh at columns x-1 .. x+3 (left / right SADs of the four cells)
-      float ph[5];
-      {
-        const float* p = Dh + o;
-        const float2 l2 = *reinterpret_cast<const float2*>(p - 2);
-        const float4 m = ld4(p), u = ld4(p - WW), d = ld4(p + WW);
-        const float r = p[4], ul = p[-WW - 1], dl = p[WW - 1];
-        ph[0] = l2.x + l2.y + m.x + ul + dl;
-        ph[1] = l2.y + m.x + m.y + u.x + d.x;
-        ph[2] = m.x + m.y + m.z + u.y + d.y;
-        ph[3] = m.y + m.z + m.w + u.z + d.z;
-        ph[4] = m.z + m.w + r + u.w + d.w;
+      // Plus-shaped sums of the differences of bufB: ph of Dh at columns x-1 .. x+3 (left / right SADs of the four
+      // cells), pu / pd of Dv at rows y-1 (up SAD) and y (down SAD). The difference rows are taken top to bottom,
+      // each folded into the sums as soon as its three channels are in, so that few stay live.
+      float ph[5], pu[4], pd[4], hu[5] = {};
+      auto row = [&](const float* p, float* r6) {  // cells x-1 .. x+4 of the row at p
+        const float4 v = ld4(p);
+        r6[0] = p[-1]; r6[1] = v.x; r6[2] = v.y; r6[3] = v.z; r6[4] = v.w; r6[5] = p[4];
+      };
+      {  // Dv at row y-2 (columns x .. x+3)
+        float va[4] = {};
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+          const float* p = bufB + c * NC + o;
+          const float4 a = ld4(p - 2 * WW), b = ld4(p - WW);
+          const float r0[4] = {a.x, a.y, a.z, a.w}, r1[4] = {b.x, b.y, b.z, b.w};
+          acc_diffs<0, 4, 0, 0>(nullptr, va, r0, r1, F.epf_channel_scale[c]);
+        }
+#pragma unroll
+        for (int i = 0; i < 4; i++) pu[i] = va[i];
       }
-      // plus-shaped sums of Dv at rows y-1 (up SAD) and y (down SAD)
-      float pu[4], pd[4];
-      {
-        const float* p = Dv + o;
-        const float4 a = ld4(p - 2 * WW), b = ld4(p - WW), m = ld4(p), e = ld4(p + WW);
-        const float bl = p[-WW - 1], br = p[-WW + 4], ml = p[-1], mr = p[4];
-        pu[0] = a.x + bl + b.x + b.y + m.x;
-        pu[1] = a.y + b.x + b.y + b.z + m.y;
-        pu[2] = a.z + b.y + b.z + b.w + m.z;
-        pu[3] = a.w + b.z + b.w + br + m.w;
-        pd[0] = b.x + ml + m.x + m.y + e.x;
-        pd[1] = b.y + m.x + m.y + m.z + e.y;
-        pd[2] = b.z + m.y + m.z + m.w + e.z;
-        pd[3] = b.w + m.z + m.w + mr + e.w;
+      {  // Dh at row y-1 (x-1 .. x+3), Dv at row y-1 (x-1 .. x+4)
+        float vb[6] = {};
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+          const float* p = bufB + c * NC + o;
+          float r1[6], r2[6];
+          row(p - WW, r1);
+          row(p, r2);
+          acc_diffs<5, 6, 0, 0>(hu, vb, r1, r2, F.epf_channel_scale[c]);
+        }
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+          pu[i] = pu[i] + vb[i] + vb[i + 1] + vb[i + 2];
+          pd[i] = vb[i + 1];
+        }
       }
+      {  // Dh at row y (x-2 .. x+4), Dv at row y (x-1 .. x+4)
+        float hm[7] = {}, vm[6] = {};
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+          const float* p = bufB + c * NC + o;
+          const float4 m = ld4(p);
+          const float2 ml = *reinterpret_cast<const float2*>(p - 2), mr = *reinterpret_cast<const float2*>(p + 4);
+          const float r2[8] = {ml.x, ml.y, m.x, m.y, m.z, m.w, mr.x, mr.y};
+          float r3[6];
+          row(p + WW, r3);
+          acc_diffs<7, 6, 1, 0>(hm, vm, r2, r3, F.epf_channel_scale[c]);
+        }
+#pragma unroll
+        for (int i = 0; i < 5; i++) ph[i] = hm[i] + hm[i + 1] + hm[i + 2] + hu[i];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+          pu[i] = pu[i] + vm[i + 1];
+          pd[i] = pd[i] + vm[i] + vm[i + 1] + vm[i + 2];
+        }
+      }
+      {  // Dh at row y+1 (x-1 .. x+3), Dv at row y+1 (x .. x+3)
+        float hd[5] = {}, ve[4] = {};
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+          const float* p = bufB + c * NC + o;
+          float r3[6];
+          row(p + WW, r3);
+          const float4 e = ld4(p + 2 * WW);
+          const float r4[4] = {e.x, e.y, e.z, e.w};
+          acc_diffs<5, 4, 1, 0>(hd, ve, r3, r4, F.epf_channel_scale[c]);
+        }
+#pragma unroll
+        for (int i = 0; i < 5; i++) ph[i] = ph[i] + hd[i];
+#pragma unroll
+        for (int i = 0; i < 4; i++) pd[i] = pd[i] + ve[i];
+      }
+      asm volatile("" ::: "memory");  // reload the rows below rather than keep all three channels live from above
       float wu[4], wl[4], wr[4], wd[4], iw[4];
 #pragma unroll
       for (int i = 0; i < 4; i++) {
@@ -2809,12 +2844,7 @@ __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev
   }
   __syncthreads();
   // ---- EPF stage 2 (epf2.rs) on the 64x32 core + colour + store ----
-  epf_maps_v4<WW, NC>(bufA, maps, 3, WH - 3, cs0, cs1, cs2);
-  __syncthreads();
   {
-    const float* Dh = maps;
-    const float* Dv = maps + NC;
-    const float sm = F.epf_pass2_sigma_scale * 1.65f, bsm = sm * F.epf_border_sad_mul;
     const int w = int(F.width);
     uint8_t* out_base = static_cast<uint8_t*>(F.out_ptr);
     for (int q = threadIdx.x; q < (kTW / 4) * kTH; q += blockDim.x) {
@@ -2829,14 +2859,25 @@ __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev
           px[c][0] = m.x; px[c][1] = m.y; px[c][2] = m.z; px[c][3] = m.w;
         }
       } else {
+        const float sm = F.epf_pass2_sigma_scale * 1.65f, bsm = sm * F.epf_border_sad_mul;  // read here: no register to spare
         const bool rowb = ((my + 1) & 7) < 2;
         const float is_n = inv_sigma_px * (rowb ? bsm : sm), is_b = inv_sigma_px * bsm;
         const bool lo4 = (mx & 4) == 0;
         const float isg[4] = {lo4 ? is_b : is_n, is_n, is_n, lo4 ? is_n : is_b};
-        const float4 su = ld4(Dv + o - WW), sd = ld4(Dv + o), sh = ld4(Dh + o);
-        const float shl = Dh[o - 1];
-        const float sup[4] = {su.x, su.y, su.z, su.w}, sdn[4] = {sd.x, sd.y, sd.z, sd.w};
-        const float shh[5] = {shl, sh.x, sh.y, sh.z, sh.w};
+        // differences of bufA: Dv at rows y-1 and y (columns x .. x+3), Dh at row y (x-1 .. x+3)
+        float sup[4] = {}, shh[5] = {}, sdn[4] = {};
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+          const float sc = F.epf_channel_scale[c];
+          const float* p = bufA + c * NC + o;
+          const float4 u = ld4(p - WW), m = ld4(p), d = ld4(p + WW);
+          const float r0[4] = {u.x, u.y, u.z, u.w};
+          const float r1[6] = {p[-1], m.x, m.y, m.z, m.w, p[4]};
+          const float r2[4] = {d.x, d.y, d.z, d.w};
+          acc_diffs<0, 4, 0, 1>(nullptr, sup, r0, r1, sc);
+          acc_diffs<5, 4, 1, 0>(shh, sdn, r1, r2, sc);
+        }
+        asm volatile("" ::: "memory");  // as in EPF stage 1
         float wu[4], wl[4], wr[4], wd[4], iw[4];
 #pragma unroll
         for (int i = 0; i < 4; i++) {
@@ -2948,7 +2989,7 @@ __device__ __forceinline__ TileRef locate_tile(const BatchDev& B, const FusedTil
 }
 
 template <bool GAB, int EPF>
-__global__ void __launch_bounds__(kFilterThreads) k_filters_store(const BatchDev B, const FusedTiles T, const float* src_planes) {
+__global__ void __launch_bounds__(FCfg<GAB, EPF>::kThreads, FCfg<GAB, EPF>::kMinCtas) k_filters_store(const BatchDev B, const FusedTiles T, const float* src_planes) {
   using C = FCfg<GAB, EPF>;
   extern __shared__ float smem[];
   const TileRef r = locate_tile<GAB, EPF>(B, T, blockIdx.x + T.tile_begin);
@@ -2956,8 +2997,7 @@ __global__ void __launch_bounds__(kFilterThreads) k_filters_store(const BatchDev
   const FrameDev& F = *r.F;
   const bool interior = r.x0 - C::H >= 0 && r.y0 - C::H >= 0 && r.x0 + kTW + C::H <= int(F.width) && r.y0 + kTH + C::H <= int(F.height);
   if (GAB && EPF == 2 && r.vec) {
-    __shared__ float s_sig[FCfg<true, 2>::SBW * FCfg<true, 2>::SBH];
-    filter_tile_v4(B, F, src_planes, smem, smem + 3 * FCfg<true, 2>::NC, smem + 6 * FCfg<true, 2>::NC, s_sig, r.x0, r.y0);
+    filter_tile_v4(B, F, src_planes, smem, smem + 3 * FCfg<true, 2>::NC, smem + 6 * FCfg<true, 2>::NC, r.x0, r.y0);
   } else if (interior) {
     filter_tile<GAB, EPF, true>(B, F, src_planes, smem, r.x0, r.y0);
   } else {
@@ -2974,7 +3014,7 @@ int sm_count() {
 
 template <bool GAB, int EPF>
 static void launch_filters(const BatchDev& B, const FusedTiles& FT, uint32_t tiles, cudaStream_t stream) {
-  k_filters_store<GAB, EPF><<<tiles, kFilterThreads, FCfg<GAB, EPF>::kSmemBytes, stream>>>(B, FT, B.planes_a);
+  k_filters_store<GAB, EPF><<<tiles, FCfg<GAB, EPF>::kThreads, FCfg<GAB, EPF>::kSmemBytes, stream>>>(B, FT, B.planes_a);
 }
 template <bool GAB, int EPF>
 static cudaError_t configure_filters() {
