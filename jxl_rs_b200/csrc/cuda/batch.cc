@@ -62,7 +62,7 @@ struct FrameOut {
 struct Batch : BatchCore {
   PinnedArena& blob;
   explicit Batch(Context* c)
-      : blob(c->blob), d_blob(c->d_blob), d_coeffs(c->d_coeffs), d_block_off(c->d_block_off), d_nz(c->d_nz),
+      : blob(c->blob), d_blob(c->d_blob), d_coeffs(c->d_coeffs), d_block_off(c->d_block_off),
         d_planes_a(c->d_planes_a), d_status(c->d_status), d_out(c->d_out) {}
   std::vector<FrameDev> frames;
   std::vector<SectionDev> sections;
@@ -72,21 +72,20 @@ struct Batch : BatchCore {
   uint32_t lean_S = 1, lean_ctas = 0;  // k_entropy_lean schedule (see schedule_lean)
   std::vector<uint32_t> lean_cta_first;
   std::vector<uint2> lean_warps;  // per warp of k_entropy_lean: first stream (relative to its frame's list), lanes
-  std::vector<uint64_t> nz_base;
   std::vector<uint32_t> fused_prefix{0};
   std::vector<FrameOut> outs;
-  uint64_t total_groups = 0, total_blocks = 0, total_plane_floats = 0, nz_bytes = 0, out_bytes = 0, orient_bytes = 0;
+  uint64_t total_groups = 0, total_blocks = 0, total_plane_floats = 0, out_bytes = 0, orient_bytes = 0;
   uint32_t lz_windows = 0;
   uint32_t filter_cfg_mask = 0;  // bit (gab * 4 + min(epf_iters, 3))
   int debug_stop = 0;
   // device
-  DevBuf &d_blob, &d_coeffs, &d_block_off, &d_nz, &d_planes_a, &d_status, &d_out;
+  DevBuf &d_blob, &d_coeffs, &d_block_off, &d_planes_a, &d_status, &d_out;
   // byte offsets of the batch tables inside the blob (they ride on the one pinned H2D copy: a cudaMemcpyAsync from
   // pageable std::vector storage blocks the calling thread until earlier device work drains, which takes long with
   // other batches in flight)
   struct {
     uint64_t frames = 0, sections = 0, streams = 0, lean_cta = 0, lean_warp = 0, streams_lean = 0, streams_fast = 0, streams_slow = 0,
-             nz_base = 0, ftiles = 0;
+             ftiles = 0;
   } tab;
   cudaEvent_t ev_handoff = nullptr;
   bool profile = false;
@@ -475,8 +474,6 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   for (uint32_t g = 0; g < F.num_groups; g++) {
     b->streams.push_back(StreamDev{uint32_t(b->frames.size()), g});
     ((F.num_passes != 1 || F.has_lz) ? b->streams_slow : ((F.passes[0].use_prefix || F.passes[0].shift != 0) ? b->streams_fast : b->streams_lean)).push_back(StreamDev{uint32_t(b->frames.size()), g});
-    b->nz_base.push_back(b->nz_bytes);
-    b->nz_bytes += size_t(F.num_passes) * 3072;
   }
   F.coeff_group_base = b->total_groups;
   b->total_groups += F.num_groups;
@@ -635,15 +632,13 @@ static BatchDev make_batch_dev(Batch* b) {
   B.nzlist = static_cast<uint32_t*>(b->d_coeffs.p);  // the pool that held the dense coefficients now holds the lists
   B.block_off = static_cast<uint32_t*>(b->d_block_off.p);
   B.lzwin = static_cast<uint32_t*>(b->ctx->d_lzwin.p);
-  B.nz = static_cast<uint8_t*>(b->d_nz.p);
-  B.nz_base = reinterpret_cast<uint64_t*>(const_cast<uint8_t*>(tab(b->tab.nz_base)));
   B.planes_a = static_cast<float*>(b->d_planes_a.p);
   B.status = static_cast<int32_t*>(b->d_status.p);
   B.queue = reinterpret_cast<uint32_t*>(B.status + b->streams.size());
   B.lean_cta_first = reinterpret_cast<const uint32_t*>(tab(b->tab.lean_cta));
   B.lean_warp = reinterpret_cast<const uint2*>(tab(b->tab.lean_warp));
-  B.desc = static_cast<uint4*>(b->ctx->d_lean_desc.p);
-  B.nblk = static_cast<uint32_t*>(b->ctx->d_lean_nblk.p);
+  B.desc = static_cast<uint4*>(b->ctx->d_desc.p);
+  B.nblk = static_cast<uint32_t*>(b->ctx->d_nblk.p);
   B.dequant_default = static_cast<const float*>(b->ctx->dequant_default.p);
   B.dequant_default_off = static_cast<const uint32_t*>(b->ctx->dequant_default_off.p);
   B.natural_orders = static_cast<const uint32_t*>(b->ctx->natural_orders.p);
@@ -743,12 +738,11 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
   if (int r = b->d_coeffs.ensure(b->sections.size() * size_t(kListStride) * 4)) return r;
   if (int r = b->d_block_off.ensure(b->total_blocks * 4)) return r;
   if (int r = b->ctx->d_lzwin.ensure(std::max<size_t>(size_t(b->lz_windows) * kLzWindow * 4, 16))) return r;
-  if (int r = b->d_nz.ensure(b->nz_bytes)) return r;
   if (int r = b->d_planes_a.ensure(b->total_plane_floats * 4)) return r;
   if (int r = b->d_status.ensure((b->streams.size() + b->frames.size() + 4) * 4)) return r;
   if (int r = b->d_out.ensure(std::max<size_t>(b->out_bytes, 16))) return r;
-  if (int r = b->ctx->d_lean_desc.ensure(std::max<size_t>(b->streams.size() * 1024 * 16, 16))) return r;
-  if (int r = b->ctx->d_lean_nblk.ensure(std::max<size_t>(b->streams.size() * 4, 16))) return r;
+  if (int r = b->ctx->d_desc.ensure(std::max<size_t>(b->streams.size() * 1024 * 16, 16))) return r;
+  if (int r = b->ctx->d_nblk.ensure(std::max<size_t>(b->streams.size() * 4, 16))) return r;
   if (int r = b->ctx->d_orient.ensure(std::max<size_t>(b->orient_bytes, 16))) return r;
   for (size_t f = 0; f < b->frames.size(); f++) {
     const FrameOut& fo = b->outs[f];
@@ -760,7 +754,7 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
       !batch_table(b->blob, b->streams, b->tab.streams) || !batch_table(b->blob, b->lean_cta_first, b->tab.lean_cta) ||
       !batch_table(b->blob, b->lean_warps, b->tab.lean_warp) || !batch_table(b->blob, b->streams_lean, b->tab.streams_lean) ||
       !batch_table(b->blob, b->streams_fast, b->tab.streams_fast) || !batch_table(b->blob, b->streams_slow, b->tab.streams_slow) ||
-      !batch_table(b->blob, b->nz_base, b->tab.nz_base) || !batch_table(b->blob, b->fused_prefix, b->tab.ftiles))
+      !batch_table(b->blob, b->fused_prefix, b->tab.ftiles))
     return set_error(JXG_ERR_CUDA, "pinned staging allocation failed");
   if (int r = b->d_blob.ensure(b->blob.size + 64)) return r;
   trace.mark("alloc");

@@ -136,7 +136,7 @@ struct Context {
   // intermediates and the pinned staging arena survive jxg_batch_end so that a
   // steady-state decode loop does no cudaMalloc / cudaHostAlloc.
   PinnedArena blob;
-  DevBuf d_blob, d_coeffs, d_block_off, d_nz, d_planes_a, d_status, d_out, d_lean_desc, d_lean_nblk, d_orient, d_lzwin,
+  DevBuf d_blob, d_coeffs, d_block_off, d_planes_a, d_status, d_out, d_desc, d_nblk, d_orient, d_lzwin,
       d_modular_lzwin, d_modular_wp;
   bool batch_live = false;
   // pinned status readback buffer, owned by the context: cudaHostAlloc / cudaFreeHost synchronise the whole

@@ -1,9 +1,9 @@
 // sm_90a kernels of the VarDCT hot path.
 //
-//   k_block_plan     varblock descriptors of every (frame, group) stream
+//   k_block_plan     K0  varblock descriptors of every (frame, group) stream, the block order of all three entropy kernels
 //   k_entropy_lean   K1  decode of the AC coefficients with the JPEG XL context model (jxl/src/frame/group.rs:454-578,
-//   k_entropy_fast       entropy_coding/*.rs): persistent lanes for single-pass ANS frames (lean), prefix-coded
-//   k_entropy            frames (fast), multi-pass and LZ77 frames
+//   k_entropy_fast       entropy_coding/*.rs): persistent lanes for single-pass ANS frames (lean), packed lanes for
+//   k_entropy            prefix-coded or shifted single-pass frames (fast), one lane per warp for multi-pass and LZ77 frames
 //   k_idct_small     K2  one CTA per group: dequant + chroma-from-luma + LLF + inverse variable-block DCT
 //   k_dequant_idct       (group.rs:100-250, jxl_transforms/src/transform.rs); small and large varblocks
 //   k_filters_store  K3-K5 fused Gaborish -> EPF 0/1/2 -> XYB -> output transfer curve -> store
@@ -53,362 +53,9 @@ __device__ float g_dither[1024] = {
 // K1: entropy decode
 // ===========================================================================
 
-// bit_reader.rs:15-219 restated for 32-bit word refills from an 8-byte aligned,
-// zero-padded section copy. Reads past the end return zeros (optimistic reads);
-// over-read is detected at the end (check_for_error, :109).
-struct DevBr {
-  const uint32_t* words;
-  uint32_t nwords, wpos;
-  uint64_t buf;
-  uint32_t bits, total;
-  __device__ __forceinline__ void init(const uint8_t* p, uint32_t len) {
-    words = reinterpret_cast<const uint32_t*>(p);
-    nwords = (len + 3) >> 2;
-    wpos = 0;
-    buf = 0;
-    bits = 0;
-    total = 0;
-  }
-  __device__ __forceinline__ void ensure(uint32_t n) {
-    if (bits < n) {
-      uint32_t w = wpos < nwords ? __ldg(words + wpos) : 0u;
-      wpos++;
-      buf |= uint64_t(w) << bits;
-      bits += 32;
-    }
-  }
-  __device__ __forceinline__ uint32_t peek(uint32_t n) {  // n <= 32
-    ensure(n);
-    return uint32_t(buf & ((1ull << n) - 1ull));
-  }
-  __device__ __forceinline__ void consume(uint32_t n) {
-    buf >>= n;
-    bits -= n;
-    total += n;
-  }
-  __device__ __forceinline__ uint32_t read(uint32_t n) {
-    uint32_t v = peek(n);
-    consume(n);
-    return v;
-  }
-};
-
-struct PassState {
-  DevBr br;
-  uint32_t ans_state;
-  uint32_t hist_idx;
-  // LZ77 (decode.rs:86-146): window of the symbols decoded so far (linear, see kLzWindow), pending copy
-  uint32_t* lz_win;
-  uint32_t lz_to_copy, lz_copy_pos, lz_decoded, lz_err;
-};
-
-// hybrid_uint.rs:87-102
-__device__ __forceinline__ uint32_t hybrid_uint(uint32_t cfg, uint32_t token, DevBr& br) {
-  uint32_t split_exponent = cfg & 0xff, msb = (cfg >> 8) & 0xff, lsb = (cfg >> 16) & 0xff;
-  uint32_t split_token = 1u << split_exponent;
-  if (token < split_token) return token;
-  uint32_t bits_in_token = lsb + msb;
-  uint32_t nbits = (split_exponent - bits_in_token + ((token - split_token) >> bits_in_token)) & 31;
-  uint32_t low = token & ((1u << lsb) - 1);
-  uint32_t token_nolow = token >> lsb;
-  uint32_t bits = br.read(nbits);
-  uint32_t hi = (token_nolow & ((1u << msb) - 1)) | (1u << msb);
-  return (((hi << nbits) | bits) << lsb) | low;
-}
-
-struct PassTables {
-  const uint8_t* context_map;
-  const uint32_t* uint_configs;
-  const uint2* ans;  // 8-byte buckets
-  const uint32_t* huff;
-  const uint32_t* huff_offset;
-  uint32_t use_prefix, log_alpha_size;
-  uint32_t lz_enabled, lz_min_symbol, lz_min_length, lz_len_cfg, lz_dist_cluster;
-};
-
-// ans.rs:356-393 / huffman.rs:446-457
-__device__ __forceinline__ uint32_t read_token(const PassTables& T, PassState& s, uint32_t cluster) {
-  if (T.use_prefix) {
-    const uint32_t* t = T.huff + __ldg(T.huff_offset + cluster);
-    uint32_t pos = s.br.peek(8);
-    uint32_t e = __ldg(t + pos);
-    uint32_t n_bits = e & 0xff;
-    if (n_bits > 8) {
-      s.br.consume(8);
-      n_bits -= 8;
-      pos += e >> 16;
-      pos += s.br.peek(n_bits);
-      e = __ldg(t + pos);
-    }
-    s.br.consume(e & 0xff);
-    return e >> 16;
-  }
-  const uint32_t log_bucket = 12 - T.log_alpha_size;
-  uint32_t idx = s.ans_state & 0xfff;
-  uint32_t i = idx >> log_bucket;
-  uint32_t pos = idx & ((1u << log_bucket) - 1);
-  uint2 b = __ldg(T.ans + ((size_t(cluster) << T.log_alpha_size) + i));
-  uint32_t alias_symbol = b.x & 0xff, alias_cutoff = (b.x >> 8) & 0xff, dist = b.x >> 16;
-  uint32_t alias_offset = b.y & 0xffff, alias_dist_xor = b.y >> 16;
-  bool alias = pos >= alias_cutoff;
-  uint32_t offset = (alias ? alias_offset : 0u) + pos;
-  dist ^= alias ? alias_dist_xor : 0u;
-  uint32_t symbol = alias ? alias_symbol : i;
-  uint32_t next = (s.ans_state >> 12) * dist + offset;
-  if (next < (1u << 16)) {
-    next = (next << 16) | s.br.peek(16);
-    s.br.consume(16);
-  }
-  s.ans_state = next;
-  return symbol;
-}
-
-// decode.rs:286-330 with dist_multiplier == 0 (HF streams create their reader without an image width, group.rs:345-349).
-__device__ __noinline__ uint32_t read_symbol_lz77(const PassTables& T, PassState& s, uint32_t ctx) {
-  auto push = [&](uint32_t sym) {
-    s.lz_win[min(s.lz_decoded, kLzWindow - 1)] = sym;
-    s.lz_decoded++;
-    return sym;
-  };
-  if (s.lz_to_copy) {  // pull_symbol
-    s.lz_to_copy--;
-    return push(s.lz_win[min(s.lz_copy_pos++, kLzWindow - 1)]);
-  }
-  const uint32_t cluster = __ldg(T.context_map + ctx);
-  const uint32_t tok = read_token(T, s, cluster);
-  if (tok < T.lz_min_symbol) return push(hybrid_uint(__ldg(T.uint_configs + cluster), tok, s.br));
-  if (s.lz_decoded == 0) {  // a copy before anything was decoded (errors.lz77_repeat)
-    s.lz_err = 1;
-    return 0;
-  }
-  const uint32_t n = hybrid_uint(T.lz_len_cfg, tok - T.lz_min_symbol, s.br);
-  if (n > 0xffffffffu - T.lz_min_length) {
-    s.lz_err = 1;
-    return 0;
-  }
-  const uint32_t dtok = read_token(T, s, T.lz_dist_cluster);
-  const uint32_t dsym = hybrid_uint(__ldg(T.uint_configs + T.lz_dist_cluster), dtok, s.br);
-  const uint32_t distance = min(min(dsym, (1u << 20) - 1u) + 1u, s.lz_decoded);  // apply_copy, decode.rs:111-124
-  s.lz_copy_pos = s.lz_decoded - distance;
-  s.lz_to_copy = n + T.lz_min_length - 1;  // the first copied symbol is returned right away
-  return push(s.lz_win[min(s.lz_copy_pos++, kLzWindow - 1)]);
-}
-
-__device__ __forceinline__ uint32_t read_symbol(const PassTables& T, PassState& s, uint32_t ctx) {
-  if (T.lz_enabled) return read_symbol_lz77(T, s, ctx);
-  uint32_t cluster = __ldg(T.context_map + ctx);
-  uint32_t tok = read_token(T, s, cluster);
-  return hybrid_uint(__ldg(T.uint_configs + cluster), tok, s.br);
-}
-
-__device__ __forceinline__ int32_t unpack_signed(uint32_t u) { return int32_t((u >> 1) ^ (((~u) & 1u) - 1u)); }
-
-// One coefficient list (device_types.h): base of the entries, offset words behind them.
-__device__ __forceinline__ uint32_t* list_base(const BatchDev& B, uint32_t section) { return B.nzlist + size_t(section) * kListStride; }
-// Writer side: the entry of coefficient value v at position pos of a varblock with 2^lnc coefficients per channel is
-// stored at the cursor whatever v is; the cursor only moves for v != 0 (branch-free; a zero is overwritten by the next
-// entry or stays behind the end of the channel). `ovf` collects values that do not fit the entry.
-__device__ __forceinline__ void list_put(uint32_t* base, uint32_t& n, uint32_t pos, int32_t v, uint32_t lnc, uint32_t& ovf) {
-  const int32_t sv = int32_t(uint32_t(v) << lnc);
-  ovf |= uint32_t((sv >> lnc) ^ v);
-  base[n] = pos | uint32_t(sv);
-  n += v != 0 ? 1u : 0u;
-}
-__device__ __forceinline__ uint32_t entry_pos(uint32_t e, uint32_t lnc) { return e & ((1u << lnc) - 1u); }
-__device__ __forceinline__ int32_t entry_value(uint32_t e, uint32_t lnc) { return int32_t(e) >> lnc; }
-
-// ---- bulk asynchronous copies (TMA engine, 1-D form) + mbarrier: global -> shared without passing through registers ----
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return uint32_t(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t arrivals) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(arrivals) : "memory");
-}
-__device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// One thread: announce `bytes` of asynchronous traffic on the barrier, then start the copy that will deliver them.
-// src, dst and bytes are multiples of 16.
-__device__ __forceinline__ void bulk_load(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst_smem)),
-               "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-                 : "=r"(done)
-                 : "r"(smem_u32(bar)), "r"(parity)
-                 : "memory");
-  } while (!done);
-}
-
-// Prefix of a stream's pass-0 coefficient list staged in shared memory by bulk copies (k_idct_small): the offset words
-// of all varblocks and the first `staged` entries; entries beyond that, and other passes, are read from global memory.
-struct ListStage {
-  const uint32_t* off;  // nullptr: nothing staged
-  const uint32_t* ent;
-  uint32_t staged;
-};
-
-struct BlockInfo {
-  uint32_t bx, by, cx, cy, shape, raw_quant, quant_lf, num_blocks, num_coeffs, log_num_blocks;
-};
-
-// One varblock, one pass: the three channels in Y, X, B order (group.rs:509-577).
-__device__ __forceinline__ int decode_block_pass(const BatchDev& B, const FrameDev& F, const PassDev& P,
-                                                 const PassTables& T, PassState& s, const BlockInfo& bi,
-                                                 uint8_t* nz_pass /* [3][1024] */, uint32_t* list, uint32_t& nlist, uint32_t bseq,
-                                                 uint32_t& ovf) {
-  const uint32_t num_ac_contexts = F.num_block_contexts * (37 + 458);
-  const uint32_t context_offset = s.hist_idx * num_ac_contexts;
-  const uint8_t* bcm = B.blob + F.block_ctx_map_off;
-#pragma unroll 1
-  for (int ci = 0; ci < 3; ci++) {
-    const int c = ci == 0 ? 1 : (ci == 1 ? 0 : 2);
-    uint8_t* nz = nz_pass + c * 1024;
-    uint32_t predicted;
-    if (bi.bx == 0) predicted = bi.by == 0 ? 32u : nz[(bi.by - 1) * 32];
-    else if (bi.by == 0) predicted = nz[bi.bx - 1];
-    else predicted = (uint32_t(nz[(bi.by - 1) * 32 + bi.bx]) + uint32_t(nz[bi.by * 32 + bi.bx - 1]) + 1u) >> 1;
-    uint32_t qf_idx = 0;
-    for (uint32_t i = 0; i < F.num_qf_thresholds; i++) qf_idx += bi.raw_quant > F.qf_thresholds[i];
-    uint32_t idx = c < 2 ? uint32_t(c ^ 1) : 2u;
-    idx = idx * 13 + bi.shape;
-    idx = idx * (F.num_qf_thresholds + 1) + qf_idx;
-    idx = idx * F.num_lf_contexts + bi.quant_lf;
-    uint32_t block_context = __ldg(bcm + idx);
-    uint32_t nzc = predicted < 8 ? predicted : (predicted < 64 ? 4 + predicted / 2 : 36);
-    uint32_t nonzeros = read_symbol(T, s, nzc * F.num_block_contexts + block_context + context_offset);
-    if (nonzeros + bi.num_blocks > bi.num_coeffs) return JXG_ERR_INVALID_NUM_NONZEROS;
-    uint8_t nzv = uint8_t((nonzeros + bi.num_blocks - 1) >> bi.log_num_blocks);
-    for (uint32_t iy = 0; iy < bi.cy; iy++)
-      for (uint32_t ix = 0; ix < bi.cx; ix++) nz[(bi.by + iy) * 32 + bi.bx + ix] = nzv;
-    const uint32_t histo_offset = F.num_block_contexts * 37 + 458 * block_context + context_offset;
-    uint32_t prev = nonzeros > bi.num_coeffs / 16 ? 0u : 1u;
-    const uint32_t* order = P.custom_orders
-                                ? reinterpret_cast<const uint32_t*>(B.blob + P.order_off) + P.order_offset[bi.shape * 3 + c]
-                                : B.natural_orders + B.natural_order_off[bi.shape];
-    list[kOffBase + bseq * 3 + ci] = nlist;  // first entry of channel ci (Y, X, B) of this varblock in this pass
-    const uint32_t lnb = bi.log_num_blocks, rnd = bi.num_blocks - 1;
-#pragma unroll 1
-    for (uint32_t k = bi.num_blocks; k < bi.num_coeffs && nonzeros != 0; k++) {
-      uint32_t ctx = histo_offset + (uint32_t(c_nz_ctx[((nonzeros + rnd) >> lnb) & 63]) + uint32_t(c_freq_ctx[(k >> lnb) & 63])) * 2 + prev;
-      uint32_t u = read_symbol(T, s, ctx);
-      int32_t coeff = int32_t(uint32_t(unpack_signed(u)) << P.shift);
-      prev = coeff != 0;
-      nonzeros -= prev;
-      list_put(list, nlist, __ldg(order + k), coeff, bi.log_num_blocks + 6, ovf);
-    }
-    if (nonzeros != 0) return JXG_ERR_RESIDUAL_NONZEROS;
-  }
-  return 0;
-}
-
-__device__ __forceinline__ PassTables make_tables(const BatchDev& B, const PassDev& P) {
-  PassTables T;
-  T.context_map = B.blob + P.context_map_off;
-  T.uint_configs = reinterpret_cast<const uint32_t*>(B.blob + P.uint_configs_off);
-  T.ans = reinterpret_cast<const uint2*>(B.blob + P.ans_off);
-  T.huff = reinterpret_cast<const uint32_t*>(B.blob + P.huff_off);
-  T.huff_offset = reinterpret_cast<const uint32_t*>(B.blob + P.huff_offset_off);
-  T.use_prefix = P.use_prefix;
-  T.log_alpha_size = P.log_alpha_size;
-  T.lz_enabled = P.lz77_enabled;
-  T.lz_min_symbol = P.lz77_min_symbol;
-  T.lz_min_length = P.lz77_min_length;
-  T.lz_len_cfg = P.lz77_length_uint;
-  T.lz_dist_cluster = P.lz_dist_cluster;
-  return T;
-}
-
-__device__ __forceinline__ int init_pass(const BatchDev& B, const FrameDev& F, uint32_t pass, uint32_t g, PassState& s) {
-  const SectionDev sec = B.sections[F.section_base + pass * F.num_groups + g];
-  s.br.init(B.blob + sec.off, sec.len);
-  uint32_t nb = 0;
-  while ((1u << nb) < F.num_histograms) nb++;
-  s.hist_idx = s.br.read(nb);  // group.rs:333-341
-  if (s.hist_idx >= F.num_histograms) return JXG_ERR_INVALID_HISTOGRAM_INDEX;
-  s.ans_state = 0x130000u;
-  if (!F.passes[pass].use_prefix) s.ans_state = s.br.read(32);  // ans.rs:431
-  s.lz_win = F.has_lz ? B.lzwin + size_t(F.lz_win_base + pass * F.num_groups + g) * kLzWindow : nullptr;
-  s.lz_to_copy = s.lz_copy_pos = s.lz_decoded = s.lz_err = 0;
-  return 0;
-}
-
-__device__ __forceinline__ int finish_pass(const BatchDev& B, const FrameDev& F, uint32_t pass, uint32_t g, const PassState& s) {
-  const SectionDev sec = B.sections[F.section_base + pass * F.num_groups + g];
-  if (s.lz_err) return JXG_ERR_LZ77;
-  if (s.br.total > sec.len * 8u) return JXG_ERR_OUT_OF_BOUNDS;                          // bit_reader.rs:109
-  if (!F.passes[pass].use_prefix && s.ans_state != 0x130000u) return JXG_ERR_ANS_CHECKSUM;  // ans.rs:441
-  return 0;
-}
-
-constexpr int kEntropyWarps = 4;
-
-__global__ void __launch_bounds__(kEntropyWarps * 32) k_entropy(const BatchDev B) {
-  const uint32_t slow_idx = blockIdx.x * kEntropyWarps + (threadIdx.x >> 5);
-  if (slow_idx >= B.num_slow || (threadIdx.x & 31) != 0) return;
-  const StreamDev sd = B.streams_slow[slow_idx];
-  const FrameDev& F = B.frames[sd.frame];
-  const uint32_t g = sd.group;
-  const uint32_t stream = F.first_stream + g;
-  const uint32_t gx = g % F.xg, gy = g / F.xg;
-  const uint32_t bx0 = gx * 32, by0 = gy * 32;
-  const uint32_t gw = min(32u, F.xb - bx0), gh = min(32u, F.yb - by0);
-  uint8_t* nz = B.nz + B.nz_base[stream];
-  const uint8_t* tmap = B.blob + F.transform_off;
-  const int32_t* rq = reinterpret_cast<const int32_t*>(B.blob + F.raw_quant_off);
-  const uint8_t* qlf = B.blob + F.quant_lf_off;
-  const uint32_t np = F.num_passes;
-  int err = 0;
-  uint32_t coeffs_offset = 0, bseq = 0;
-  // one coefficient list per pass (section = pass * num_groups + group); the transform kernels add the passes up
-  PassState st[kMaxPasses];
-  uint32_t nlist[kMaxPasses];
-  for (uint32_t p = 0; p < np; p++) nlist[p] = 0;
-  uint32_t ovf = 0;
-  for (uint32_t p = 0; p < np && !err; p++) err = init_pass(B, F, p, g, st[p]);
-  for (uint32_t by = 0; by < gh && !err; by++) {
-    for (uint32_t bx = 0; bx < gw && !err; bx++) {
-      const size_t bidx = size_t(by0 + by) * F.xb + bx0 + bx;
-      uint32_t raw_t = tmap[bidx];
-      if (raw_t < 128) continue;
-      uint32_t t = raw_t & 127;
-      if (t >= 27) { err = JXG_ERR_INVALID_TRANSFORM; break; }
-      BlockInfo bi;
-      bi.bx = bx; bi.by = by; bi.cx = c_cov_x[t]; bi.cy = c_cov_y[t]; bi.shape = c_shape[t];
-      bi.raw_quant = uint32_t(rq[bidx]); bi.quant_lf = qlf[bidx];
-      bi.num_blocks = bi.cx * bi.cy; bi.num_coeffs = bi.num_blocks * 64;
-      bi.log_num_blocks = 31 - __clz(bi.num_blocks);
-      if (coeffs_offset + bi.num_coeffs > kGroupCoeffs || bseq >= 1024) { err = JXG_ERR_INVALID_TRANSFORM; break; }  // overlapping varblocks
-      for (uint32_t p = 0; p < np && !err; p++) {
-        PassState s = st[p];
-        const PassTables T = make_tables(B, F.passes[p]);
-        const uint32_t section = F.section_base + p * F.num_groups + g;
-        uint32_t n = nlist[p];
-        err = decode_block_pass(B, F, F.passes[p], T, s, bi, nz + p * 3072, list_base(B, section), n, bseq, ovf);
-        nlist[p] = n;
-        st[p] = s;
-      }
-      coeffs_offset += bi.num_coeffs;
-      bseq++;
-    }
-  }
-  for (uint32_t p = 0; p < np && !err; p++) {
-    list_base(B, F.section_base + p * F.num_groups + g)[kOffBase + bseq * 3] = nlist[p];
-    err = finish_pass(B, F, p, g, st[p]);
-  }
-  if (!err && ovf) err = JXG_ERR_UNSUPPORTED;  // a coefficient beyond the entry width (device_types.h)
-  B.status[stream] = err;
-}
-
-// ---------------------------------------------------------------------------
-// K1 fast path (single-pass frames): S streams per warp, one lane per stream,
-// the decode loop written as a small state machine so that the lanes of a warp
-// stay converged on the common "decode one symbol" body. A stream's symbols are
-// strictly serial (one rANS state, contexts depend on the previous values), so
-// throughput comes from packing independent streams: S is chosen by the host so
-// that the grid is about one resident wave of warps.
-// ---------------------------------------------------------------------------
+// The symbol reader of k_entropy_fast and k_entropy: bit reader, token step (ANS alias bucket or two-level prefix table)
+// and hybrid uint, over the table formats of PassDev. k_entropy_lean reads the same formats with its own fused per-symbol
+// step: the speculative context look-ups and the register bit window are its measured form (DESIGN §3).
 struct LaneBr {  // 32-bit window bit reader (bit_reader.rs semantics: zeros past the end, checked at the end)
   const uint32_t* words;
   uint32_t nwords, bitpos, ci, lo, hi;
@@ -459,9 +106,302 @@ __device__ __forceinline__ uint32_t lane_hybrid(uint32_t cfg, uint32_t token, La
   return (((hi << nbits) | bits) << lsb) | low;
 }
 
+struct PassState {
+  LaneBr br;
+  uint32_t ans_state;
+  uint32_t hist_idx;
+  // LZ77 (decode.rs:86-146): window of the symbols decoded so far (linear, see kLzWindow), pending copy
+  uint32_t* lz_win;
+  uint32_t lz_to_copy, lz_copy_pos, lz_decoded, lz_err;
+};
+
+struct PassTables {
+  const uint8_t* context_map;
+  const uint32_t* uint_configs;
+  const uint2* ans;  // 8-byte buckets
+  const uint32_t* huff;
+  const uint32_t* huff_offset;
+  uint32_t use_prefix, log_alpha_size;
+  uint32_t lz_enabled, lz_min_symbol, lz_min_length, lz_len_cfg, lz_dist_cluster;
+};
+
+// ans.rs:356-393 / huffman.rs:446-457
+__device__ __forceinline__ uint32_t lane_token(const PassTables& T, PassState& s, uint32_t cluster) {
+  LaneBr& br = s.br;
+  if (T.use_prefix) {
+    const uint32_t* tb = T.huff + __ldg(T.huff_offset + cluster);
+    uint32_t p = br.peek(8);
+    uint32_t e = __ldg(tb + p);
+    uint32_t n_bits = e & 0xff;
+    if (n_bits > 8) {
+      br.skip(8);
+      n_bits -= 8;
+      p += e >> 16;
+      p += br.peek(n_bits);
+      e = __ldg(tb + p);
+    }
+    br.skip(e & 0xff);
+    return e >> 16;
+  }
+  const uint32_t log_bucket = 12 - T.log_alpha_size;
+  const uint32_t idx = s.ans_state & 0xfff;
+  const uint32_t i = idx >> log_bucket, p = idx & ((1u << log_bucket) - 1u);
+  const uint2 b = __ldg(T.ans + ((cluster << T.log_alpha_size) + i));
+  const bool alias = p >= ((b.x >> 8) & 0xff);
+  const uint32_t dist = (b.x >> 16) ^ (alias ? (b.y >> 16) : 0u);
+  const uint32_t offset = p + (alias ? (b.y & 0xffff) : 0u);
+  uint32_t next = (s.ans_state >> 12) * dist + offset;
+  if (next < (1u << 16)) {
+    next = (next << 16) | br.peek(16);
+    br.skip(16);
+  }
+  s.ans_state = next;
+  return alias ? (b.x & 0xff) : i;
+}
+
+// One symbol of a stream without LZ77.
+__device__ __forceinline__ uint32_t lane_symbol(const PassTables& T, PassState& s, uint32_t ctx) {
+  const uint32_t cluster = __ldg(T.context_map + ctx);
+  const uint32_t tok = lane_token(T, s, cluster);
+  return lane_hybrid(__ldg(T.uint_configs + cluster), tok, s.br);
+}
+
+// decode.rs:286-330 with dist_multiplier == 0 (HF streams create their reader without an image width, group.rs:345-349).
+// Inlined: behind a call the stream state would live in local memory on k_entropy's per-symbol path.
+__device__ __forceinline__ uint32_t read_symbol_lz77(const PassTables& T, PassState& s, uint32_t ctx) {
+  auto push = [&](uint32_t sym) {
+    s.lz_win[min(s.lz_decoded, kLzWindow - 1)] = sym;
+    s.lz_decoded++;
+    return sym;
+  };
+  if (s.lz_to_copy) {  // pull_symbol
+    s.lz_to_copy--;
+    return push(s.lz_win[min(s.lz_copy_pos++, kLzWindow - 1)]);
+  }
+  const uint32_t cluster = __ldg(T.context_map + ctx);
+  const uint32_t tok = lane_token(T, s, cluster);
+  if (tok < T.lz_min_symbol) return push(lane_hybrid(__ldg(T.uint_configs + cluster), tok, s.br));
+  if (s.lz_decoded == 0) {  // a copy before anything was decoded (errors.lz77_repeat)
+    s.lz_err = 1;
+    return 0;
+  }
+  const uint32_t n = lane_hybrid(T.lz_len_cfg, tok - T.lz_min_symbol, s.br);
+  if (n > 0xffffffffu - T.lz_min_length) {
+    s.lz_err = 1;
+    return 0;
+  }
+  const uint32_t dtok = lane_token(T, s, T.lz_dist_cluster);
+  const uint32_t dsym = lane_hybrid(__ldg(T.uint_configs + T.lz_dist_cluster), dtok, s.br);
+  const uint32_t distance = min(min(dsym, (1u << 20) - 1u) + 1u, s.lz_decoded);  // apply_copy, decode.rs:111-124
+  s.lz_copy_pos = s.lz_decoded - distance;
+  s.lz_to_copy = n + T.lz_min_length - 1;  // the first copied symbol is returned right away
+  return push(s.lz_win[min(s.lz_copy_pos++, kLzWindow - 1)]);
+}
+
+__device__ __forceinline__ uint32_t read_symbol(const PassTables& T, PassState& s, uint32_t ctx) {
+  return T.lz_enabled ? read_symbol_lz77(T, s, ctx) : lane_symbol(T, s, ctx);
+}
+
+__device__ __forceinline__ int32_t unpack_signed(uint32_t u) { return int32_t((u >> 1) ^ (((~u) & 1u) - 1u)); }
+
+// One coefficient list (device_types.h): base of the entries, offset words behind them.
+__device__ __forceinline__ uint32_t* list_base(const BatchDev& B, uint32_t section) { return B.nzlist + size_t(section) * kListStride; }
+// Writer side: the entry of coefficient value v at position pos of a varblock with 2^lnc coefficients per channel is
+// stored at the cursor whatever v is; the cursor only moves for v != 0 (branch-free; a zero is overwritten by the next
+// entry or stays behind the end of the channel). `ovf` collects values that do not fit the entry.
+__device__ __forceinline__ void list_put(uint32_t* base, uint32_t& n, uint32_t pos, int32_t v, uint32_t lnc, uint32_t& ovf) {
+  const int32_t sv = int32_t(uint32_t(v) << lnc);
+  ovf |= uint32_t((sv >> lnc) ^ v);
+  base[n] = pos | uint32_t(sv);
+  n += v != 0 ? 1u : 0u;
+}
+__device__ __forceinline__ uint32_t entry_pos(uint32_t e, uint32_t lnc) { return e & ((1u << lnc) - 1u); }
+__device__ __forceinline__ int32_t entry_value(uint32_t e, uint32_t lnc) { return int32_t(e) >> lnc; }
+
+// ---- bulk asynchronous copies (TMA engine, 1-D form) + mbarrier: global -> shared without passing through registers ----
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return uint32_t(__cvta_generic_to_shared(p)); }
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t arrivals) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(arrivals) : "memory");
+}
+__device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// One thread: announce `bytes` of asynchronous traffic on the barrier, then start the copy that will deliver them.
+// src, dst and bytes are multiples of 16.
+__device__ __forceinline__ void bulk_load(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst_smem)),
+               "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t done;
+  do {
+    asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
+                 : "=r"(done)
+                 : "r"(smem_u32(bar)), "r"(parity)
+                 : "memory");
+  } while (!done);
+}
+
+// Prefix of a stream's pass-0 coefficient list staged in shared memory by bulk copies (k_idct_small): the offset words
+// of all varblocks and the first `staged` entries; entries beyond that, and other passes, are read from global memory.
+struct ListStage {
+  const uint32_t* off;  // nullptr: nothing staged
+  const uint32_t* ent;
+  uint32_t staged;
+};
+
+// Non-zero count predicted for a channel's varblock at (bx, by) from the column bytes of the channel (group.rs:489-505).
+// Varblocks are visited in raster order of their top-left corner (the block plan's order), so the last count written to
+// a column is the one of the block right above the current row, and for column bx - 1 the one of the block to the left.
+__device__ __forceinline__ uint32_t predict_nz(const uint8_t* col, uint32_t bx, uint32_t by) {
+  if (bx == 0) return by == 0 ? 32u : col[0];
+  if (by == 0) return col[bx - 1];
+  return (uint32_t(col[bx]) + uint32_t(col[bx - 1]) + 1u) >> 1;
+}
+
+// One varblock (descriptor d of k_block_plan), one pass: the three channels in Y, X, B order (group.rs:509-577).
+__device__ __forceinline__ int decode_block_pass(const BatchDev& B, const FrameDev& F, const PassDev& P,
+                                                 const PassTables& T, PassState& s, const uint4 d,
+                                                 uint8_t* nzcol /* [3][32] */, uint32_t* list, uint32_t& nlist, uint32_t bi,
+                                                 uint32_t& ovf) {
+  const uint32_t context_offset = s.hist_idx * F.num_block_contexts * (37 + 458);
+  const uint32_t bx = d.x & 31, by = (d.x >> 5) & 31, cx = (d.x >> 10) & 63, shape = (d.x >> 22) & 15, lnb = d.x >> 26;
+  const uint32_t num_blocks = 1u << lnb, num_coeffs = num_blocks * 64;
+#pragma unroll 1
+  for (int ci = 0; ci < 3; ci++) {
+    const int c = ci == 0 ? 1 : (ci == 1 ? 0 : 2);
+    uint8_t* col = nzcol + c * 32;
+    const uint32_t predicted = predict_nz(col, bx, by);
+    const uint32_t block_context = (d.y >> (8 * ci)) & 0xff;
+    uint32_t nzc = predicted < 8 ? predicted : (predicted < 64 ? 4 + predicted / 2 : 36);
+    uint32_t nonzeros = read_symbol(T, s, nzc * F.num_block_contexts + block_context + context_offset);
+    if (nonzeros + num_blocks > num_coeffs) return JXG_ERR_INVALID_NUM_NONZEROS;
+    const uint8_t nzv = uint8_t((nonzeros + num_blocks - 1) >> lnb);
+    for (uint32_t ix = 0; ix < cx; ix++) col[bx + ix] = nzv;
+    const uint32_t histo_offset = F.num_block_contexts * 37 + 458 * block_context + context_offset;
+    uint32_t prev = nonzeros > num_coeffs / 16 ? 0u : 1u;
+    const uint32_t* order = P.custom_orders
+                                ? reinterpret_cast<const uint32_t*>(B.blob + P.order_off) + P.order_offset[shape * 3 + c]
+                                : B.natural_orders + B.natural_order_off[shape];
+    list[kOffBase + bi * 3 + ci] = nlist;  // first entry of channel ci (Y, X, B) of this varblock in this pass
+    const uint32_t rnd = num_blocks - 1;
+#pragma unroll 1
+    for (uint32_t k = num_blocks; k < num_coeffs && nonzeros != 0; k++) {
+      uint32_t ctx = histo_offset + (uint32_t(c_nz_ctx[((nonzeros + rnd) >> lnb) & 63]) + uint32_t(c_freq_ctx[(k >> lnb) & 63])) * 2 + prev;
+      uint32_t u = read_symbol(T, s, ctx);
+      int32_t coeff = int32_t(uint32_t(unpack_signed(u)) << P.shift);
+      prev = coeff != 0;
+      nonzeros -= prev;
+      list_put(list, nlist, __ldg(order + k), coeff, lnb + 6, ovf);
+    }
+    if (nonzeros != 0) return JXG_ERR_RESIDUAL_NONZEROS;
+  }
+  return 0;
+}
+
+__device__ __forceinline__ PassTables make_tables(const BatchDev& B, const PassDev& P) {
+  PassTables T;
+  T.context_map = B.blob + P.context_map_off;
+  T.uint_configs = reinterpret_cast<const uint32_t*>(B.blob + P.uint_configs_off);
+  T.ans = reinterpret_cast<const uint2*>(B.blob + P.ans_off);
+  T.huff = reinterpret_cast<const uint32_t*>(B.blob + P.huff_off);
+  T.huff_offset = reinterpret_cast<const uint32_t*>(B.blob + P.huff_offset_off);
+  T.use_prefix = P.use_prefix;
+  T.log_alpha_size = P.log_alpha_size;
+  T.lz_enabled = P.lz77_enabled;
+  T.lz_min_symbol = P.lz77_min_symbol;
+  T.lz_min_length = P.lz77_min_length;
+  T.lz_len_cfg = P.lz77_length_uint;
+  T.lz_dist_cluster = P.lz_dist_cluster;
+  return T;
+}
+
+__device__ __forceinline__ int init_pass(const BatchDev& B, const FrameDev& F, uint32_t pass, uint32_t g, PassState& s) {
+  const SectionDev sec = B.sections[F.section_base + pass * F.num_groups + g];
+  s.br.init(B.blob + sec.off, sec.len);
+  uint32_t nb = 0;
+  while ((1u << nb) < F.num_histograms) nb++;
+  s.hist_idx = s.br.peek(nb);  // group.rs:333-341
+  s.br.skip(nb);
+  if (s.hist_idx >= F.num_histograms) return JXG_ERR_INVALID_HISTOGRAM_INDEX;
+  s.ans_state = 0x130000u;
+  if (!F.passes[pass].use_prefix) {  // ans.rs:431
+    s.ans_state = s.br.peek32();
+    s.br.skip(32);
+  }
+  s.lz_win = F.has_lz ? B.lzwin + size_t(F.lz_win_base + pass * F.num_groups + g) * kLzWindow : nullptr;
+  s.lz_to_copy = s.lz_copy_pos = s.lz_decoded = s.lz_err = 0;
+  return 0;
+}
+
+// check_final_state (decode.rs:400)
+__device__ __forceinline__ int finish_pass(const BatchDev& B, const FrameDev& F, uint32_t pass, uint32_t g, const PassState& s) {
+  const SectionDev sec = B.sections[F.section_base + pass * F.num_groups + g];
+  if (s.lz_err) return JXG_ERR_LZ77;
+  if (s.br.bitpos > sec.len * 8u) return JXG_ERR_OUT_OF_BOUNDS;                         // bit_reader.rs:109
+  if (!F.passes[pass].use_prefix && s.ans_state != 0x130000u) return JXG_ERR_ANS_CHECKSUM;  // ans.rs:441
+  return 0;
+}
+
+constexpr int kEntropyWarps = 4;
+
+// K1 slow path (multi-pass and LZ77 frames): one lane per warp and stream, the varblocks of the block plan in order,
+// each through all passes.
+__global__ void __launch_bounds__(kEntropyWarps * 32) k_entropy(const BatchDev B) {
+  // non-zero counts by column (see predict_nz), one set per pass: group.rs keeps one count per pass
+  __shared__ uint8_t s_nzcol[kEntropyWarps][kMaxPasses][3 * 32];
+  const uint32_t warp = threadIdx.x >> 5;
+  const uint32_t slow_idx = blockIdx.x * kEntropyWarps + warp;
+  if (slow_idx >= B.num_slow || (threadIdx.x & 31) != 0) return;
+  const StreamDev sd = B.streams_slow[slow_idx];
+  const FrameDev& F = B.frames[sd.frame];
+  const uint32_t g = sd.group;
+  const uint32_t stream = F.first_stream + g;
+  const uint32_t nblk = B.nblk[stream];
+  if (nblk == 0xffffffffu) {  // the block plan failed: invalid or overlapping varblocks
+    B.status[stream] = JXG_ERR_INVALID_TRANSFORM;
+    return;
+  }
+  const uint4* desc = B.desc + size_t(stream) * 1024;
+  const uint32_t np = F.num_passes;
+  int err = 0;
+  // one coefficient list per pass (section = pass * num_groups + group); the transform kernels add the passes up
+  PassState st[kMaxPasses];
+  uint32_t nlist[kMaxPasses];
+  for (uint32_t p = 0; p < np; p++) nlist[p] = 0;
+  uint32_t ovf = 0;
+  for (uint32_t p = 0; p < np && !err; p++) err = init_pass(B, F, p, g, st[p]);
+  for (uint32_t bi = 0; bi < nblk && !err; bi++) {
+    const uint4 d = __ldg(desc + bi);
+    for (uint32_t p = 0; p < np && !err; p++) {
+      PassState s = st[p];
+      const PassTables T = make_tables(B, F.passes[p]);
+      const uint32_t section = F.section_base + p * F.num_groups + g;
+      uint32_t n = nlist[p];
+      err = decode_block_pass(B, F, F.passes[p], T, s, d, s_nzcol[warp][p], list_base(B, section), n, bi, ovf);
+      nlist[p] = n;
+      st[p] = s;
+    }
+  }
+  for (uint32_t p = 0; p < np && !err; p++) {
+    list_base(B, F.section_base + p * F.num_groups + g)[kOffBase + nblk * 3] = nlist[p];
+    err = finish_pass(B, F, p, g, st[p]);
+  }
+  if (!err && ovf) err = JXG_ERR_UNSUPPORTED;  // a coefficient beyond the entry width (device_types.h)
+  B.status[stream] = err;
+}
+
+// ---------------------------------------------------------------------------
+// K1 fast path (single-pass frames that are prefix coded or shifted): S streams per warp, one lane per stream,
+// the decode loop written as a small state machine so that the lanes of a warp stay converged on the common
+// "decode one symbol" body. A stream's symbols are strictly serial (one rANS state, contexts depend on the previous
+// values), so throughput comes from packing independent streams: S is chosen by the host so that the grid is about
+// one resident wave of warps.
+// ---------------------------------------------------------------------------
 template <int S>
 __global__ void __launch_bounds__(128, 8) k_entropy_fast(const BatchDev B) {
   __shared__ uint16_t s_nz_ctx[64], s_freq_ctx[64];
+  __shared__ uint8_t s_nzcol[4 * S][3 * 32];  // per lane: non-zero counts by column (see predict_nz)
   if (threadIdx.x < 64) {
     s_nz_ctx[threadIdx.x] = c_nz_ctx[threadIdx.x];
     s_freq_ctx[threadIdx.x] = c_freq_ctx[threadIdx.x];
@@ -475,157 +415,70 @@ __global__ void __launch_bounds__(128, 8) k_entropy_fast(const BatchDev B) {
   const FrameDev& F = B.frames[sd.frame];
   const uint32_t g = sd.group;
   const uint32_t gsid = F.first_stream + g;
-  const uint32_t bx0 = (g % F.xg) * 32, by0 = (g / F.xg) * 32;
-  const uint32_t gw = min(32u, F.xb - bx0), gh = min(32u, F.yb - by0), gn = gw * gh;
-  const uint32_t lsec = F.section_base + g;  // single pass: list of section `group`
-  uint32_t* const list = list_base(B, lsec);
-  uint32_t nlist = 0, bseq = 0, ovf = 0;
-  uint8_t* const nz = B.nz + B.nz_base[gsid];
-  const uint8_t* const tmap = B.blob + F.transform_off;
-  const int32_t* const rq = reinterpret_cast<const int32_t*>(B.blob + F.raw_quant_off);
-  const uint8_t* const qlf = B.blob + F.quant_lf_off;
-  const uint8_t* const bcm = B.blob + F.block_ctx_map_off;
+  uint32_t* const list = list_base(B, F.section_base + g);  // single pass: list of section `group`
+  uint32_t nlist = 0, ovf = 0;
+  uint8_t* const nz = s_nzcol[(threadIdx.x >> 5) * S + (lane < S ? lane : 0)];
+  const uint4* const desc = B.desc + size_t(gsid) * 1024;
+  const uint32_t nblk = done ? 0u : B.nblk[gsid];
   const PassDev& P = F.passes[0];
-  const uint8_t* const ctxmap = B.blob + P.context_map_off;
-  const uint32_t* const ucfg = reinterpret_cast<const uint32_t*>(B.blob + P.uint_configs_off);
-  const uint2* const ans = reinterpret_cast<const uint2*>(B.blob + P.ans_off);
-  const uint32_t* const huff = reinterpret_cast<const uint32_t*>(B.blob + P.huff_off);
-  const uint32_t* const huff_offset = reinterpret_cast<const uint32_t*>(B.blob + P.huff_offset_off);
-  const bool use_prefix = P.use_prefix != 0;
-  const uint32_t log_alpha = P.log_alpha_size, log_bucket = 12 - P.log_alpha_size, bucket_mask = (1u << (12 - P.log_alpha_size)) - 1;
+  const PassTables T = make_tables(B, P);
   const uint32_t shift = P.shift;
   const uint32_t nbc = F.num_block_contexts;
-  const uint32_t num_ac_contexts = nbc * (37 + 458);
-  int err = 0;
-  LaneBr br;
-  uint32_t ans_state = 0x130000u, context_offset = 0;
+  PassState s;
+  uint32_t context_offset = 0;
   if (!done) {
-    const SectionDev sec = B.sections[F.section_base + g];
-    br.init(B.blob + sec.off, sec.len);
-    uint32_t nb = 0;
-    while ((1u << nb) < F.num_histograms) nb++;
-    const uint32_t hist_idx = br.peek(nb);  // group.rs:333-341
-    br.skip(nb);
-    if (hist_idx >= F.num_histograms) {
-      err = JXG_ERR_INVALID_HISTOGRAM_INDEX;
-      done = true;
+    // nblk == 0xffffffff: the block plan failed (invalid or overlapping varblocks)
+    const int err = nblk == 0xffffffffu ? JXG_ERR_INVALID_TRANSFORM : init_pass(B, F, 0, g, s);
+    if (err) {
       B.status[gsid] = err;
+      done = true;
+    } else {
+      context_offset = s.hist_idx * nbc * (37 + 458);
     }
-    context_offset = hist_idx * num_ac_contexts;
-    if (!use_prefix) {
-      ans_state = br.peek32();
-      br.skip(32);
-    }
-  } else {
-    br.words = nullptr;
-    br.nwords = br.bitpos = br.ci = br.lo = br.hi = 0;
   }
-  enum { PH_SCAN = 0, PH_NNZ = 1, PH_COEF = 2 };
-  uint32_t phase = PH_SCAN, pos = 0, coeffs_offset = 0;
+  enum { PH_BLOCK = 0, PH_NNZ = 1, PH_COEF = 2 };
+  uint32_t phase = PH_BLOCK, bi = 0;
   // current block / channel
-  uint32_t bx = 0, by = 0, cx = 1, cy = 1, shape = 0, qf_idx = 0, quant_lf = 0, num_blocks = 1, num_coeffs = 64, lnb = 0;
-  uint32_t ci = 0, k = 0, nonzeros = 0, prev = 0, histo_offset = 0;
+  uint32_t bx = 0, by = 0, cx = 1, shape = 0, bctx3 = 0, num_blocks = 1, num_coeffs = 64, lnb = 0;
+  uint32_t ci = 0, k = 0, nonzeros = 0, prev = 0, histo_offset = 0, block_context = 0;
   const uint32_t* order = B.natural_orders;
 
   for (;;) {
     if (!__any_sync(0xffffffffu, !done)) break;
-    if (!done && phase == PH_SCAN) {
-      uint32_t raw_t = 0;
-      while (pos < gn) {
-        bx = pos % gw;
-        by = pos / gw;
-        raw_t = tmap[size_t(by0 + by) * F.xb + bx0 + bx];
-        if (raw_t >= 128) break;
-        pos++;
-      }
-      if (pos >= gn) {  // stream finished: check_final_state (decode.rs:400)
-        const SectionDev sec = B.sections[F.section_base + g];
-        if (br.bitpos > sec.len * 8u) err = JXG_ERR_OUT_OF_BOUNDS;
-        else if (!use_prefix && ans_state != 0x130000u) err = JXG_ERR_ANS_CHECKSUM;
-        else if (ovf) err = JXG_ERR_UNSUPPORTED;  // a coefficient beyond the entry width (device_types.h)
+    if (!done && phase == PH_BLOCK) {
+      if (bi == nblk) {  // stream finished
+        int err = finish_pass(B, F, 0, g, s);
+        if (!err && ovf) err = JXG_ERR_UNSUPPORTED;  // a coefficient beyond the entry width (device_types.h)
         B.status[gsid] = err;
-        list[kOffBase + bseq * 3] = nlist;
+        list[kOffBase + nblk * 3] = nlist;
         done = true;
       } else {
-        const uint32_t t = raw_t & 127;
-        if (t >= 27) {
-          B.status[gsid] = JXG_ERR_INVALID_TRANSFORM;
-          done = true;
-        } else {
-          const size_t bidx = size_t(by0 + by) * F.xb + bx0 + bx;
-          cx = c_cov_x[t];
-          cy = c_cov_y[t];
-          shape = c_shape[t];
-          const uint32_t raw_quant = uint32_t(rq[bidx]);
-          quant_lf = qlf[bidx];
-          qf_idx = 0;
-          for (uint32_t i = 0; i < F.num_qf_thresholds; i++) qf_idx += raw_quant > F.qf_thresholds[i];
-          num_blocks = cx * cy;
-          num_coeffs = num_blocks * 64;
-          lnb = 31 - __clz(num_blocks);
-          if (coeffs_offset + num_coeffs > kGroupCoeffs || bseq >= 1024) {  // overlapping varblocks: the group's coefficient area would overflow
-            B.status[gsid] = JXG_ERR_INVALID_TRANSFORM;
-            done = true;
-          } else {
-            ci = 0;
-            phase = PH_NNZ;
-          }
-        }
+        const uint4 d = __ldg(desc + bi);
+        bx = d.x & 31;
+        by = (d.x >> 5) & 31;
+        cx = (d.x >> 10) & 63;
+        shape = (d.x >> 22) & 15;
+        lnb = d.x >> 26;
+        num_blocks = 1u << lnb;
+        num_coeffs = num_blocks * 64;
+        bctx3 = d.y;
+        ci = 0;
+        phase = PH_NNZ;
       }
     }
     if (done) continue;
     // ---- one symbol ----
-    uint32_t ctx, block_context = 0;
+    uint32_t ctx;
     const int c = ci == 0 ? 1 : (ci == 1 ? 0 : 2);  // Y, X, B
     if (phase == PH_NNZ) {
-      const uint8_t* nzc_map = nz + c * 1024;
-      uint32_t predicted;
-      if (bx == 0) predicted = by == 0 ? 32u : nzc_map[(by - 1) * 32];
-      else if (by == 0) predicted = nzc_map[bx - 1];
-      else predicted = (uint32_t(nzc_map[(by - 1) * 32 + bx]) + uint32_t(nzc_map[by * 32 + bx - 1]) + 1u) >> 1;
-      uint32_t idx = c < 2 ? uint32_t(c ^ 1) : 2u;
-      idx = idx * 13 + shape;
-      idx = idx * (F.num_qf_thresholds + 1) + qf_idx;
-      idx = idx * F.num_lf_contexts + quant_lf;
-      block_context = __ldg(bcm + idx);
+      const uint32_t predicted = predict_nz(nz + c * 32, bx, by);
+      block_context = (bctx3 >> (8 * ci)) & 0xff;
       const uint32_t nzc = predicted < 8 ? predicted : (predicted < 64 ? 4 + predicted / 2 : 36);
       ctx = nzc * nbc + block_context + context_offset;
     } else {
       ctx = histo_offset + (uint32_t(s_nz_ctx[((nonzeros + num_blocks - 1) >> lnb) & 63]) + uint32_t(s_freq_ctx[(k >> lnb) & 63])) * 2 + prev;
     }
-    const uint32_t cluster = __ldg(ctxmap + ctx);
-    uint32_t token;
-    if (use_prefix) {  // huffman.rs:446-457
-      const uint32_t* tb = huff + __ldg(huff_offset + cluster);
-      uint32_t p = br.peek(8);
-      uint32_t e = __ldg(tb + p);
-      uint32_t n_bits = e & 0xff;
-      if (n_bits > 8) {
-        br.skip(8);
-        n_bits -= 8;
-        p += e >> 16;
-        p += br.peek(n_bits);
-        e = __ldg(tb + p);
-      }
-      br.skip(e & 0xff);
-      token = e >> 16;
-    } else {  // ans.rs:356-393
-      const uint32_t idx = ans_state & 0xfff;
-      const uint32_t i = idx >> log_bucket, p = idx & bucket_mask;
-      const uint2 b = __ldg(ans + ((cluster << log_alpha) + i));
-      const uint32_t alias_cutoff = (b.x >> 8) & 0xff;
-      const bool alias = p >= alias_cutoff;
-      const uint32_t dist = (b.x >> 16) ^ (alias ? (b.y >> 16) : 0u);
-      const uint32_t offset = p + (alias ? (b.y & 0xffff) : 0u);
-      token = alias ? (b.x & 0xff) : i;
-      uint32_t next = (ans_state >> 12) * dist + offset;
-      if (next < (1u << 16)) {
-        next = (next << 16) | br.peek(16);
-        br.skip(16);
-      }
-      ans_state = next;
-    }
-    const uint32_t value = lane_hybrid(__ldg(ucfg + cluster), token, br);
+    const uint32_t value = lane_symbol(T, s, ctx);
     bool next_channel = false;
     if (phase == PH_NNZ) {
       nonzeros = value;
@@ -634,16 +487,15 @@ __global__ void __launch_bounds__(128, 8) k_entropy_fast(const BatchDev B) {
         done = true;
         continue;
       }
-      uint8_t* nzc_map = nz + c * 1024;
+      uint8_t* col = nz + c * 32;
       const uint8_t nzv = uint8_t((nonzeros + num_blocks - 1) >> lnb);
-      for (uint32_t iy = 0; iy < cy; iy++)
-        for (uint32_t ix = 0; ix < cx; ix++) nzc_map[(by + iy) * 32 + bx + ix] = nzv;
+      for (uint32_t ix = 0; ix < cx; ix++) col[bx + ix] = nzv;
       histo_offset = nbc * 37 + 458 * block_context + context_offset;
       prev = nonzeros > num_coeffs / 16 ? 0u : 1u;
       k = num_blocks;
       order = P.custom_orders ? reinterpret_cast<const uint32_t*>(B.blob + P.order_off) + P.order_offset[shape * 3 + c]
                               : B.natural_orders + B.natural_order_off[shape];
-      list[kOffBase + bseq * 3 + ci] = nlist;
+      list[kOffBase + bi * 3 + ci] = nlist;
       if (nonzeros == 0) next_channel = true;
       else phase = PH_COEF;
     } else {
@@ -667,10 +519,8 @@ __global__ void __launch_bounds__(128, 8) k_entropy_fast(const BatchDev B) {
       ci++;
       phase = PH_NNZ;
       if (ci == 3) {
-        coeffs_offset += num_coeffs;
-        bseq++;
-        pos++;
-        phase = PH_SCAN;
+        bi++;
+        phase = PH_BLOCK;
       }
     }
   }
@@ -691,7 +541,7 @@ __global__ void __launch_bounds__(128, 8) k_entropy_fast(const BatchDev B) {
 // corrupt stream cannot walk out of the blob (the over-read is reported from bitpos at the end).
 // ---------------------------------------------------------------------------
 // ---------------------------------------------------------------------------
-// K0: block plan of the lean entropy path. One warp per (frame, group) stream walks the group's 32x32 transform map
+// K0: block plan of the entropy kernels. One warp per (frame, group) stream walks the group's 32x32 transform map
 // in raster order and writes, for every varblock, a 16-byte descriptor
 //   x: bx | by << 5 | cx << 10 | cy << 16 | shape << 22 | log2(cx * cy) << 26
 //   y: block contexts of Y, X, B (block_context_map.rs:128-150), one byte each
