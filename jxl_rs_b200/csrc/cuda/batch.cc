@@ -398,24 +398,25 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   for (uint32_t p = 0; p < d->num_passes; p++) {
     const JxgPassDesc& s = d->passes[p];
     PassDev& P = F.passes[p];
+    CodeDev& c = P.code;
     if (s.lz77_enabled) F.has_lz = 1;  // routed to the one-lane-per-warp kernel, which carries the LZ77 window
-    P.lz77_enabled = s.lz77_enabled;
-    P.lz77_min_symbol = s.lz77_min_symbol;
-    P.lz77_min_length = s.lz77_min_length;
-    P.lz77_length_uint = s.lz77_length_uint;
-    P.lz_dist_cluster = s.lz_dist_cluster;
+    c.lz_enabled = s.lz77_enabled;
+    c.lz_min_symbol = s.lz77_min_symbol;
+    c.lz_min_length = s.lz77_min_length;
+    c.lz_len_cfg = s.lz77_length_uint;
+    c.lz_dist_cluster = s.lz_dist_cluster;
+    c.use_prefix = s.use_prefix;
+    c.log_alpha = s.log_alpha_size;
+    c.num_clusters = s.num_clusters;
     P.shift = s.shift;
-    P.use_prefix = s.use_prefix;
-    P.log_alpha_size = s.log_alpha_size;
-    P.num_clusters = s.num_clusters;
     P.custom_orders = s.coeff_order != nullptr;
-    APPEND(P.context_map_off, s.context_map, s.num_contexts, 16);
-    APPEND(P.uint_configs_off, s.uint_configs, size_t(s.num_clusters) * 4, 16);
+    APPEND(c.cmap_off, s.context_map, s.num_contexts, 16);
+    APPEND(c.cfg_off, s.uint_configs, size_t(s.num_clusters) * 4, 16);
     if (s.use_prefix) {
-      APPEND(P.huff_off, s.huff_entries, size_t(s.huff_entries_len) * 4, 16);
-      APPEND(P.huff_offset_off, s.huff_offset, size_t(s.num_clusters) * 4, 16);
+      APPEND(c.huff_off, s.huff_entries, size_t(s.huff_entries_len) * 4, 16);
+      APPEND(c.huff_offset_off, s.huff_offset, size_t(s.num_clusters) * 4, 16);
     } else {
-      APPEND(P.ans_off, s.ans_buckets, (size_t(s.num_clusters) << s.log_alpha_size) * 8, 16);
+      APPEND(c.ans_off, s.ans_buckets, (size_t(s.num_clusters) << s.log_alpha_size) * 8, 16);
     }
     if (P.custom_orders) {
       APPEND(P.order_off, s.coeff_order, size_t(s.coeff_order_len) * 4, 16);
@@ -464,16 +465,16 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
     F.lz_win_base = b->lz_windows;
     b->lz_windows += F.num_passes * F.num_groups;
   }
-  if (F.num_passes == 1 && !F.has_lz && !F.passes[0].use_prefix && F.passes[0].shift == 0 &&
+  if (F.num_passes == 1 && !F.has_lz && !F.passes[0].code.use_prefix && F.passes[0].shift == 0 &&
       size_t(F.num_histograms) * F.num_block_contexts * 495 + 64 > 16384)
     b->lean_ctx_smem = false;
-  if (F.num_passes == 1 && !F.has_lz && !F.passes[0].use_prefix)
+  if (F.num_passes == 1 && !F.has_lz && !F.passes[0].code.use_prefix)
     for (uint32_t c = 0; c < d->passes[0].num_clusters; c++)
       if (d->passes[0].uint_configs[c] != (4u | (2u << 8))) b->lean_all_420 = false;
   F.first_stream = uint32_t(b->streams.size());
   for (uint32_t g = 0; g < F.num_groups; g++) {
     b->streams.push_back(StreamDev{uint32_t(b->frames.size()), g});
-    ((F.num_passes != 1 || F.has_lz) ? b->streams_slow : ((F.passes[0].use_prefix || F.passes[0].shift != 0) ? b->streams_fast : b->streams_lean)).push_back(StreamDev{uint32_t(b->frames.size()), g});
+    ((F.num_passes != 1 || F.has_lz) ? b->streams_slow : ((F.passes[0].code.use_prefix || F.passes[0].shift != 0) ? b->streams_fast : b->streams_lean)).push_back(StreamDev{uint32_t(b->frames.size()), g});
   }
   F.coeff_group_base = b->total_groups;
   b->total_groups += F.num_groups;

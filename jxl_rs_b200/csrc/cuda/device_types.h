@@ -31,16 +31,25 @@ constexpr uint32_t kOffBase = kListCap + kListPad;     // first offset word
 constexpr uint32_t kOffWords = 3 * 1024 + 4;           // offsets of <= 1024 varblocks x 3 channels + end, 16-byte multiple
 constexpr uint32_t kListStride = kOffBase + kOffWords;  // u32 words per list
 
+// One entropy code (decode.rs:36-58) of a VarDCT pass (PassDev::code) or a Modular stream (MBatchDev::codes), tables in
+// the blob.
+struct CodeDev {
+  uint32_t use_prefix, log_alpha, num_clusters;
+  // LZ77 (decode.rs:36-45): tokens >= lz_min_symbol start a copy of hybrid(lz_len_cfg) + lz_min_length symbols, whose
+  // distance is read from cluster lz_dist_cluster
+  uint32_t lz_enabled, lz_min_symbol, lz_min_length, lz_len_cfg, lz_dist_cluster;
+  uint64_t cmap_off;         // u8[num_contexts]
+  uint64_t cfg_off;          // u32[num_clusters], packed as HybridUint::packed()
+  uint64_t ans_off;          // u64[num_clusters << log_alpha] alias buckets (ans.rs:31-39)
+  uint64_t huff_off;         // u32[] bits | value << 16
+  uint64_t huff_offset_off;  // u32[num_clusters]
+};
+
 struct PassDev {
-  uint32_t shift, use_prefix, log_alpha_size, num_clusters;
-  uint32_t lz77_enabled, lz77_min_symbol, lz77_min_length, lz77_length_uint, lz_dist_cluster;
+  CodeDev code;
+  uint32_t shift;
   uint32_t custom_orders;
-  uint64_t context_map_off;   // u8[]
-  uint64_t uint_configs_off;  // u32[num_clusters]
-  uint64_t ans_off;           // u64[num_clusters << log_alpha_size]
-  uint64_t huff_off;          // u32[] entries
-  uint64_t huff_offset_off;   // u32[num_clusters]
-  uint64_t order_off;         // u32[] custom orders
+  uint64_t order_off;  // u32[] custom orders
   uint32_t order_offset[39];
 };
 

@@ -301,18 +301,18 @@ __device__ __forceinline__ int decode_block_pass(const BatchDev& B, const FrameD
 
 __device__ __forceinline__ PassTables make_tables(const BatchDev& B, const PassDev& P) {
   PassTables T;
-  T.context_map = B.blob + P.context_map_off;
-  T.uint_configs = reinterpret_cast<const uint32_t*>(B.blob + P.uint_configs_off);
-  T.ans = reinterpret_cast<const uint2*>(B.blob + P.ans_off);
-  T.huff = reinterpret_cast<const uint32_t*>(B.blob + P.huff_off);
-  T.huff_offset = reinterpret_cast<const uint32_t*>(B.blob + P.huff_offset_off);
-  T.use_prefix = P.use_prefix;
-  T.log_alpha_size = P.log_alpha_size;
-  T.lz_enabled = P.lz77_enabled;
-  T.lz_min_symbol = P.lz77_min_symbol;
-  T.lz_min_length = P.lz77_min_length;
-  T.lz_len_cfg = P.lz77_length_uint;
-  T.lz_dist_cluster = P.lz_dist_cluster;
+  T.context_map = B.blob + P.code.cmap_off;
+  T.uint_configs = reinterpret_cast<const uint32_t*>(B.blob + P.code.cfg_off);
+  T.ans = reinterpret_cast<const uint2*>(B.blob + P.code.ans_off);
+  T.huff = reinterpret_cast<const uint32_t*>(B.blob + P.code.huff_off);
+  T.huff_offset = reinterpret_cast<const uint32_t*>(B.blob + P.code.huff_offset_off);
+  T.use_prefix = P.code.use_prefix;
+  T.log_alpha_size = P.code.log_alpha;
+  T.lz_enabled = P.code.lz_enabled;
+  T.lz_min_symbol = P.code.lz_min_symbol;
+  T.lz_min_length = P.code.lz_min_length;
+  T.lz_len_cfg = P.code.lz_len_cfg;
+  T.lz_dist_cluster = P.code.lz_dist_cluster;
   return T;
 }
 
@@ -325,7 +325,7 @@ __device__ __forceinline__ int init_pass(const BatchDev& B, const FrameDev& F, u
   s.br.skip(nb);
   if (s.hist_idx >= F.num_histograms) return JXG_ERR_INVALID_HISTOGRAM_INDEX;
   s.ans_state = 0x130000u;
-  if (!F.passes[pass].use_prefix) {  // ans.rs:431
+  if (!F.passes[pass].code.use_prefix) {  // ans.rs:431
     s.ans_state = s.br.peek32();
     s.br.skip(32);
   }
@@ -339,7 +339,7 @@ __device__ __forceinline__ int finish_pass(const BatchDev& B, const FrameDev& F,
   const SectionDev sec = B.sections[F.section_base + pass * F.num_groups + g];
   if (s.lz_err) return JXG_ERR_LZ77;
   if (s.br.bitpos > sec.len * 8u) return JXG_ERR_OUT_OF_BOUNDS;                         // bit_reader.rs:109
-  if (!F.passes[pass].use_prefix && s.ans_state != 0x130000u) return JXG_ERR_ANS_CHECKSUM;  // ans.rs:441
+  if (!F.passes[pass].code.use_prefix && s.ans_state != 0x130000u) return JXG_ERR_ANS_CHECKSUM;  // ans.rs:441
   return 0;
 }
 
@@ -673,12 +673,12 @@ __global__ void __launch_bounds__(128, 6) k_entropy_lean(const BatchDev B) {
   const uint32_t nbc = F.num_block_contexts;
   if (CTXS) {
     const uint32_t num_ctx = F.num_histograms * nbc * (37 + 458);
-    const uint8_t* src = B.blob + P.context_map_off;  // 16-byte aligned in the blob
+    const uint8_t* src = B.blob + P.code.cmap_off;  // 16-byte aligned in the blob
     for (uint32_t i = threadIdx.x * 16; i < num_ctx + 64; i += blockDim.x * 16)  // speculative look-ups run a bit past the end
       *reinterpret_cast<uint4*>(s_ctxmap + i) = __ldg(reinterpret_cast<const uint4*>(src + i));
   }
   __syncthreads();
-  const uint8_t* const ctxmap_g = B.blob + P.context_map_off;
+  const uint8_t* const ctxmap_g = B.blob + P.code.cmap_off;
   // Shared-window addresses of the three look-up tables, made opaque so that they stay in registers: left to itself the
   // compiler rematerialises them inside the per-symbol loop (S2R SR_CgaCtaId + LEA + adds, ~8 of the ~92 instructions).
   uint32_t ctxmap_s = uint32_t(__cvta_generic_to_shared(s_ctxmap));
@@ -696,9 +696,9 @@ __global__ void __launch_bounds__(128, 6) k_entropy_lean(const BatchDev B) {
   bool done = !(lane < wsched.y && qpos < F.lean_count);
   uint8_t* const nz = s_nzcol[(threadIdx.x >> 5) * S + (lane < S ? lane : 0)];
   // ---- per-frame constants ----
-  const uint32_t* const ucfg = reinterpret_cast<const uint32_t*>(B.blob + P.uint_configs_off);
-  const uint2* const ans = reinterpret_cast<const uint2*>(B.blob + P.ans_off);
-  const uint32_t log_alpha = P.log_alpha_size, log_bucket = 12 - P.log_alpha_size, bucket_mask = (1u << (12 - P.log_alpha_size)) - 1;
+  const uint32_t* const ucfg = reinterpret_cast<const uint32_t*>(B.blob + P.code.cfg_off);
+  const uint2* const ans = reinterpret_cast<const uint2*>(B.blob + P.code.ans_off);
+  const uint32_t log_alpha = P.code.log_alpha, log_bucket = 12 - P.code.log_alpha, bucket_mask = (1u << (12 - P.code.log_alpha)) - 1;
   // ---- per-stream state (re-initialised by the set-up path when a lane takes a new stream) ----
   uint32_t gsid = 0, nblk = 0, bi = 0;
   const uint4* desc = B.desc;

@@ -40,7 +40,7 @@ struct ModularBatch : BatchCore {
   std::vector<MStreamDev> streams;
   std::vector<uint32_t> order, rct_streams;
   std::vector<MRectDev> rects;
-  std::vector<MCodeDev> codes;
+  std::vector<CodeDev> codes;
   std::vector<MRctDev> rcts;
   std::vector<uint32_t> refs;
   std::vector<std::vector<MJobDev>> levels;  // jobs grouped by plan step index
@@ -64,7 +64,7 @@ uint64_t blob_append(ModularBatch* b, const void* p, size_t bytes, size_t align 
 }
 
 uint32_t add_code(ModularBatch* b, const jxg::EntropyCode& c) {
-  MCodeDev d;
+  CodeDev d;
   memset(&d, 0, sizeof(d));
   if (c.lz77_enabled) {
     d.lz_enabled = 1;
@@ -456,7 +456,7 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
   B.order = reinterpret_cast<const uint32_t*>(B.blob + b->tab.order);
   B.rct_streams = reinterpret_cast<const uint32_t*>(B.blob + b->tab.rct_streams);
   B.rects = reinterpret_cast<const MRectDev*>(B.blob + b->tab.rects);
-  B.codes = reinterpret_cast<const MCodeDev*>(B.blob + b->tab.codes);
+  B.codes = reinterpret_cast<const CodeDev*>(B.blob + b->tab.codes);
   B.rcts = reinterpret_cast<const MRctDev*>(B.blob + b->tab.rcts);
   B.refs = reinterpret_cast<const uint32_t*>(B.blob + b->tab.refs);
   B.planes = static_cast<int32_t*>(cx->d_planes_a.p);

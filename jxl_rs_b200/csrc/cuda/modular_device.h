@@ -3,19 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-namespace jxgpu {
+#include "device_types.h"  // CodeDev
 
-struct MCodeDev {  // one EntropyCode (decode.rs:36-58), tables in the blob
-  uint32_t use_prefix, log_alpha, num_clusters, pad;
-  uint64_t cmap_off;         // u8[num_contexts]
-  uint64_t cfg_off;          // u32[num_clusters], packed as HybridUint::packed()
-  uint64_t ans_off;          // u64[num_clusters << log_alpha] alias buckets (ans.rs:31-39)
-  uint64_t huff_off;         // u32[] bits | value << 16
-  uint64_t huff_offset_off;  // u32[num_clusters]
-  // LZ77 (decode.rs:36-45): tokens >= lz_min_symbol start a copy of hybrid(lz_len_cfg) + lz_min_length symbols, whose
-  // distance is read from cluster lz_dist_cluster
-  uint32_t lz_enabled, lz_min_symbol, lz_min_length, lz_len_cfg, lz_dist_cluster, lz_pad;
-};
+namespace jxgpu {
 
 struct MStreamDev {  // one ModularHF(group) section
   uint32_t frame, group;
@@ -72,7 +62,7 @@ struct MBatchDev {
   const uint32_t* order;        // stream indices, longest section first
   const uint32_t* rct_streams;  // streams with local RCTs
   const MRectDev* rects;
-  const MCodeDev* codes;
+  const CodeDev* codes;
   const MRctDev* rcts;
   const uint32_t* refs;  // rect indices, see MRectDev::ref_first
   int32_t* planes;

@@ -425,7 +425,7 @@ __global__ void __launch_bounds__(128) k_modular_decode(const MBatchDev B, const
   if (lane >= S) return;
   for (uint32_t sidx = warp * S + lane; sidx < B.num_streams; sidx = atomicAdd(B.queue, 1u) + total_lanes) {
     const MStreamDev& st = B.streams[B.order[sidx]];
-    const MCodeDev& code = B.codes[st.code];
+    const CodeDev& code = B.codes[st.code];
     MSym sym;
     sym.br.init(reinterpret_cast<const uint32_t*>(B.blob + st.sec_off), (st.sec_len >> 2) + 1, st.data_bitpos);
     sym.cmap = B.blob + code.cmap_off;

@@ -76,7 +76,7 @@ struct EntropyCode {
 };
 
 
-// decode.rs:177-405 (host copy; the device kernel has its own).
+// decode.rs:177-405 (host copy; the VarDCT and Modular device kernels each have their own, DESIGN §9 item 6).
 class SymbolReader {
  public:
   SymbolReader(const EntropyCode& code, BitReader& br, size_t dist_multiplier);
