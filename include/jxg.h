@@ -296,6 +296,13 @@ int jxg_modular_batch_stats(void* batch, uint64_t* h2d_bytes, uint64_t* d2h_byte
 /* Group streams of the frames added so far whose code uses LZ77; of those, the ones whose copies all have distance 1
  * (Histograms::is_rle, the shape of libjxl's fastest lossless mode); device bytes of their symbol windows. */
 int jxg_modular_batch_lz77_stats(void* batch, uint32_t* lz77_streams, uint32_t* rle_streams, uint64_t* window_bytes);
+/* Non-empty group-stream rects of the frames added so far, by the channel walk the decode kernel takes for them (the
+ * walk chosen at jxg_modular_batch_add, after the channel / stream decisions of the tree): the generic tree walk; the
+ * table walk of a single leaf; the table walk over property p in by_property[p] (16 entries, 2..15 used, see
+ * jxg_modular_walk_table); and of the table rects, those whose stream uses the weighted predictor. Any pointer may be
+ * NULL. */
+int jxg_modular_batch_walk_stats(void* batch, uint32_t* generic, uint32_t* single_leaf, uint32_t* by_property,
+                                 uint32_t* table_wp);
 void jxg_modular_batch_end(void* batch);
 /* Parity tap (no device needed): the table form of one channel's MA-tree walk as the Modular path builds it - the device
  * counterpart of the single-property specialisations of frame/modular/decode/specialized_trees.rs:197-372.

@@ -74,7 +74,7 @@ EXPORTS = [
     "jxg_modular_parse_file", "jxg_modular_parsed_free", "jxg_modular_batch_begin", "jxg_modular_batch_add",
     "jxg_modular_batch_set_lanes", "jxg_modular_batch_run", "jxg_modular_batch_wait", "jxg_modular_batch_rerun_device",
     "jxg_modular_batch_read_planes", "jxg_modular_batch_stats", "jxg_modular_batch_end", "jxg_modular_walk_table",
-    "jxg_modular_batch_lz77_stats",
+    "jxg_modular_batch_lz77_stats", "jxg_modular_batch_walk_stats",
 ]
 
 _LIB = None
@@ -127,6 +127,7 @@ def load_library():
                                             C.POINTER(C.c_float)]
     lib.jxg_modular_batch_end.argtypes = [vp]
     lib.jxg_modular_batch_lz77_stats.argtypes = [vp, u32p, u32p, C.POINTER(C.c_uint64)]
+    lib.jxg_modular_batch_walk_stats.argtypes = [vp, u32p, u32p, u32p, u32p]
     lib.jxg_modular_walk_table.argtypes = [C.POINTER(C.c_int32), C.c_uint32, C.POINTER(C.c_uint8), C.c_uint32, C.c_uint32,
                                            C.c_uint32, u32p, u32p]
     lib.jxg_modular_batch_end.restype = None

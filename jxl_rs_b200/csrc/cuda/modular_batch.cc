@@ -34,6 +34,12 @@ struct MFrame {
   size_t dev_out_off = 0;
 };
 
+// Non-empty group-stream rects by the channel walk the decode kernel takes for them: the generic tree walk, the table
+// walk without a property (a single leaf) or over property p (2..15); of the table rects, those whose stream uses WP.
+struct WalkStats {
+  uint32_t generic = 0, single = 0, by_prop[16] = {}, table_wp = 0;
+};
+
 // Device buffers: the context's pools; tables: in its pinned blob. A steady-state loop of batches allocates nothing.
 struct ModularBatch : BatchCore {
   std::vector<MFrame> frames;
@@ -50,6 +56,7 @@ struct ModularBatch : BatchCore {
   uint64_t lz_window_elems = 0;             // symbol windows of the LZ77 streams, one per stream
   uint32_t lz77_streams = 0, rle_streams = 0;  // streams with LZ77; of those, streams whose copies all have distance 1
   uint32_t num_plain = 0;                   // streams without LZ77: the first ones of `order`
+  WalkStats walks;                          // routes of the non-empty group-stream rects (jxg_modular_batch_walk_stats)
   uint32_t lanes_per_warp = 1;
   cudaEvent_t ev_decode = nullptr;
   struct {  // byte offsets of the batch tables in the blob
@@ -203,13 +210,14 @@ struct BatchMark {
   std::vector<size_t> level_jobs;
   uint64_t arena_elems, wp_bytes, out_bytes, lz_window_elems;
   uint32_t lz77_streams, rle_streams;
+  WalkStats walks;
 
   explicit BatchMark(const ModularBatch* b)
       : frames(b->frames.size()), streams(b->streams.size()), rct_streams(b->rct_streams.size()), rects(b->rects.size()),
         codes(b->codes.size()), rcts(b->rcts.size()), refs(b->refs.size()), levels(b->levels.size()),
         store_jobs(b->store_jobs.size()), blob(b->ctx->blob.size), blob_pending(b->ctx->blob.pending.size()),
         arena_elems(b->arena_elems), wp_bytes(b->wp_bytes), out_bytes(b->out_bytes), lz_window_elems(b->lz_window_elems),
-        lz77_streams(b->lz77_streams), rle_streams(b->rle_streams) {
+        lz77_streams(b->lz77_streams), rle_streams(b->rle_streams), walks(b->walks) {
     for (const auto& l : b->levels) level_jobs.push_back(l.size());
   }
   void restore(ModularBatch* b) const {
@@ -232,6 +240,7 @@ struct BatchMark {
     b->lz_window_elems = lz_window_elems;
     b->lz77_streams = lz77_streams;
     b->rle_streams = rle_streams;
+    b->walks = walks;
   }
 };
 
@@ -327,6 +336,13 @@ void add_streams(ModularBatch* b, MFrame& f) {
         }
         rd.walk = it->second.walk;
         rd.lut_off = it->second.lut_off;
+        if ((rd.walk & 0xff) != kWalkLut) {
+          b->walks.generic++;
+        } else {
+          if ((rd.walk >> 8) == kLutNoProperty) b->walks.single++;
+          else b->walks.by_prop[(rd.walk >> 8) & 15]++;
+          if (d.uses_wp) b->walks.table_wp++;
+        }
       }
       // reference channels: earlier channels of the stream with the same shape, nearest first (common.rs:52-60)
       rd.ref_first = uint32_t(b->refs.size());
@@ -671,6 +687,17 @@ int jxg_modular_batch_lz77_stats(void* bp, uint32_t* lz77_streams, uint32_t* rle
   if (lz77_streams) *lz77_streams = b->lz77_streams;
   if (rle_streams) *rle_streams = b->rle_streams;
   if (window_bytes) *window_bytes = b->lz_window_elems * 4;
+  return JXG_OK;
+}
+
+int jxg_modular_batch_walk_stats(void* bp, uint32_t* generic, uint32_t* single_leaf, uint32_t* by_property,
+                                 uint32_t* table_wp) {
+  ModularBatch* b = static_cast<ModularBatch*>(bp);
+  if (!b) return JXG_ERR_ARGUMENT;
+  if (generic) *generic = b->walks.generic;
+  if (single_leaf) *single_leaf = b->walks.single;
+  if (by_property) memcpy(by_property, b->walks.by_prop, sizeof(b->walks.by_prop));
+  if (table_wp) *table_wp = b->walks.table_wp;
   return JXG_OK;
 }
 

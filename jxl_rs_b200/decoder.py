@@ -493,6 +493,18 @@ class ModularBatch(_BatchHandle):
         abi.check(self._lib, self._lib.jxg_modular_batch_lz77_stats(self._h, C.byref(n), C.byref(rle), C.byref(win)))
         return {"lz77_streams": n.value, "rle_streams": rle.value, "window_bytes": win.value}
 
+    def walk_stats(self):
+        """Non-empty group-stream rects of the added frames by the channel walk they take on the device: "generic" (the
+        tree walk), "single_leaf" (the table walk of a tree left with one leaf), "by_property" {p: rects} (the table
+        walk over property p, 2..15; properties without rects left out) and "table_wp" (table rects whose stream uses
+        the weighted predictor)."""
+        gen, single, wp = C.c_uint32(), C.c_uint32(), C.c_uint32()
+        by = (C.c_uint32 * 16)()
+        abi.check(self._lib, self._lib.jxg_modular_batch_walk_stats(self._h, C.byref(gen), C.byref(single), by,
+                                                                    C.byref(wp)))
+        return {"generic": gen.value, "single_leaf": single.value,
+                "by_property": {p: by[p] for p in range(16) if by[p]}, "table_wp": wp.value}
+
     def read_planes(self, f: int):
         import numpy as np
         fr = self.frames[f]

@@ -4,10 +4,10 @@ import pytest
 from jxl_rs_b200 import abi
 
 
-def gpu_decode(ctx, files, lanes=1, lz77_stats=False, expect_error=False, refused=()):
+def gpu_decode(ctx, files, lanes=1, lz77_stats=False, expect_error=False, refused=(), walk_stats=False):
     """Decodes `files` as one ModularBatch with `lanes` lanes per warp into pinned host buffers. Returns the u8 outputs
-    and the i32 planes of the frames the batch kept, then, when asked for, the batch's lz77_stats() before run() and
-    the JxgError of wait() (None if it succeeded; without `expect_error` the error is raised). Adding a frame whose
+    and the i32 planes of the frames the batch kept, then, when asked for, the batch's lz77_stats() before run(), its
+    walk_stats() before run() and the JxgError of wait() (None if it succeeded; without `expect_error` the error is raised). Adding a frame whose
     index is in `refused` must raise JxgError; the batch goes on without it."""
     import torch
     import jxl_rs_b200 as j
@@ -25,6 +25,7 @@ def gpu_decode(ctx, files, lanes=1, lz77_stats=False, expect_error=False, refuse
                 b.add(fr, o.data_ptr(), fr.width * 3, False)
                 kept.append(i)
         stats = b.lz77_stats()
+        walks = b.walk_stats()
         b.run()
         try:
             b.wait()
@@ -38,6 +39,8 @@ def gpu_decode(ctx, files, lanes=1, lz77_stats=False, expect_error=False, refuse
     result = ([outs[i].numpy().copy() for i in kept], planes)
     if lz77_stats:
         result += (stats,)
+    if walk_stats:
+        result += (walks,)
     if expect_error:
         result += (err,)
     return result

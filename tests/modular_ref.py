@@ -119,14 +119,22 @@ def validate_tree(nodes, num_properties):
         stack.append((n[3], depth + 1, left))
 
 
-def walk(nodes, props, trace=None):
-    """tree.rs:364-390: property > value goes left."""
+def walk(nodes, props, trace=None, cov=None):
+    """tree.rs:364-390: property > value goes left. cov: records the sides of each split taken and the range of the
+    values each split property had there."""
     i = 0
     while nodes[i][0] == "split":
         _, p, val, left, right = nodes[i]
-        go_left = props[p] > val
+        v = props[p]
+        go_left = v > val
         if trace is not None:
             trace.add((p, go_left))
+        if cov is not None:
+            cov.split_sides.add((p, val, go_left))
+            if 0 <= v - val <= 1:
+                cov.split_edges.add((p, val, v - val))
+            lo, hi = cov.prop_range.get(p, (v, v))
+            cov.prop_range[p] = (min(lo, v), max(hi, v))
         i = left if go_left else right
     return nodes[i]
 
@@ -285,7 +293,9 @@ def make_pixel(dec, mul, guess):
 # ---------------------------------------------------------------------------------------------------------------------
 class Coverage:
     """What a run reached: pixels per predictor, (property, branch) pairs, offset / multiplier leaves, wrapped
-    make_pixel results, RCT types; for Squeeze: (tendency branch, clamp, fired) triples, tail columns / rows ("h" /
+    make_pixel results, RCT types, (property, split value, went left) triples of the splits taken, (property, split
+    value, 0 or 1) for a property value equal to the split value or one above it, and per split property the least
+    and greatest value it had at a split; for Squeeze: (tendency branch, clamp, fired) triples, tail columns / rows ("h" /
     "v"), zero-width / zero-height residuals, in_place = false and meta squeezes, the default rules that fired,
     (section kind, shift) pairs of the coded channels, and outputs the `as i32` of unsqueeze wrapped."""
 
@@ -307,6 +317,9 @@ class Coverage:
         self.ref_slots = set()
         self.palette = set()
         self.wrapped_props = set()
+        self.split_sides = set()
+        self.split_edges = set()
+        self.prop_range = {}
 
     def merge(self, o):
         self.predictors |= o.predictors
@@ -319,6 +332,11 @@ class Coverage:
         self.ref_slots |= o.ref_slots
         self.palette |= o.palette
         self.wrapped_props |= o.wrapped_props
+        self.split_sides |= o.split_sides
+        self.split_edges |= o.split_edges
+        for p, (lo, hi) in o.prop_range.items():
+            a, b = self.prop_range.get(p, (lo, hi))
+            self.prop_range[p] = (min(a, lo), max(b, hi))
         for k in self.SQUEEZE_SETS:
             getattr(self, k).update(getattr(o, k))
         self.not_in_place += o.not_in_place
@@ -382,7 +400,7 @@ def decode_channels(chans, stream_id, tree, wp_hdr, chooser, cov, faults=()):
                     dv = v - clamped_gradient(vl, vt, vtl)
                     props[16 + 4 * k: 20 + 4 * k] = [wrap32(abs(v)), v, wrap32(abs(dv)), wrap32(dv)]
                     cov.ref_slots.add(k)
-                leaf = walk(nodes, props, cov.branches)
+                leaf = walk(nodes, props, cov.branches, cov)
                 _, pred, off, mul, leaf_id = leaf
                 guess = predict_one(pred, d, wp_pred, faults) + off
                 dec = chooser(guess, mul, x, y, ci)
