@@ -20,7 +20,7 @@ def _lib():
         _LIB.jxs_encode_synthetic_ex.restype = C.c_int64
         _LIB.jxs_encode_synthetic_ex.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64, C.c_float, C.c_uint32, C.c_uint32,
                                                  C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,
-                                                 C.c_void_p, C.c_size_t]
+                                                 C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
         _LIB.jxs_last_error.restype = C.c_char_p
         _LIB.jxs_set_threads.argtypes = [C.c_int]
         _LIB.jxs_encode_modular.restype = C.c_int64
@@ -45,7 +45,7 @@ def _lib():
 
 
 def encode_synthetic(width, height, seed, distance=1.0, epf_iters=2, gab=1, profile=1, lf_tree=0, entropy=0, orientation=1,
-                     colour=0, dequant=None, x_qm_scale=3, b_qm_scale=2) -> bytes:
+                     colour=0, dequant=None, x_qm_scale=3, b_qm_scale=2, header=None) -> bytes:
     """One synthetic VarDCT frame. profile 0: DCT8x8 only; 1: mixed transforms up to 32x32;
     2: also 64x64 / 64x32 / 32x64; 3: also the 128 / 256 families (DCT128X128 ... DCT256X256, transform types 21..26);
     4: profile 3 plus IDENTITY, DCT2X2 and AFV0-3 among the 8x8 blocks, so that every dequantisation table is used.
@@ -58,18 +58,26 @@ def encode_synthetic(width, height, seed, distance=1.0, epf_iters=2, gab=1, prof
     dequant: None (DequantMatrices all_default) or 17 entries, each None (library table) or a custom encoding in the
     form of tests/f64_quant.py (a dict with "mode" 1..7 and its parameters as f16 bit patterns), written as given,
     also when the decoder must refuse it. x_qm_scale, b_qm_scale: the frame header's 0..7. The coefficients are
-    quantised with the tables the decoder computes from what is written."""
+    quantised with the tables the decoder computes from what is written.
+    header: None (default fields) or a dict of fields written as given, every float a 16-bit f16 pattern (see
+    _header_words); the writer checks nothing, so frames the decoder must refuse can be written. The source picture
+    is converted with the opsin matrix and biases written, and quantised with the colour correlation (factor, bases,
+    LF factors, tile maps clamped to i8) the decoder derives, so the round trip holds as for default headers; a
+    non-finite f16 falls back to the default value there (the decoder refuses such a frame). Gaborish and EPF are not
+    inverted by the writer, as with the default weights."""
     profile = ((profile & 0xff) | ((lf_tree & 1) << 8) | ((entropy & 3) << 9) | (((orientation - 1) & 7) << 12)
                | ((colour & 15) << 16))
     lib = _lib()
     words = _dequant_words(dequant)
     arr = (C.c_uint32 * max(1, len(words)))(*[w & 0xFFFFFFFF for w in words])
+    hwords = _header_words(header)
+    harr = (C.c_uint32 * max(1, len(hwords)))(*[int(w) & 0xFFFFFFFF for w in hwords])
 
     def run(buf, cap):
-        if not words and (x_qm_scale, b_qm_scale) == (3, 2):
+        if not words and not hwords and (x_qm_scale, b_qm_scale) == (3, 2):
             return lib.jxs_encode_synthetic(width, height, seed, distance, epf_iters, gab, profile, buf, cap)
         return lib.jxs_encode_synthetic_ex(width, height, seed, distance, epf_iters, gab, profile, x_qm_scale, b_qm_scale,
-                                           arr, len(words), buf, cap)
+                                           arr, len(words), harr, len(hwords), buf, cap)
     cap = max(1 << 16, width * height * 2 + 4 * len(words))
     buf = C.create_string_buffer(cap)
     n = run(buf, cap)
@@ -114,6 +122,46 @@ def _dequant_words(dequant):
         if mode == 7:
             import numpy as np
             words += np.asarray(enc["raw"], np.int64).ravel().tolist()
+    return words
+
+
+def _header_words(header):
+    """The flat u32 array of jxs_encode_synthetic_ex's header. Keys of `header`, each optional (absent: not custom):
+      gab: the six Gaborish weights x w1, x w2, y w1, y w2, b w1, b w2 (written when gab = 1);
+      sharp: the 8 entries of epf_sharp_lut; weight: epf_channel_scale X, Y, B and the two zeroflush values (parsed
+      and ignored); sigma: epf_quant_mul, epf_pass0_sigma_scale, epf_pass2_sigma_scale, epf_border_sad_mul (the EPF
+      groups are written when epf_iters > 0);
+      color: {"factor": (selector 0..3, bits: 84 / 256 / bits + 2 (8 bits) / bits + 258 (16 bits)), "base_x",
+      "base_b", "ytox_lf", "ytob_lf" (integers -128..127)};
+      opsin: {"matrix": 9, "biases": 3, "quant_biases": 4};
+      cfl: (ytox, ytob), each one integer per 64x64 tile in raster order, any i32 (the decoder clamps to i8)."""
+    if not header:
+        return []
+    words = []
+    for key, n in (("gab", 6), ("sharp", 8), ("weight", 5), ("sigma", 4)):
+        v = header.get(key)
+        assert v is None or len(v) == n, key
+        words += [0] * (n + 1) if v is None else [1] + [int(x) & 0xFFFF for x in v]
+    cc = header.get("color")
+    if cc is None:
+        words += [0, 0, 0, 0, 0, 128, 128]
+    else:
+        sel, bits = cc.get("factor", (0, 0))
+        words += [1, sel, bits, cc.get("base_x", 0), cc.get("base_b", 0x3C00), cc.get("ytox_lf", 0) + 128,
+                  cc.get("ytob_lf", 0) + 128]
+    op = header.get("opsin")
+    if op is None:
+        words += [0] * 17
+    else:
+        assert len(op["matrix"]) == 9 and len(op["biases"]) == 3 and len(op["quant_biases"]) == 4
+        words += [1] + [int(x) & 0xFFFF for x in list(op["matrix"]) + list(op["biases"]) + list(op["quant_biases"])]
+    cfl = header.get("cfl")
+    if cfl is None:
+        words.append(0)
+    else:
+        ytox, ytob = (list(_flat(m)) for m in cfl)
+        assert len(ytox) == len(ytob)
+        words += [len(ytox)] + [int(v) for v in ytox] + [int(v) for v in ytob]
     return words
 
 
@@ -270,8 +318,9 @@ def encode_modular_tokens(spec) -> bytes:
 
 def encode_vardct_tokens(spec) -> bytes:
     """One VarDCT frame whose AC coefficient streams hold exactly the given tokens; the writer predicts nothing and checks
-    nothing (frames a decoder must refuse can be written). The image metadata, the LF quantisation, the dequantisation
-    matrices, the colour correlation and the filters are the defaults. `spec` is a dict:
+    nothing (frames a decoder must refuse can be written). The image metadata, the LF quantisation and the
+    dequantisation matrices are the defaults; so are the colour correlation, the opsin fields, the filter weights and
+    the CfL maps unless `header` / `cfl` give them. `spec` is a dict:
       width, height; shifts: one per pass (1..11 passes), the last one 0;
       bcm: None (the default BlockContextMap) or {"lf": [X, Y, B threshold lists], "qf": [thresholds as decoded, >= 1],
       "map": block context per (channel, order, qf bucket, LF bucket)};
@@ -281,9 +330,16 @@ def encode_vardct_tokens(spec) -> bytes:
       permutation of 64 * num_blocks entries, the first num_blocks fixed}, "cmap": context -> cluster, "cfgs": hybrid
       (split_exponent, msb, lsb) per cluster, "log_alpha": the smallest ANS alphabet (log2), "prefix": prefix codes,
       "lz77": None or (min_symbol, min_length)};
-      sections: per pass, per group: (histogram index, [(context, u32 value), ...])."""
+      sections: per pass, per group: (histogram index, [(context, u32 value), ...]);
+      header (optional): the header fields of encode_synthetic's `header` dict (_header_words), written as given; its
+      restoration filter groups apply to the frame's Gaborish + EPF 2 header;
+      cfl (optional): (ytox, ytob) CfL tile maps, one i32 per 64x64 tile in raster order (default: zeros)."""
     import numpy as np
-    words = [spec["width"], spec["height"], len(spec["shifts"])] + list(spec["shifts"][:-1])
+    header = dict(spec.get("header") or {})
+    if spec.get("cfl") is not None:
+        header["cfl"] = spec["cfl"]
+    hwords = _header_words(header)
+    words = [len(hwords)] + hwords + [spec["width"], spec["height"], len(spec["shifts"])] + list(spec["shifts"][:-1])
     bcm = spec.get("bcm")
     if bcm is None:
         words.append(0)

@@ -60,6 +60,25 @@ struct Params {
     std::vector<int32_t> raw;                            // mode 7: 3 channels of 8*REQUIRED_SIZE_X columns
   };
   std::vector<DequantSpec> dequant = {};                 // empty or kNumQuantTables entries
+  // Header fields written as given (see jxs_encode_synthetic_ex); every float is a 16-bit f16 pattern. A group whose
+  // flag is off keeps the bitstream's default (all_default / *_custom = 0).
+  struct HeaderSpec {
+    bool gab_custom = false;
+    uint16_t gab[6] = {};           // x w1, x w2, y w1, y w2, b w1, b w2 (frame_header.rs:157-179)
+    bool sharp_custom = false;
+    uint16_t sharp[8] = {};         // epf_sharp_lut
+    bool weight_custom = false;
+    uint16_t weight[5] = {};        // epf_channel_scale[3], epf_pass1_zeroflush, epf_pass2_zeroflush
+    bool sigma_custom = false;
+    uint16_t sigma[4] = {};         // epf_quant_mul, epf_pass0_sigma_scale, epf_pass2_sigma_scale, epf_border_sad_mul
+    bool cc_custom = false;         // ColorCorrelationParams (color_correlation_map.rs:42-72)
+    uint32_t cf_sel = 0, cf_bits = 0;
+    uint16_t base_x = 0, base_b = 0;
+    uint32_t ytox_lf = 128, ytob_lf = 128;  // the 8-bit fields: value + 128
+    bool ct_custom = false;         // CustomTransformData's OpsinInverseMatrix (transform_data.rs:18-32)
+    uint16_t opsin[9] = {}, bias[3] = {}, qbias[4] = {};
+    std::vector<int32_t> cfl_x, cfl_b;  // CfL tile maps, one value per 64x64 tile; empty: random small values
+  } hdr = {};
 };
 
 // Worker threads inside one encode (jxs_set_threads): only loops whose result does not depend on the order of
@@ -273,7 +292,7 @@ struct Frame {
   std::vector<uint8_t> transform_map;  // t | 128 first
   std::vector<uint8_t> raw_quant;      // 1..255
   std::vector<uint8_t> sharp;
-  std::vector<int8_t> ytox, ytob;
+  std::vector<int32_t> ytox, ytob;     // CfL tile maps as written (the decoder clamps them to i8)
   std::vector<int32_t> lfq[3];         // quantised LF ints (X, Y, B)
   std::vector<Varblock> blocks;        // raster order of first blocks
   std::vector<std::vector<int32_t>> coeffs;  // per varblock: 3 * num_coeffs quantised ints (storage layout)
@@ -606,6 +625,52 @@ static const uint16_t kNzCtx[64] = {0xBAD, 0,   31,  62,  62,  93,  93,  93,  93
 static const uint8_t kDefaultBlockCtx[39] = {0, 1, 2, 2, 3,  3,  4,  5,  6,  6,  6,  6,  6,  7, 8, 9, 9, 10, 11, 12,
                                              13, 14, 14, 14, 14, 14, 7, 8, 9, 9, 10, 11, 12, 13, 14, 14, 14, 14, 14};
 
+// Header groups written as given by a HeaderSpec (shared by the synthetic and the token-level writers).
+static void write_color_correlation(BitWriter& bw, const Params::HeaderSpec& hd) {  // color_correlation_map.rs:42-72
+  bw.write(hd.cc_custom ? 0 : 1, 1);
+  if (!hd.cc_custom) return;
+  bw.write(hd.cf_sel & 3, 2);
+  if ((hd.cf_sel & 3) == 2) bw.write(hd.cf_bits & 0xff, 8);
+  if ((hd.cf_sel & 3) == 3) bw.write(hd.cf_bits & 0xffff, 16);
+  bw.write(hd.base_x, 16);
+  bw.write(hd.base_b, 16);
+  bw.write(hd.ytox_lf & 0xff, 8);
+  bw.write(hd.ytob_lf & 0xff, 8);
+}
+
+static void write_custom_transform_data(BitWriter& out, const Params::HeaderSpec& hd) {  // transform_data.rs:325-345
+  out.write(hd.ct_custom ? 0 : 1, 1);
+  if (!hd.ct_custom) return;
+  out.write(0, 1);  // OpsinInverseMatrix all_default (xyb_encoded is always set)
+  for (uint16_t v : hd.opsin) out.write(v, 16);
+  for (uint16_t v : hd.bias) out.write(v, 16);
+  for (uint16_t v : hd.qbias) out.write(v, 16);
+  out.write(0, 3);  // custom_weight_mask: default upsampling weights
+}
+
+// RestorationFilter after its all_default bit (frame_header.rs:146-234), extensions included
+static void write_restoration_filter(BitWriter& out, uint32_t gab, uint32_t epf_iters, const Params::HeaderSpec& hd) {
+  out.write(gab, 1);
+  if (gab) {
+    out.write(hd.gab_custom, 1);
+    if (hd.gab_custom)
+      for (uint16_t v : hd.gab) out.write(v, 16);
+  }
+  out.write(epf_iters, 2);
+  if (epf_iters > 0) {  // the custom groups exist only with EPF on (frame_header.rs:185-227)
+    out.write(hd.sharp_custom, 1);
+    if (hd.sharp_custom)
+      for (uint16_t v : hd.sharp) out.write(v, 16);
+    out.write(hd.weight_custom, 1);
+    if (hd.weight_custom)
+      for (uint16_t v : hd.weight) out.write(v, 16);
+    out.write(hd.sigma_custom, 1);
+    if (hd.sigma_custom)
+      for (uint16_t v : hd.sigma) out.write(v, 16);
+  }
+  out.write_u64(0);  // restoration filter extensions
+}
+
 std::vector<uint8_t> encode(const Params& p) {
   Frame f;
   f.p = p;
@@ -621,9 +686,31 @@ std::vector<uint8_t> encode(const Params& p) {
   const uint32_t PW = f.xb * 8, PH = f.yb * 8;
 
   // ---- source image -> padded XYB planes ----
+  // The values the decoder derives from the header fields as written; a non-finite f16 (a header the decoder refuses)
+  // falls back to the default so that the quantisation below stays defined.
+  const Params::HeaderSpec& hd = p.hdr;
+  auto f16v = [](uint16_t bits, float dflt) {
+    const float v = jxg::f16_bits_to_float(bits);
+    return std::isfinite(v) ? v : dflt;
+  };
+  jxg::OpsinInverseMatrix opsin;
+  if (hd.ct_custom) {
+    for (int i = 0; i < 9; i++) opsin.inverse_matrix[i] = f16v(hd.opsin[i], opsin.inverse_matrix[i]);
+    for (int i = 0; i < 3; i++) opsin.opsin_biases[i] = f16v(hd.bias[i], opsin.opsin_biases[i]);
+  }
+  float color_factor = 84.0f, base_x = 0.0f, base_b = 1.0f;
+  int ytox_lf = 0, ytob_lf = 0;
+  if (hd.cc_custom) {  // color_correlation_map.rs:46-64
+    const uint32_t cf[4] = {84, 256, hd.cf_bits + 2, hd.cf_bits + 258};
+    color_factor = float(cf[hd.cf_sel & 3]);
+    base_x = f16v(hd.base_x, 0.0f);
+    base_b = f16v(hd.base_b, 1.0f);
+    ytox_lf = int(hd.ytox_lf & 255) - 128;
+    ytob_lf = int(hd.ytob_lf & 255) - 128;
+  }
+  const float x_cc_lf = base_x + float(ytox_lf) / color_factor, b_cc_lf = base_b + float(ytob_lf) / color_factor;
   std::vector<float> img[3];
   make_image(p, img);
-  jxg::OpsinInverseMatrix opsin;
   to_xyb(img, opsin);
   std::vector<float> xyb[3];
   for (int c = 0; c < 3; c++) {
@@ -689,8 +776,14 @@ std::vector<uint8_t> encode(const Params& p) {
   const uint32_t cxb = (f.xb + 7) / 8, cyb = (f.yb + 7) / 8;
   f.ytox.assign(size_t(cxb) * cyb, 0);
   f.ytob.assign(size_t(cxb) * cyb, 0);
-  for (auto& v : f.ytox) v = int8_t(int(rng.below(9)) - 4);
-  for (auto& v : f.ytob) v = int8_t(int(rng.below(17)) - 8);
+  for (auto& v : f.ytox) v = int(rng.below(9)) - 4;
+  for (auto& v : f.ytob) v = int(rng.below(17)) - 8;
+  if (!hd.cfl_x.empty()) {
+    if (hd.cfl_x.size() != f.ytox.size() || hd.cfl_b.size() != f.ytob.size())
+      throw std::runtime_error("CfL maps take one value per 64x64 tile");
+    f.ytox = hd.cfl_x;
+    f.ytob = hd.cfl_b;
+  }
 
   // ---- transforms + quantisation ----
   for (auto& q : f.lfq) q.assign(nb, 0);
@@ -711,15 +804,16 @@ std::vector<uint8_t> encode(const Params& p) {
         int32_t qy = int32_t(std::lround(lf[1][i] / lf_fac[1]));
         float yy = float(qy) * lf_fac[1];
         f.lfq[1][o] = qy;
-        f.lfq[0][o] = int32_t(std::lround((lf[0][i] - yy * 0.0f) / lf_fac[0]));
-        f.lfq[2][o] = int32_t(std::lround((lf[2][i] - yy * 1.0f) / lf_fac[2]));
+        f.lfq[0][o] = int32_t(std::lround((lf[0][i] - yy * x_cc_lf) / lf_fac[0]));
+        f.lfq[2][o] = int32_t(std::lround((lf[2][i] - yy * b_cc_lf) / lf_fac[2]));
       }
     // HF (group.rs:100-177 inverted, without the decoder-side bias adjustment)
     const float* mat = tables[jxg::quant_table_for_transform(t)];
     const float rq = float(f.raw_quant[size_t(vb.by) * f.xb + vb.bx]);
     const float sy = inv_global_scale / rq, sx = sy * x_dm, sb = sy * b_dm;
     const size_t ci = size_t(vb.by / 8) * cxb + vb.bx / 8;
-    const float x_cc = 0.0f + float(f.ytox[ci]) / 84.0f, b_cc = 1.0f + float(f.ytob[ci]) / 84.0f;
+    const float x_cc = base_x + float(std::clamp(f.ytox[ci], -128, 127)) / color_factor;  // modular/mod.rs:1020-1029
+    const float b_cc = base_b + float(std::clamp(f.ytob[ci], -128, 127)) / color_factor;
     std::vector<int32_t>& q = f.coeffs[bi];
     q.assign(3 * num_coeffs, 0);
     auto quant = [](float v) {
@@ -845,7 +939,7 @@ std::vector<uint8_t> encode(const Params& p) {
     lf_global.write(0, 2);  // quant_lf = 16
   }
   lf_global.write(1, 1);  // default BlockContextMap
-  lf_global.write(1, 1);  // default ColorCorrelationParams
+  write_color_correlation(lf_global, hd);
   lf_global.write(0, 1);  // no global tree
 
   std::vector<BitWriter> lf_groups(f.num_lf_groups);
@@ -1024,10 +1118,11 @@ std::vector<uint8_t> encode(const Params& p) {
     }
     out.write_u64(0);                   // extensions
   }
-  out.write(1, 1);  // CustomTransformData all_default
+  write_custom_transform_data(out, hd);
   out.zero_pad_to_byte();
   // FrameHeader (frame_header.rs:267-444)
-  const bool default_header = p.epf_iters == 2 && p.gab == 1 && p.x_qm_scale == 3 && p.b_qm_scale == 2;
+  const bool custom_rf = hd.gab_custom || hd.sharp_custom || hd.weight_custom || hd.sigma_custom;
+  const bool default_header = p.epf_iters == 2 && p.gab == 1 && p.x_qm_scale == 3 && p.b_qm_scale == 2 && !custom_rf;
   if (default_header) {
     out.write(1, 1);
   } else {
@@ -1044,15 +1139,7 @@ std::vector<uint8_t> encode(const Params& p) {
     out.write(1, 1);       // is_last
     out.write(0, 2);       // name length 0
     out.write(0, 1);       // RestorationFilter all_default = 0
-    out.write(p.gab, 1);   // gab
-    if (p.gab) out.write(0, 1);  // gab_custom
-    out.write(p.epf_iters, 2);
-    if (p.epf_iters > 0) {
-      out.write(0, 1);  // epf_sharp_custom
-      out.write(0, 1);  // epf_weight_custom
-      out.write(0, 1);  // epf_sigma_custom
-    }
-    out.write_u64(0);  // restoration filter extensions
+    write_restoration_filter(out, p.gab, p.epf_iters, hd);
     out.write_u64(0);  // frame header extensions
   }
   std::vector<std::vector<uint8_t>> sections;
@@ -1077,6 +1164,37 @@ std::vector<uint8_t> encode(const Params& p) {
   std::vector<uint8_t> bytes = out.finish();
   for (auto& s : sections) bytes.insert(bytes.end(), s.begin(), s.end());
   return bytes;
+}
+
+// The header words of jxs_encode_synthetic_ex (synth/__init__.py _header_words gives the layout).
+static void read_header_words(const uint32_t* w, size_t n, Params::HeaderSpec& h) {
+  size_t pos = 0;
+  auto next = [&]() -> uint32_t {
+    if (pos >= n) throw std::runtime_error("header array too short");
+    return w[pos++];
+  };
+  auto group = [&](bool& flag, uint16_t* v, int count) {
+    flag = next() != 0;
+    for (int i = 0; i < count; i++) v[i] = uint16_t(next());
+  };
+  group(h.gab_custom, h.gab, 6);
+  group(h.sharp_custom, h.sharp, 8);
+  group(h.weight_custom, h.weight, 5);
+  group(h.sigma_custom, h.sigma, 4);
+  h.cc_custom = next() != 0;
+  h.cf_sel = next();
+  h.cf_bits = next();
+  h.base_x = uint16_t(next());
+  h.base_b = uint16_t(next());
+  h.ytox_lf = next();
+  h.ytob_lf = next();
+  group(h.ct_custom, h.opsin, 9);
+  for (uint16_t& v : h.bias) v = uint16_t(next());
+  for (uint16_t& v : h.qbias) v = uint16_t(next());
+  const uint32_t tiles = next();
+  for (uint32_t i = 0; i < tiles; i++) h.cfl_x.push_back(int32_t(next()));
+  for (uint32_t i = 0; i < tiles; i++) h.cfl_b.push_back(int32_t(next()));
+  if (pos != n) throw std::runtime_error("header array too long");
 }
 
 // ---------------------------------------------------------------------------
@@ -1138,12 +1256,21 @@ std::vector<uint8_t> encode_vardct_tokens(const uint32_t* w, size_t len) {
     if (pos >= len) throw std::runtime_error("VarDCT token spec too short");
     return w[pos++];
   };
+  // the header words (read_header_words) sit in front: their length, then the words
+  const uint32_t header_len = next();
+  if (header_len > len - pos) throw std::runtime_error("VarDCT token spec too short for its header");
+  Params::HeaderSpec hd;
+  if (header_len) read_header_words(w + pos, header_len, hd);
+  pos += header_len;
   const uint32_t W = next(), H = next(), num_passes = next();
   if (!W || !H || num_passes < 1 || num_passes > 11) throw std::runtime_error("bad size or pass count");
   std::vector<uint32_t> shifts(num_passes - 1);
   for (auto& s : shifts) s = next();
   const uint32_t xb = (W + 7) / 8, yb = (H + 7) / 8, xg = (W + 255) / 256, yg = (H + 255) / 256, num_groups = xg * yg;
   const uint32_t xlfg = (xb + 255) / 256, ylfg = (yb + 255) / 256, num_lf_groups = xlfg * ylfg;
+  const uint32_t cxb = (xb + 7) / 8, cyb = (yb + 7) / 8;
+  if (!hd.cfl_x.empty() && (hd.cfl_x.size() != size_t(cxb) * cyb || hd.cfl_b.size() != size_t(cxb) * cyb))
+    throw std::runtime_error("CfL maps take one value per 64x64 tile");
   BitWriter lf_global;
   lf_global.write(1, 1);                // LfQuantFactors default
   lf_global.u2s_sel(0, 1024 - 1, 11);   // global_scale 1024
@@ -1180,7 +1307,7 @@ std::vector<uint8_t> encode_vardct_tokens(const uint32_t* w, size_t len) {
     }
     write_context_map(lf_global, map, nc);
   }
-  lf_global.write(1, 1);  // default ColorCorrelationParams
+  write_color_correlation(lf_global, hd);
   lf_global.write(0, 1);  // no global tree
   // quantised LF integers, X / Y / B per block in raster order
   std::vector<int32_t> lfq[3];
@@ -1238,6 +1365,12 @@ std::vector<uint8_t> encode_vardct_tokens(const uint32_t* w, size_t len) {
     mc[0].h = mc[1].h = chh;
     mc[0].d.assign(size_t(cw) * chh, 0);
     mc[1].d.assign(size_t(cw) * chh, 0);
+    if (!hd.cfl_x.empty())
+      for (uint32_t y = 0; y < chh; y++)
+        for (uint32_t x = 0; x < cw; x++) {
+          mc[0].d[size_t(y) * cw + x] = hd.cfl_x[size_t(y0 / 8 + y) * cxb + x0 / 8 + x];
+          mc[1].d[size_t(y) * cw + x] = hd.cfl_b[size_t(y0 / 8 + y) * cxb + x0 / 8 + x];
+        }
     mc[2].w = count;
     mc[2].h = 2;
     mc[2].d = types;
@@ -1382,9 +1515,9 @@ std::vector<uint8_t> encode_vardct_tokens(const uint32_t* w, size_t len) {
   out.write(0, 3);  // explicit xsize
   write_dim(W);
   out.write(1, 1);  // ImageMetadata all_default
-  out.write(1, 1);  // CustomTransformData all_default
+  write_custom_transform_data(out, hd);
   out.zero_pad_to_byte();
-  // FrameHeader (frame_header.rs:267-444) with the default filters and qm scales
+  // FrameHeader (frame_header.rs:267-444) with the default filters (custom groups as the header words give) and qm scales
   out.write(0, 1);  // all_default
   out.write(0, 2);  // RegularFrame
   out.write(0, 1);  // VarDCT
@@ -1404,13 +1537,7 @@ std::vector<uint8_t> encode_vardct_tokens(const uint32_t* w, size_t len) {
   out.write(1, 1);  // is_last
   out.write(0, 2);  // name length 0
   out.write(0, 1);  // RestorationFilter all_default = 0
-  out.write(1, 1);  // gab
-  out.write(0, 1);  // gab_custom
-  out.write(2, 2);  // epf_iters
-  out.write(0, 1);  // epf_sharp_custom
-  out.write(0, 1);  // epf_weight_custom
-  out.write(0, 1);  // epf_sigma_custom
-  out.write_u64(0);  // restoration filter extensions
+  write_restoration_filter(out, 1, 2, hd);
   out.write_u64(0);  // frame header extensions
   std::vector<std::vector<uint8_t>> sections;
   if (num_groups == 1 && num_passes == 1) {  // single TOC entry: sections concatenated bitwise
@@ -1478,9 +1605,11 @@ int64_t jxs_encode_synthetic(uint32_t width, uint32_t height, uint64_t seed, flo
 //   mode 7:     additionally 3 * 64 * REQUIRED_SIZE_X * REQUIRED_SIZE_Y raw entries (int32, each channel in raster
 //               order, 8 * REQUIRED_SIZE_X wide), written as a Modular sub-bitstream after the fields.
 // dequant_len 0: all library tables (the same bitstream as jxs_encode_synthetic).
+// header: the restoration filter, colour correlation, opsin and CfL fields to write (header_len 0: defaults).
 int64_t jxs_encode_synthetic_ex(uint32_t width, uint32_t height, uint64_t seed, float distance, uint32_t epf_iters,
                                 uint32_t gab, uint32_t profile, uint32_t x_qm_scale, uint32_t b_qm_scale,
-                                const uint32_t* dequant, size_t dequant_len, uint8_t* out, size_t cap) {
+                                const uint32_t* dequant, size_t dequant_len, const uint32_t* header, size_t header_len,
+                                uint8_t* out, size_t cap) {
   try {
     jxs::Params p{width, height, seed, distance, epf_iters, gab, profile & 0xff, (profile >> 8) & 1, (profile >> 9) & 3,
                   ((profile >> 12) & 7) + 1, (profile >> 16) & 15};
@@ -1513,6 +1642,7 @@ int64_t jxs_encode_synthetic_ex(uint32_t width, uint32_t height, uint64_t seed, 
       }
       if (pos != dequant_len) throw std::runtime_error("dequant array too long");
     }
+    if (header_len) jxs::read_header_words(header, header_len, p.hdr);
     std::vector<uint8_t> b = jxs::encode(p);
     if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
     return int64_t(b.size());

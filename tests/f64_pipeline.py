@@ -273,9 +273,14 @@ def dequant_table(t, encodings=None):
 class Frame:
     """The fields of a JxgFrameDesc the float path reads, as numpy arrays (edited by the sensitivity tests).
     encodings: the 17 dequantisation encodings the frame was written with (None: library table), required when the
-    descriptor carries custom tables, so that stage A never takes its matrices from the code under test."""
+    descriptor carries custom tables, so that stage A never takes its matrices from the code under test.
+    header: the header fields the frame was written with (synth.encode_synthetic's dict; tests/f64_header.py). The
+    Gaborish, EPF, colour correlation and opsin parameters and the CfL maps are taken from what it decodes to, and the
+    descriptor must hold the same values (this pins the front end's parse). Without it the descriptor must hold the
+    defaults: a frame with other values is refused, for the same reason as with encodings."""
 
-    def __init__(self, d, encodings=None):
+    def __init__(self, d, encodings=None, header=None):
+        from tests import f64_header as fh
         self.width, self.height = int(d.width), int(d.height)
         self.xb, self.yb = (self.width + 7) // 8, (self.height + 7) // 8
         xb, yb = self.xb, self.yb
@@ -289,8 +294,6 @@ class Frame:
                 raise ValueError(f"custom tables {custom} in the frame, encodings given for {want}")
         self.encodings = encodings
         self.global_scale, self.x_qm_scale, self.b_qm_scale = int(d.global_scale), int(d.x_qm_scale), int(d.b_qm_scale)
-        self.quant_biases = np.array(list(d.quant_biases), np.float64)
-        self.base_x, self.base_b, self.color_factor = float(d.base_correlation_x), float(d.base_correlation_b), int(d.color_factor)
         self.lf = np.stack([_arr(d.lf[c], C.c_float, (yb, xb)) for c in range(3)]).astype(np.float64)
         self.transform_map = _arr(d.transform_map, C.c_uint8, (yb, xb))
         self.raw_quant = _arr(d.raw_quant_map, C.c_int32, (yb, xb))
@@ -299,21 +302,31 @@ class Frame:
         self.ytox = _arr(d.ytox_map, C.c_int8, (ty, tx)).astype(np.int32)
         self.ytob = _arr(d.ytob_map, C.c_int8, (ty, tx)).astype(np.int32)
         self.gab = int(d.gab)
-        self.gab_w1, self.gab_w2 = np.array(list(d.gab_w1), np.float64), np.array(list(d.gab_w2), np.float64)
         self.epf_iters = int(d.epf_iters)
-        self.epf_sharp_lut = np.array(list(d.epf_sharp_lut), np.float64)
-        self.epf_channel_scale = np.array(list(d.epf_channel_scale), np.float64)
-        self.epf_quant_mul = float(d.epf_quant_mul)
-        self.epf_pass0_sigma_scale, self.epf_pass2_sigma_scale = float(d.epf_pass0_sigma_scale), float(d.epf_pass2_sigma_scale)
-        self.epf_border_sad_mul = float(d.epf_border_sad_mul)
-        self.opsin_inverse_matrix = np.array(list(d.opsin_inverse_matrix), np.float64).reshape(3, 3)
-        self.opsin_biases = np.array(list(d.opsin_biases), np.float64)
         self.intensity_target = float(d.intensity_target)
         self.output_tf, self.orientation = int(d.output_tf), int(d.orientation)
         self.output_gamma = float(d.output_gamma)
         self.output_luminances = np.array(list(d.output_luminances), np.float64)
         self.output_format = int(d.output_format)
         self.dequant = {}
+        want = fh.decode(header, self.gab, self.epf_iters)
+        have = fh.descriptor_values(d)
+        bad = fh.differing(want, have)
+        if bad and header is None:
+            raise ValueError(f"the frame has non-default header fields {bad}: pass the header it was written with")
+        assert not bad, f"descriptor fields {bad} differ from the header written: {[(have[k], want[k]) for k in bad]}"
+        self.gab_w1, self.gab_w2 = want["gab_w1"], want["gab_w2"]
+        self.epf_sharp_lut, self.epf_channel_scale = want["epf_sharp_lut"], want["epf_channel_scale"]
+        self.epf_quant_mul, self.epf_border_sad_mul = want["epf_quant_mul"], want["epf_border_sad_mul"]
+        self.epf_pass0_sigma_scale, self.epf_pass2_sigma_scale = want["epf_pass0_sigma_scale"], want["epf_pass2_sigma_scale"]
+        self.color_factor, self.base_x, self.base_b = want["color_factor"], want["base_x"], want["base_b"]
+        self.opsin_inverse_matrix = np.array(list(d.opsin_inverse_matrix), np.float64).reshape(3, 3)  # output colour
+        self.written_opsin_matrix = want["opsin_inverse_matrix"].reshape(3, 3)
+        self.opsin_biases, self.quant_biases = want["opsin_biases"], want["quant_biases"]
+        maps = fh.cfl_maps(header, ty, tx)
+        if maps is not None:
+            assert np.array_equal(maps[0], self.ytox) and np.array_equal(maps[1], self.ytob), "CfL maps differ from those written"
+            self.ytox, self.ytob = maps
 
     def matrix(self, t):
         """(table, M) of transform type t; sensitivity tests may plant their own in self.dequant."""
@@ -379,7 +392,12 @@ def stage_a(fr, coeffs):
         x_cc = (fr.base_x + fr.ytox[ty, tx] / fr.color_factor)[:, None]  # color_correlation_map.rs:76-88
         b_cc = (fr.base_b + fr.ytob[ty, tx] / fr.color_factor)[:, None]
         deq = np.stack([x_cc * d[1] + d[0], d[1], b_cc * d[1] + d[2]])  # dequant_lane (group.rs:128-129)
-        mdeq = np.stack([np.abs(x_cc) * md[1] + md[0], md[1], np.abs(b_cc) * md[1] + md[2]])
+        # f32 x_cc = fl(base + fl(map / factor)) is off by up to 2^-24 (|map| / factor + |x_cc|): relative to the
+        # operands, not to |x_cc|, which a base can cancel (base -0.5, map 43, factor 84: |x_cc| = 0.012, operands
+        # 0.51). The |x_cc| part is inside K_A |x_cc| M_y; the operand part is added, twice, in units of K_A 2^-24.
+        ax_cc = np.abs(x_cc) + 2.0 / BOUND_K["A"] * (abs(fr.base_x) + np.abs(fr.ytox[ty, tx]) / fr.color_factor)[:, None]
+        ab_cc = np.abs(b_cc) + 2.0 / BOUND_K["A"] * (abs(fr.base_b) + np.abs(fr.ytob[ty, tx]) / fr.color_factor)[:, None]
+        mdeq = np.stack([ax_cc * md[1] + md[0], md[1], ab_cc * md[1] + md[2]])
         rows = bys[:, None, None] * 8 + np.arange(8 * cy)[None, :, None]
         cols = bxs[:, None, None] * 8 + np.arange(8 * cx)[None, None, :]
         lrows = bys[:, None, None] + np.arange(cy)[None, :, None]
@@ -402,7 +420,12 @@ def filter_input(planes, width, height):
 
 
 def gaborish_f64(img, w1, w2, mag=None):
-    """render/stages/gaborish.rs:20-28 (weights normalised to sum 1) on (3, h, w), mirrored edges."""
+    """render/stages/gaborish.rs:20-28 (weights normalised to sum 1) on (3, h, w), mirrored edges.
+    Magnitude: the stencil on magnitudes, times 1 + 2 (S / |T| - 1) / K_B with T = 1 + 4 w1 + 4 w2 and
+    S = 1 + 4 |w1| + 4 |w2|. The normalised weights w / T are rounded in f32 (gaborish.rs:20-27): fl(fl(1 + 4 w1) +
+    4 w2) is off by up to 2^-24 (|1 + 4 w1| + |T|) <= 2^-24 (S + |T|), so each weight is off by (S / |T| + 2) 2^-24
+    relative, and the output by that times the stencil on magnitudes. For weights >= 0, S = T and the 3 2^-24 is
+    inside K_B; a negative weight adds (S / |T| - 1) 2^-24 M, counted twice."""
     def run(x, absolute):
         p = np.pad(x, ((0, 0), (1, 1), (1, 1)), mode="symmetric")
         h, w = x.shape[1:]
@@ -411,7 +434,8 @@ def gaborish_f64(img, w1, w2, mag=None):
             tot = 1.0 + 4.0 * w1[c] + 4.0 * w2[c]
             k0, k1, k2 = 1.0 / tot, w1[c] / tot, w2[c] / tot
             if absolute:
-                k0, k1, k2 = abs(k0), abs(k1), abs(k2)
+                grow = 1.0 + 2.0 * ((1.0 + 4.0 * abs(w1[c]) + 4.0 * abs(w2[c])) / abs(tot) - 1.0) / BOUND_K["B"]
+                k0, k1, k2 = abs(k0) * grow, abs(k1) * grow, abs(k2) * grow
             s = lambda dx, dy: p[c, 1 + dy:1 + dy + h, 1 + dx:1 + dx + w]  # noqa: E731
             out[c] = (k0 * s(0, 0) + k1 * (s(0, -1) + s(0, 1) + s(-1, 0) + s(1, 0))
                       + k2 * (s(-1, -1) + s(1, -1) + s(-1, 1) + s(1, 1)))
@@ -430,11 +454,12 @@ def epf_border(ys, xs):
     return np.isin(ys % 8, (0, 7)) | np.isin(xs % 8, (0, 7))
 
 
-def epf_stage_f64(stage, img, inv_sigma, channel_scale, sigma_scale, border_sad_mul, mag=None):
+def epf_stage_f64(stage, img, inv_sigma, channel_scale, sigma_scale, border_sad_mul, mag=None, keep=None):
     """img: (3, h, w) float64. Whole-image mirroring at the edges (render/simple_pipeline/run_stage.rs:127-134 with
     util/mirror.rs:8 = numpy's 'symmetric' padding). With `mag`, also returns the magnitude of each output sample: the
     weighted magnitudes of the inputs, the rounding of the division, and the effect of a SAD error on each weight
-    (|inv_sigma * sad_mul| times the SAD computed on magnitudes, times |x_j - out|)."""
+    (|inv_sigma * sad_mul| times the SAD computed on magnitudes, times |x_j - out|). keep: per block, the blocks that
+    pass through (default: inv_sigma < MIN_SIGMA in float64)."""
     _, h, w = img.shape
     R = 3
     P = np.pad(img, ((0, 0), (R, R), (R, R)), mode="symmetric")
@@ -463,7 +488,7 @@ def epf_stage_f64(stage, img, inv_sigma, channel_scale, sigma_scale, border_sad_
     wts = [np.maximum(s * inv_s + 1.0, 0.0) for s in sads]
     wsum = 1.0 + sum(wts)
     out = (sh(0, 0) + sum(wt[None] * sh(ox, oy) for wt, (ox, oy) in zip(wts, offs))) / wsum[None]
-    keep = (sig < MIN_SIGMA)[None]  # sigma_mask: MIN_SIGMA > sigma passes through
+    keep = (sig < MIN_SIGMA if keep is None else keep[ys // 8, xs // 8])[None]  # MIN_SIGMA > sigma passes through
     out = np.where(keep, img, out)
     if mag is None:
         return out
@@ -478,6 +503,18 @@ def sigma_image_f64(global_scale, raw_quant, sharpness, quant_mul, sharp_lut):  
     return 1.0 / np.minimum(sigma_quant * np.asarray(sharp_lut, np.float64)[sharpness], -1e-4)
 
 
+def pass_through_f32(global_scale, raw_quant, sharpness, quant_mul, sharp_lut):
+    """The blocks EPF passes through: MIN_SIGMA > sigma, decided on the sigma the reference computes in f32, in its
+    operation order (features/epf.rs:53-75, lib.rs:28). It is a branch: a block whose f64 sigma lies within f32
+    rounding of MIN_SIGMA (custom LUTs and quant_mul can put one there) takes the f32 side, as every f32
+    implementation does. A LUT entry <= 0 gives sigma_quant * lut >= 0, clamped to -1e-4: 1 / sigma = -1e4."""
+    f = np.float32
+    quant_scale = f(1.0) / (f(65536.0) / f(global_scale))
+    sigma_quant = f(quant_mul) / (quant_scale * raw_quant.astype(f) * f(INV_SIGMA_NUM))
+    sigma = np.minimum(sigma_quant * np.asarray(sharp_lut, f)[sharpness], f(-1e-4))
+    return f(1.0) / sigma < f(MIN_SIGMA)
+
+
 def stage_b(fr, planes, mag=None):
     """planes: stage-A output [3][yb*8][xb*8]. Returns the filtered coded frame (3, h, w) and its magnitude."""
     x = filter_input(planes, fr.width, fr.height)
@@ -488,10 +525,11 @@ def stage_b(fr, planes, mag=None):
     if fr.epf_iters > 0:
         # the sigma of a varblock's first block covers the whole varblock: raw_quant_map holds it on every block
         sig = sigma_image_f64(fr.global_scale, fr.raw_quant, fr.epf_map, fr.epf_quant_mul, fr.epf_sharp_lut)
+        keep = pass_through_f32(fr.global_scale, fr.raw_quant, fr.epf_map, fr.epf_quant_mul, fr.epf_sharp_lut)
         stages = ([(0, fr.epf_pass0_sigma_scale)] if fr.epf_iters >= 3 else []) + [(1, 1.0)]
         stages += [(2, fr.epf_pass2_sigma_scale)] if fr.epf_iters >= 2 else []  # frame/render.rs: epf_iters
         for st, ss in stages:
-            x, m = epf_stage_f64(st, x, sig, fr.epf_channel_scale, ss, fr.epf_border_sad_mul, m)
+            x, m = epf_stage_f64(st, x, sig, fr.epf_channel_scale, ss, fr.epf_border_sad_mul, m, keep)
     return x[:, :h, :w], m[:, :h, :w]
 
 
@@ -743,6 +781,20 @@ def stage_c(fr, xyb, mag=None, full=False):
         rgb, mrgb, allow, amb = linear_to_hlg_f64(rgb, fr.intensity_target, fr.output_luminances, mrgb)
     out = (rgb.transpose(1, 2, 0), mrgb.transpose(1, 2, 0))
     return out + (allow.transpose(1, 2, 0), amb) if full else out
+
+
+SRGB_F32_LIMIT = float(np.finfo(np.float32).max) / 4 / float(SRGB_P[-1])
+
+
+def srgb_f32_overflow(fr, xyb):
+    """(h, w, 3) mask of the samples an f32 sRGB curve cannot compute: the rational polynomial of sqrt(a) (tf.rs:13-44,
+    degree 4, Horner) overflows f32 where a^2 p4 > FLT_MAX (here: above FLT_MAX / 4), giving +-inf or NaN while the
+    f64 ratio tends to 30.3. Only frames with XYB planes of 1e6 and more (coefficient-entry edges, shifted multi-pass
+    frames) reach linear values of 1e19; the mask is empty for every other frame and every other curve."""
+    if fr.output_tf != TF_SRGB:
+        return np.zeros((fr.height, fr.width, 3), bool)
+    lin = np.abs(linear_rgb_f64(fr, np.asarray(xyb, np.float64)))
+    return lin * lin > SRGB_F32_LIMIT
 
 
 def linear_rgb_f64(fr, xyb):

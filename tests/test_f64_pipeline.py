@@ -30,6 +30,12 @@ def _case_id(c):
     return f"{c[0]}x{c[1]}-epf{c[4]}-gab{c[5]}-p{c[6]}-colour{c[8]}"
 
 
+def _synthetic_h(case, header):
+    import synth
+    w, h, seed, dist, epf, gab, profile, entropy, colour = case
+    return synth.encode_synthetic(w, h, seed, dist, epf, gab, profile, entropy=entropy, colour=colour, header=header)
+
+
 def _read(name):
     import os
     return open(os.path.join(fp.ROOT, GOLDEN, name + ".jxl"), "rb").read()
@@ -41,26 +47,32 @@ def _synthetic(case):
     return synth.encode_synthetic(w, h, seed, dist, epf, gab, profile, entropy=entropy, colour=colour)
 
 
-def _frame(data, fmt=abi.FORMAT_RGB_F32):
+def _frame(data, fmt=abi.FORMAT_RGB_F32, header=None):
     import jxl_rs_b200 as j
     pf = j.ParsedFrame(data)
     d, *_ = pf.desc(fmt)
-    return fp.Frame(d)
+    return fp.Frame(d, header=header)
 
 
-def _check_file(data, what):
+def _fixture_header(name):
+    """The non-default header fields of a fixture (tests/f64_header.py holds them as f16 literals)."""
+    from tests import f64_header as fh
+    return fh.OPSIN_INVERSE_FIXTURE if name == "opsin_inverse" else None
+
+
+def _check_file(data, what, header=None):
     from tests import oracle_binding as ob
-    fr = _frame(data)
+    fr = _frame(data, header=header)
     out, taps = ob.decode_file(data, abi.FORMAT_RGB_F32, taps=True)
     a, ma = fp.stage_a(fr, taps["coeffs"])
     ratios = [fp.check("A", taps["xyb_idct"], a, ma, what)]
     b, mb = fp.stage_b(fr, taps["xyb_idct"].astype(np.float64))
     ratios.append(fp.check("B", taps["xyb_filtered"], b, mb, what))
-    ratios.append(_check_outputs(data, None, taps["xyb_filtered"], what, {abi.FORMAT_RGB_F32: out}))
+    ratios.append(_check_outputs(data, None, taps["xyb_filtered"], what, {abi.FORMAT_RGB_F32: out}, header))
     return ratios
 
 
-def _check_outputs(data, fr, xyb, what, have=None):
+def _check_outputs(data, fr, xyb, what, have=None, header=None):
     """fr: an edited frame descriptor used for every format, or None for the file's own (per format). Every output format of the oracle against stage C of its own filtered planes, in display orientation; the
     oracle is also allowed its fast_powf / fast_log2f error (3e-5 relative) for gamma and HLG. RGBA must equal the
     RGB_U8 output byte for byte, with alpha 255. Returns the largest err / (2^-24 M) of the f32 output."""
@@ -70,7 +82,7 @@ def _check_outputs(data, fr, xyb, what, have=None):
     for fmt in FORMATS:
         if fmt not in outs:
             outs[fmt], _ = ob.decode_file(data, fmt)
-        ff = _frame(data, fmt) if fr is None else fr  # the output curve can depend on the format (float: linear)
+        ff = _frame(data, fmt, header) if fr is None else fr  # the output curve can depend on the format (float: linear)
         key = (ff.output_tf, ff.output_gamma, ff.intensity_target)
         if key not in refs:
             refs[key] = fp.stage_c(ff, xyb.astype(np.float64), full=True)
@@ -88,7 +100,7 @@ def test_synthetic_frames_match_f64(case):
 
 @pytest.mark.parametrize("name", FIXTURES)
 def test_fixtures_match_f64(name):
-    _check_file(_read(name), name)
+    _check_file(_read(name), name, _fixture_header(name))
 
 
 def test_afv_basis_is_orthonormal():
@@ -185,24 +197,15 @@ def test_fault_mirroring_at_padded_edge(monkeypatch):
 
 
 def test_fault_gaborish_weights_of_x_and_b_swapped():
-    """Every available frame carries the default Gaborish weights, equal in all channels, so the frame is decoded by the
-    oracle with distinct X / Y / B weights written into its descriptor; swapping X and B on the f64 side must fail.
-    Old abs-or-rel 1e-3 bar on the same planes: caught (largest difference 1.1e-2)."""
-    import jxl_rs_b200 as j
+    """A frame written with distinct X / Y / B Gaborish weights (EPF off) is decoded by the oracle; swapping X and B
+    on the f64 side must fail. Old abs-or-rel 1e-3 bar on the same planes: caught (largest difference 1.1e-2)."""
     from tests import oracle_binding as ob
-    data = _synthetic((129, 97, 7, 1.0, 0, 1, 1, 0, 0))
-    pf = j.ParsedFrame(data)
-    d, hf, off, ln, n = pf.desc(abi.FORMAT_XYB_F32_PLANAR)
-    d.gab, d.epf_iters = 1, 0
-    for c, (w1, w2) in enumerate([(0.09, 0.05), (0.115169525, 0.061248592), (0.14, 0.075)]):
-        d.gab_w1[c], d.gab_w2[c] = w1, w2
-    fr = fp.Frame(d)
-    ps, pr = fr.xb * 8, fr.yb * 8
-    taps = {"coeffs": np.zeros((pf.info.num_groups, 3, 65536), np.int32), "xyb_idct": np.zeros((3, pr, ps), np.float32),
-            "xyb_filtered": np.zeros((3, fr.height, fr.width), np.float32)}
-    t = ob.JxoTaps(taps["coeffs"].ctypes.data, taps["xyb_idct"].ctypes.data, taps["xyb_filtered"].ctypes.data)
-    bad = C.c_uint32()
-    assert ob.load().jxo_decode_frame(C.byref(d), hf, off, ln, n, None, 0, C.byref(t), 1, C.byref(bad)) == 0
+    ws = [0.09, 0.05, 0.115169525, 0.061248592, 0.14, 0.075]
+    header = {"gab": [int(np.array(np.float16(w)).view(np.uint16)) for w in ws]}
+    data = _synthetic_h((129, 97, 7, 1.0, 0, 1, 1, 0, 0), header)
+    fr = _frame(data, header=header)
+    assert len(set(fr.gab_w1)) == 3 and len(set(fr.gab_w2)) == 3
+    _, taps = ob.decode_file(data, abi.FORMAT_RGB_F32, taps=True)
     b, mb = fp.stage_b(fr, taps["xyb_idct"].astype(np.float64))
     fp.check("B", taps["xyb_filtered"], b, mb)  # the distinct weights themselves are followed
     fr.gab_w1, fr.gab_w2 = fr.gab_w1[[2, 1, 0]], fr.gab_w2[[2, 1, 0]]
