@@ -161,6 +161,17 @@ int jxg_device_streams(int device, void** entropy_stream, void** post_stream);
 int jxg_init(int device, void** ctx);
 void jxg_shutdown(void* ctx);
 
+/* Test hook, off by default: with `byte` in 0..255, every later jxg_batch_run / jxg_modular_batch_run of the context
+ * first writes `byte` over the whole capacity of each of the context's device pools (the intermediates of both engines
+ * and the device copy of the staging blob, whose tail past the uploaded bytes keeps the pattern), on the stream that
+ * carries the upload, and jxg_batch_begin / jxg_modular_batch_begin write it over the pinned staging arena on the host;
+ * jxg_batch_rerun_device / jxg_modular_batch_rerun_device fill every pool but the staging blob, which the rerun reuses.
+ * Output bytes must not depend on the byte: a kernel that reads device memory its batch did not write shows up as a
+ * difference. Constant tables of the context, caller-owned outputs and the status readback buffer are not touched.
+ * byte = -1 turns the hook off. Each begin, run and rerun uses the byte in force when it is called. JXG_ERR_ARGUMENT for a
+ * NULL context or a byte outside -1..255. */
+int jxg_context_set_pool_fill(void* ctx, int byte);
+
 /* Batch of frames decoded together (one kernel pipeline over all groups of
  * all frames). Replaces N calls of decode_and_render_hf_groups. */
 int jxg_batch_begin(void* ctx, uint32_t n_frames_hint, void** batch);

@@ -66,7 +66,7 @@ class JxgImageInfo(C.Structure):
 
 # every symbol include/jxg.h declares (tests check the .so exports all of them)
 EXPORTS = [
-    "jxg_init", "jxg_shutdown", "jxg_batch_begin", "jxg_batch_add_frame", "jxg_batch_run", "jxg_batch_wait",
+    "jxg_init", "jxg_shutdown", "jxg_context_set_pool_fill", "jxg_batch_begin", "jxg_batch_add_frame", "jxg_batch_run", "jxg_batch_wait",
     "jxg_batch_rerun_device", "jxg_batch_end", "jxg_batch_read_coeffs", "jxg_batch_read_xyb",
     "jxg_batch_set_debug_stop", "jxg_batch_set_profile", "jxg_batch_stage_times", "jxg_batch_stage_marks", "jxg_batch_stats",
     "jxg_batch_entropy_stats", "jxg_parse_file", "jxg_parse_file_mt", "jxg_parsed_free", "jxg_parsed_desc",
@@ -102,6 +102,7 @@ def load_library():
     lib.jxg_device_streams.argtypes = [C.c_int, C.POINTER(vp), C.POINTER(vp)]
     lib.jxg_shutdown.argtypes = [vp]
     lib.jxg_shutdown.restype = None
+    lib.jxg_context_set_pool_fill.argtypes = [vp, C.c_int]
     lib.jxg_batch_begin.argtypes = [vp, C.c_uint32, C.POINTER(vp)]
     lib.jxg_batch_add_frame.argtypes = [vp, C.POINTER(JxgFrameDesc), vp, vp, vp, C.c_uint32, vp, C.c_size_t, C.c_int]
     lib.jxg_batch_run.argtypes = [vp, vp]

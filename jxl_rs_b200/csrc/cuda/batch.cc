@@ -256,6 +256,13 @@ void jxg_shutdown(void* c) {
   delete ctx;
 }
 
+int jxg_context_set_pool_fill(void* c, int byte) {
+  Context* cx = static_cast<Context*>(c);
+  if (!cx || byte < -1 || byte > 255) return set_error(JXG_ERR_ARGUMENT, "pool fill: a context and a byte in -1..255");
+  cx->pool_fill = byte;
+  return JXG_OK;
+}
+
 int jxg_batch_begin(void* c, uint32_t n_frames_hint, void** out_batch) {
   if (!c || !out_batch) return JXG_ERR_ARGUMENT;
   Context* cx = static_cast<Context*>(c);
@@ -761,6 +768,7 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
   trace.mark("alloc");
   b->blob.flush();
   trace.mark("flush");
+  if (int r = fill_pools(b->ctx, use_pair ? b->ctx->stream : se, true)) return r;
   if (use_pair) {
     // the upload rides on the context's own stream so that it overlaps the entropy kernel of the batch before;
     // the entropy stream picks it up through the hand-off event (free again once launch() re-records it)
@@ -804,6 +812,7 @@ int jxg_batch_rerun_device(void* bp, void* cuda_stream) {
   cudaStream_t s = cuda_stream ? se : (use_pair ? ds.post : b->ctx->stream);
   b->last_stream = s;
   CUDA_TRY(cudaStreamWaitEvent(se, b->ev1, 0));  // the previous run of this batch still owns its device buffers
+  if (int r = fill_pools(b->ctx, se, false)) return r;
   CUDA_TRY(cudaEventRecord(b->ev0, se));
   if (int r = launch(b, se, s, false)) return r;
   CUDA_TRY(cudaMemcpyAsync(b->status_host, b->d_status.p, b->status_n * 4, cudaMemcpyDeviceToHost, s));

@@ -49,6 +49,7 @@ struct DevBuf {
 struct PinnedArena {
   uint8_t* p = nullptr;
   size_t size = 0, cap = 0;
+  int fill = -1;  // the context's pool fill byte for this batch (jxg_context_set_pool_fill), -1: off
   ~PinnedArena() {
     if (p) cudaFreeHost(p);
   }
@@ -62,6 +63,7 @@ struct PinnedArena {
       memcpy(np, p, size);
       cudaFreeHost(p);
     }
+    if (fill >= 0) memset(np + size, fill, ncap - size);
     p = np;
     cap = ncap;
     return true;
@@ -138,6 +140,7 @@ struct Context {
   PinnedArena blob;
   DevBuf d_blob, d_coeffs, d_block_off, d_planes_a, d_status, d_out, d_desc, d_nblk, d_orient, d_lzwin,
       d_modular_lzwin, d_modular_wp;
+  int pool_fill = -1;  // test hook (jxg_context_set_pool_fill): byte written over the pools before each run, -1: off
   bool batch_live = false;
   // pinned status readback buffer, owned by the context: cudaHostAlloc / cudaFreeHost synchronise the whole
   // device, so they must not happen per batch when batches of several contexts are in flight
@@ -164,6 +167,8 @@ inline int batch_begin(BatchCore& b, Context* cx, cudaEvent_t* extra, unsigned e
   cx->blob.size = 0;
   cx->blob.pending.clear();
   cx->blob.deferred_threads = 0;
+  cx->blob.fill = cx->pool_fill;
+  if (cx->pool_fill >= 0 && cx->blob.p) memset(cx->blob.p, cx->pool_fill, cx->blob.cap);
   cudaError_t e = cudaEventCreate(&b.ev0);
   if (e == cudaSuccess) e = cudaEventCreate(&b.ev1);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(extra, extra_flags);
@@ -220,6 +225,17 @@ bool batch_table(PinnedArena& blob, const std::vector<T>& v, uint64_t& off) {
   const int64_t o = blob.append(v.empty() ? nullptr : v.data(), v.size() * sizeof(T), 16, 16);
   off = uint64_t(o);
   return o >= 0;
+}
+
+// Test hook (jxg_context_set_pool_fill): writes the fill byte over the whole capacity of every pool of the context, on
+// the stream of the upload, so that a kernel reading a word its batch did not write sees the pattern, not what an
+// earlier batch left there. A run fills d_blob as well (the upload then overwrites its own part); a rerun keeps it.
+inline int fill_pools(Context* cx, cudaStream_t s, bool with_blob) {
+  if (cx->pool_fill < 0) return 0;
+  for (DevBuf* d : {&cx->d_blob, &cx->d_coeffs, &cx->d_block_off, &cx->d_planes_a, &cx->d_status, &cx->d_out, &cx->d_desc,
+                    &cx->d_nblk, &cx->d_orient, &cx->d_lzwin, &cx->d_modular_lzwin, &cx->d_modular_wp})
+    if (d->p && (with_blob || d != &cx->d_blob)) CUDA_TRY(cudaMemsetAsync(d->p, cx->pool_fill, d->cap, s));
+  return 0;
 }
 
 // Read taps copy device buffers of the last run, which may have run on a caller's stream: they wait for its ev1.

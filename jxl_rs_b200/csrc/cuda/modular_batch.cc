@@ -619,6 +619,7 @@ int jxg_modular_batch_run(void* bp, void* cuda_stream) {
       !batch_table(blob, b->refs, b->tab.refs) || !batch_table(blob, all_jobs, b->tab.jobs))
     return set_error(JXG_ERR_CUDA, "pinned staging allocation failed");
   if (int r = cx->d_blob.ensure(blob.size + 64)) return r;
+  if (int r = fill_pools(cx, s, true)) return r;
   CUDA_TRY(cudaEventRecord(b->ev0, s));
   CUDA_TRY(cudaMemcpyAsync(cx->d_blob.p, blob.p, blob.size, cudaMemcpyHostToDevice, s));
   b->h2d += blob.size;
@@ -635,6 +636,7 @@ int jxg_modular_batch_rerun_device(void* bp, void* cuda_stream) {
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : b->ctx->stream;
   b->last_stream = s;
   CUDA_TRY(cudaStreamWaitEvent(s, b->ev1, 0));  // the previous run of this batch still owns its device buffers
+  if (int r = fill_pools(b->ctx, s, false)) return r;
   CUDA_TRY(cudaEventRecord(b->ev0, s));
   if (int r = launch_all(b, s, false)) return r;
   CUDA_TRY(cudaEventRecord(b->ev1, s));

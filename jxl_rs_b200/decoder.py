@@ -73,6 +73,12 @@ class JxgContext:
         abi.check(self._lib, self._lib.jxg_init(device, C.byref(self._h)))
         self.device = device
 
+    def set_pool_fill(self, byte: int):
+        """Test hook (jxg_context_set_pool_fill): with `byte` in 0..255 every later batch run writes it over the
+        context's device pools and staging arena first, so that outputs cannot depend on what earlier batches left
+        there; -1 (the default) turns it off. Each begin, run and rerun uses the byte in force when it is called."""
+        abi.check(self._lib, self._lib.jxg_context_set_pool_fill(self._h, int(byte)))
+
     def close(self):
         if self._h.value:
             self._lib.jxg_shutdown(self._h)

@@ -163,12 +163,28 @@ def test_c_abi_rejects_inconsistent_descriptors():
     ctx.close()
 
 
+def overlapping_varblocks(d, w, h):
+    """Mutates descriptor `d` of a w x h frame: a DCT32X32 varblock starts at every block whose 4x4 cover fits its group
+    and the frame. Returns the replacement buffers, which must stay alive while `d` is used."""
+    import ctypes as C
+    xb, yb = (w + 7) // 8, (h + 7) // 8
+    tmap = (C.c_uint8 * (xb * yb))()
+    for by in range(yb):
+        for bx in range(xb):
+            if (bx & 31) + 4 <= 32 and (by & 31) + 4 <= 32 and bx + 4 <= xb and by + 4 <= yb:
+                tmap[by * xb + bx] = 128 | 5  # DCT32X32: 4x4 blocks
+    rq = (C.c_int32 * (xb * yb)).from_buffer_copy(C.string_at(d.raw_quant_map, 4 * xb * yb))
+    for i in range(xb * yb):
+        rq[i] = max(rq[i], 1)  # every varblock start needs raw_quant >= 1
+    d.transform_map, d.raw_quant_map = C.cast(tmap, C.c_void_p), C.cast(rq, C.c_void_p)
+    return tmap, rq
+
+
 def test_overlapping_varblocks_fail_on_every_entropy_route():
     """The descriptor checks do not look for overlapping varblocks. A transform map with a 32x32 varblock starting at
     every block whose cover fits its group and the frame passes them, overflows every group's coefficient area, and
     each entropy kernel (ANS single pass: lean, prefix: fast, LZ77: slow) reports JXG_ERR_INVALID_TRANSFORM from the
     block plan. The unmutated twin of each frame decodes."""
-    import ctypes as C
     import torch
     import jxl_rs_b200 as j
     import synth
@@ -177,24 +193,11 @@ def test_overlapping_varblocks_fail_on_every_entropy_route():
     groups = ((xb + 31) // 32) * ((yb + 31) // 32)
     ctx = j.JxgContext(0)
     out = torch.empty((h, w, 3), dtype=torch.uint8, device="cuda:0")
-
-    def overlapping(d):
-        tmap = (C.c_uint8 * (xb * yb))()
-        for by in range(yb):
-            for bx in range(xb):
-                if (bx & 31) + 4 <= 32 and (by & 31) + 4 <= 32 and bx + 4 <= xb and by + 4 <= yb:
-                    tmap[by * xb + bx] = 128 | 5  # DCT32X32: 4x4 blocks
-        rq = (C.c_int32 * (xb * yb)).from_buffer_copy(C.string_at(d.raw_quant_map, 4 * xb * yb))
-        for i in range(xb * yb):
-            rq[i] = max(rq[i], 1)  # every varblock start needs raw_quant >= 1
-        d.transform_map, d.raw_quant_map = C.cast(tmap, C.c_void_p), C.cast(rq, C.c_void_p)
-        return tmap, rq
-
     for entropy, route in ((0, "lean"), (1, "fast"), (2, "slow")):
         fr = j.ParsedFrame(synth.encode_synthetic(w, h, 9, 0.5, 2, 1, 1, entropy=entropy))
-        for mutate in (None, overlapping):
+        for mutate in (None, overlapping_varblocks):
             d, hf, off, ln, n = fr.desc(abi.FORMAT_RGB_U8)
-            keep = mutate(d) if mutate else None  # noqa: F841 - keeps replacement buffers alive
+            keep = mutate(d, w, h) if mutate else None  # noqa: F841 - keeps replacement buffers alive
             b = j.Batch(ctx, 1)
             try:
                 b.add_desc(d, hf, off, ln, n, out.data_ptr(), w * 3, True)
