@@ -152,11 +152,6 @@ typedef struct JxgFrameDesc {
  * threads and pinned allocations to the GPU's NUMA node before jxg_init. buf: >= 16 bytes. */
 int jxg_device_pci_bus_id(int device, char* buf, int len);
 
-/* The device's two optional stage streams (JXG_STAGE_STREAMS=1: block plan + entropy decode of every batch on the first,
- * transforms + filters + stores on the second). Off by default - every batch runs on its context's own stream, which
- * measured faster (DESIGN.md section 3); returned so that a host that turns them on can record events on them. */
-int jxg_device_streams(int device, void** entropy_stream, void** post_stream);
-
 /* Context: one per device/rank. Owns streams, pinned staging and device pools. */
 int jxg_init(int device, void** ctx);
 void jxg_shutdown(void* ctx);

@@ -5,5 +5,5 @@ front-end) and the host-side mirror of the reference's decoder interface.
 """
 from .abi import JxgError, library_path, load_library  # noqa: F401
 from .decoder import (Batch, JxgContext, JxlPixelFormat, ModularBatch, ModularParsedFrame, ParsedFrame,  # noqa: F401
-                      PipelinedDecoder, bind_to_gpu_numa_node, decode_files, device_streams, decode_modular_files, effective_cpus,
+                      PipelinedDecoder, bind_to_gpu_numa_node, decode_files, decode_modular_files, effective_cpus,
                       gpu_numa_cpus)

@@ -27,20 +27,17 @@ namespace detail {
 thread_local std::string g_error;
 std::atomic<int> g_live_contexts[64];  // per device: contexts between jxg_init and jxg_shutdown
 
-DeviceStreams device_streams(int device) {
+cudaStream_t device_d2h_stream(int device) {
   static std::mutex mu;
-  static DeviceStreams table[64];
+  static cudaStream_t table[64];
   std::lock_guard<std::mutex> lk(mu);
-  if (device < 0 || device >= 64) return DeviceStreams{};
-  DeviceStreams& d = table[device];
-  if (!d.entropy) {
+  if (device < 0 || device >= 64) return nullptr;
+  cudaStream_t& s = table[device];
+  if (!s) {
     cudaSetDevice(device);
-    if (cudaStreamCreateWithFlags(&d.entropy, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&d.post, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&d.d2h, cudaStreamNonBlocking) != cudaSuccess)
-      d = DeviceStreams{};
+    if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) s = nullptr;
   }
-  return d;
+  return s;
 }
 }
 }  // namespace jxgpu
@@ -87,7 +84,6 @@ struct Batch : BatchCore {
     uint64_t frames = 0, sections = 0, streams = 0, lean_cta = 0, lean_warp = 0, streams_lean = 0, streams_fast = 0, streams_slow = 0,
              ftiles = 0;
   } tab;
-  cudaEvent_t ev_handoff = nullptr;
   bool profile = false;
   cudaEvent_t stage_ev[kNumStages + 1] = {nullptr};
   float last_ms = 0;
@@ -180,15 +176,6 @@ int jxg_device_pci_bus_id(int device, char* buf, int len) {
   return JXG_OK;
 }
 
-// The device's stage streams (see DeviceStreams), for hosts that want to bracket batches with their own events.
-int jxg_device_streams(int device, void** entropy_stream, void** post_stream) {
-  const DeviceStreams ds = device_streams(device);
-  if (!ds.entropy) return set_error(JXG_ERR_CUDA, "cannot create the device's stage streams");
-  if (entropy_stream) *entropy_stream = ds.entropy;
-  if (post_stream) *post_stream = ds.post;
-  return JXG_OK;
-}
-
 int jxg_init(int device, void** out_ctx) {
   if (!out_ctx) return JXG_ERR_ARGUMENT;
   int n = 0;
@@ -196,11 +183,11 @@ int jxg_init(int device, void** out_ctx) {
     return set_error(JXG_ERR_NO_DEVICE, "no CUDA device: libjxgpu has no CPU fallback");
   if (device < 0 || device >= n) return set_error(JXG_ERR_ARGUMENT, "bad device index");
   CUDA_TRY(cudaSetDevice(device));
-  const DeviceStreams ds = device_streams(device);
-  if (!ds.d2h) return set_error(JXG_ERR_CUDA, "cannot create the device's stage and D2H streams");
+  cudaStream_t d2h = device_d2h_stream(device);
+  if (!d2h) return set_error(JXG_ERR_CUDA, "cannot create the device's D2H stream");
   auto ctx = std::make_unique<Context>();
   ctx->device = device;
-  ctx->d2h = ds.d2h;
+  ctx->d2h = d2h;
   CUDA_TRY(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
   for (auto& e : ctx->range_done) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming | cudaEventBlockingSync));
   CUDA_TRY(cudaEventCreateWithFlags(&ctx->copy_done, cudaEventDisableTiming | cudaEventBlockingSync));
@@ -267,7 +254,7 @@ int jxg_batch_begin(void* c, uint32_t n_frames_hint, void** out_batch) {
   if (!c || !out_batch) return JXG_ERR_ARGUMENT;
   Context* cx = static_cast<Context*>(c);
   auto b = std::make_unique<Batch>(cx);
-  if (int r = batch_begin(*b, cx, &b->ev_handoff, cudaEventDisableTiming)) return r;
+  if (int r = batch_begin(*b, cx)) return r;
   b->frames.reserve(n_frames_hint);
   *out_batch = b.release();
   return JXG_OK;
@@ -277,7 +264,6 @@ void jxg_batch_end(void* bp) {
   Batch* b = static_cast<Batch*>(bp);
   if (!b) return;
   batch_end(*b);
-  cudaEventDestroy(b->ev_handoff);
   for (auto& e : b->stage_ev)
     if (e) cudaEventDestroy(e);
   delete b;
@@ -636,7 +622,6 @@ static BatchDev make_batch_dev(Batch* b) {
   B.streams_slow = reinterpret_cast<const StreamDev*>(tab(b->tab.streams_slow));
   B.num_fast = uint32_t(b->streams_fast.size());
   B.num_slow = uint32_t(b->streams_slow.size());
-  B.reg_idct32 = (getenv("JXG_REG_IDCT32") && atoi(getenv("JXG_REG_IDCT32"))) ? 1u : 0u;
   B.nzlist = static_cast<uint32_t*>(b->d_coeffs.p);  // the pool that held the dense coefficients now holds the lists
   B.block_off = static_cast<uint32_t*>(b->d_block_off.p);
   B.lzwin = static_cast<uint32_t*>(b->ctx->d_lzwin.p);
@@ -654,17 +639,10 @@ static BatchDev make_batch_dev(Batch* b) {
   return B;
 }
 
-// se: stream of the upload, block plan and entropy kernels; s: stream of everything after them (== se when the caller
-// brought its own stream).
-static int launch(Batch* b, cudaStream_t se, cudaStream_t s, bool copy_to_host) {
+static int launch(Batch* b, cudaStream_t s, bool copy_to_host) {
   const BatchDev B = make_batch_dev(b);
   cudaEvent_t* ev = b->profile ? b->stage_ev : nullptr;
-  b->launches = uint64_t(launch_pipeline(B, se, b->debug_stop, ev, b->lean_all_420, b->lean_S, b->lean_ctas, b->lean_ctx_smem,
-                                         s, b->ev_handoff));
-  if (b->debug_stop == 1 && s != se) {  // stopped after the entropy stage: the post stream still has to cover it
-    cudaEventRecord(b->ev_handoff, se);
-    cudaStreamWaitEvent(s, b->ev_handoff, 0);
-  }
+  b->launches = uint64_t(launch_pipeline(B, s, b->debug_stop, ev, b->lean_all_420, b->lean_S, b->lean_ctas, b->lean_ctx_smem));
   if (b->debug_stop == 0) {
     // Fused filter + colour + store, launched per range of frames; each finished range is copied to the host on the
     // device's D2H stream while the next range is being filtered.
@@ -732,13 +710,7 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
   if (!b || b->frames.empty()) return JXG_ERR_ARGUMENT;
   RunTrace trace;
   CUDA_TRY(cudaSetDevice(b->ctx->device));
-  // the caller's stream for everything, or the device's stage streams (see DeviceStreams)
-  const DeviceStreams ds = device_streams(b->ctx->device);
-  static const bool staged = getenv("JXG_STAGE_STREAMS") && atoi(getenv("JXG_STAGE_STREAMS")) != 0;
-  const bool use_pair = !cuda_stream && staged && ds.entropy;
-  cudaStream_t se = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : (use_pair ? ds.entropy : b->ctx->stream);
-  cudaStream_t s = cuda_stream ? se : (use_pair ? ds.post : b->ctx->stream);
-  b->last_stream = s;
+  cudaStream_t s = batch_stream(*b, cuda_stream);
   b->h2d = b->d2h = 0;
   schedule_lean(b);
   // device allocations
@@ -768,27 +740,18 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
   trace.mark("alloc");
   b->blob.flush();
   trace.mark("flush");
-  if (int r = fill_pools(b->ctx, use_pair ? b->ctx->stream : se, true)) return r;
-  if (use_pair) {
-    // the upload rides on the context's own stream so that it overlaps the entropy kernel of the batch before;
-    // the entropy stream picks it up through the hand-off event (free again once launch() re-records it)
-    CUDA_TRY(cudaEventRecord(b->ev0, b->ctx->stream));
-    CUDA_TRY(cudaMemcpyAsync(b->d_blob.p, b->blob.p, b->blob.size, cudaMemcpyHostToDevice, b->ctx->stream));
-    CUDA_TRY(cudaEventRecord(b->ev_handoff, b->ctx->stream));
-    CUDA_TRY(cudaStreamWaitEvent(se, b->ev_handoff, 0));
-  } else {
-    CUDA_TRY(cudaEventRecord(b->ev0, se));
-    CUDA_TRY(cudaMemcpyAsync(b->d_blob.p, b->blob.p, b->blob.size, cudaMemcpyHostToDevice, se));
-  }
+  if (int r = fill_pools(b->ctx, s, true)) return r;
+  CUDA_TRY(cudaEventRecord(b->ev0, s));
+  CUDA_TRY(cudaMemcpyAsync(b->d_blob.p, b->blob.p, b->blob.size, cudaMemcpyHostToDevice, s));
   trace.mark("blob_h2d");
   b->h2d += b->blob.size;
   b->uploaded = true;
   trace.mark("uploads");
-  if (int r = launch(b, se, s, true)) return r;
+  if (int r = launch(b, s, true)) return r;
   trace.mark("launch");
   CUDA_TRY(cudaMemcpyAsync(b->status_host, b->d_status.p, b->status_n * 4, cudaMemcpyDeviceToHost, s));
-  // ev1 = everything of this batch done. The D2H stream joins the post stream and carries ev1 when it holds the output
-  // copies (no debug stop): the post stream itself must not wait for them (the next batch's transforms follow on it).
+  // ev1 = everything of this batch done. The D2H stream joins the batch's stream and carries ev1 when it holds the output
+  // copies (no debug stop): the batch's stream itself must not wait for them (later work on it does not need the copies).
   if (b->debug_stop == 0) {
     Context* cx = b->ctx;
     CUDA_TRY(cudaEventRecord(cx->copy_done, s));
@@ -805,16 +768,11 @@ int jxg_batch_rerun_device(void* bp, void* cuda_stream) {
   Batch* b = static_cast<Batch*>(bp);
   if (!b || !b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch was never submitted");
   CUDA_TRY(cudaSetDevice(b->ctx->device));
-  const DeviceStreams ds = device_streams(b->ctx->device);
-  static const bool staged = getenv("JXG_STAGE_STREAMS") && atoi(getenv("JXG_STAGE_STREAMS")) != 0;
-  const bool use_pair = !cuda_stream && staged && ds.entropy;
-  cudaStream_t se = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : (use_pair ? ds.entropy : b->ctx->stream);
-  cudaStream_t s = cuda_stream ? se : (use_pair ? ds.post : b->ctx->stream);
-  b->last_stream = s;
-  CUDA_TRY(cudaStreamWaitEvent(se, b->ev1, 0));  // the previous run of this batch still owns its device buffers
-  if (int r = fill_pools(b->ctx, se, false)) return r;
-  CUDA_TRY(cudaEventRecord(b->ev0, se));
-  if (int r = launch(b, se, s, false)) return r;
+  cudaStream_t s = batch_stream(*b, cuda_stream);
+  CUDA_TRY(cudaStreamWaitEvent(s, b->ev1, 0));  // the previous run of this batch still owns its device buffers
+  if (int r = fill_pools(b->ctx, s, false)) return r;
+  CUDA_TRY(cudaEventRecord(b->ev0, s));
+  if (int r = launch(b, s, false)) return r;
   CUDA_TRY(cudaMemcpyAsync(b->status_host, b->d_status.p, b->status_n * 4, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaEventRecord(b->ev1, s));
   return JXG_OK;
@@ -829,7 +787,7 @@ int jxg_batch_wait(void* bp, uint32_t* first_bad_frame, uint32_t* first_bad_grou
     const auto t0 = std::chrono::steady_clock::now();
     const bool was_done = traced && cudaEventQuery(b->ev1) == cudaSuccess;
     CUDA_TRY(cudaEventSynchronize(b->ev1));  // recorded behind the status words and the D2H copies; no stream-wide wait:
-                                             // the stage streams carry later batches too
+                                             // a caller's stream may carry later work too
     if (traced)
       fprintf(stderr, "[jxg_batch_wait] done on entry %d, event wait %.1f ms\n", int(was_done),
               std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());

@@ -110,25 +110,17 @@ struct PinnedArena {
   }
 };
 
-// Optional (JXG_STAGE_STREAMS=1): two streams per DEVICE shared by all its contexts — every batch runs its block plan and
-// entropy kernels on the entropy stream and its transforms, filters and stores on the post stream, so that at most one
-// kernel of each kind runs at a time. It was slower than one stream per batch on a 64-frame 4K step: the entropy kernel
-// parks ~30 K of an SM's 64 K registers for its whole duration, so the transforms / filters beside it run at one CTA per SM, and nothing is gained over letting
-// batches overlap in the entropy kernel's tail. The default is one stream per batch.
-struct DeviceStreams {
-  cudaStream_t entropy = nullptr, post = nullptr;
-  // One D2H stream for all contexts of the device: output copies leave in launch order. With a copy stream per context
-  // the copies of all batches in flight share the host link evenly, so they all end together, all contexts come free
-  // together and the next batches start together: a convoy that leaves the SMs idle for the length of the D2H tail.
-  // First in, first out retires the oldest batch early and keeps the launches staggered.
-  cudaStream_t d2h = nullptr;
-};
-DeviceStreams device_streams(int device);  // created on first use
+// One D2H stream per DEVICE, shared by all its contexts: output copies leave in launch order. With a copy stream per
+// context the copies of all batches in flight share the host link evenly, so they all end together, all contexts come
+// free together and the next batches start together: a convoy that leaves the SMs idle for the length of the D2H tail.
+// First in, first out retires the oldest batch early and keeps the launches staggered. Created on first use; nullptr
+// when that fails.
+cudaStream_t device_d2h_stream(int device);
 
 struct Context {
   int device = 0;
   cudaStream_t stream = nullptr;
-  // Output copies of a batch leave on the device's D2H stream (DeviceStreams::d2h) in up to kMaxRanges frame ranges: the
+  // Output copies of a batch leave on the device's D2H stream (device_d2h_stream) in up to kMaxRanges frame ranges: the
   // copy of a finished range overlaps the filtering of the later ones.
   cudaStream_t d2h = nullptr;
   static constexpr int kMaxRanges = 8;
@@ -159,8 +151,9 @@ struct BatchCore {
   uint64_t launches = 0, h2d = 0, d2h = 0;
 };
 
-// One live batch per context. Creates ev0, ev1 and the engine's own event `extra`; on failure the context stays free.
-inline int batch_begin(BatchCore& b, Context* cx, cudaEvent_t* extra, unsigned extra_flags) {
+// One live batch per context. Creates ev0, ev1 and, if `extra` is given, the engine's own timing event; on failure the
+// context stays free.
+inline int batch_begin(BatchCore& b, Context* cx, cudaEvent_t* extra = nullptr) {
   if (cx->batch_live) return set_error(JXG_ERR_ARGUMENT, "one live batch per context: end the previous batch first");
   CUDA_TRY(cudaSetDevice(cx->device));
   b.ctx = cx;
@@ -171,14 +164,20 @@ inline int batch_begin(BatchCore& b, Context* cx, cudaEvent_t* extra, unsigned e
   if (cx->pool_fill >= 0 && cx->blob.p) memset(cx->blob.p, cx->pool_fill, cx->blob.cap);
   cudaError_t e = cudaEventCreate(&b.ev0);
   if (e == cudaSuccess) e = cudaEventCreate(&b.ev1);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(extra, extra_flags);
+  if (e == cudaSuccess && extra) e = cudaEventCreate(extra);
   if (e != cudaSuccess) {
-    for (cudaEvent_t ev : {b.ev0, b.ev1, *extra})
+    for (cudaEvent_t ev : {b.ev0, b.ev1, extra ? *extra : nullptr})
       if (ev) cudaEventDestroy(ev);
     return set_error(JXG_ERR_CUDA, std::string("cudaEventCreate: ") + cudaGetErrorString(e));
   }
   cx->batch_live = true;  // only once nothing can fail any more
   return 0;
+}
+
+// The stream of a run or rerun, `cuda_stream` of the entry point: the caller's, or else the context's; kept as last_stream.
+inline cudaStream_t batch_stream(BatchCore& b, void* cuda_stream) {
+  b.last_stream = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : b.ctx->stream;
+  return b.last_stream;
 }
 
 // Waits for the last run (the context's pools are then free for the next batch); the engine destroys its own events.

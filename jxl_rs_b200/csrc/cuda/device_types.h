@@ -121,7 +121,6 @@ struct BatchDev {
   const StreamDev* streams_fast;  // single-pass prefix-coded or shifted frames: k_entropy_fast
   const StreamDev* streams_slow;  // multi-pass and LZ77 frames: k_entropy
   uint32_t num_frames, num_streams, num_lean, num_fast, num_slow;
-  uint32_t reg_idct32;  // 1: rows of 32 coefficients also go through the register path (experiment knob)
   uint32_t* nzlist;     // [sections][kListStride]: list of section (pass * num_groups + group) of a frame, see above
   uint32_t* lzwin;      // [lz sections][kLzWindow] LZ77 windows (decode.rs:86-146), frames with has_lz only
   uint32_t* block_off;  // per 8x8 block: ordinal (raster order) of the varblock starting there within its group

@@ -1325,10 +1325,9 @@ __device__ __noinline__ void warp_col_pass(float* ch, int lane_col, int stride) 
 }
 
 // Types transformed in registers by k_idct_small: 8x8-footprint transforms and plain DCTs with rows of <= 16
-// coefficients. Rows of 32 (32x8 ... 32x32) unroll into ~300 KB of code and starve on instruction fetch, so they take the compact shared-memory path of k_dequant_idct unless
-// JXG_REG_IDCT32 is set.
-__device__ __forceinline__ bool is_small_reg_type(int t, bool reg32) {
-  return (t == 0) || (t >= 3 && t <= 13 && (reg32 || !(t == 5 || (t >= 8 && t <= 11))));
+// coefficients. Rows of 32 (32x8 ... 32x32) unroll into ~300 KB of code and starve on instruction fetch, so they take the compact shared-memory path of k_dequant_idct.
+__device__ __forceinline__ bool is_small_reg_type(int t) {
+  return (t == 0) || (t >= 3 && t <= 13 && !(t == 5 || (t >= 8 && t <= 11)));
 }
 
 constexpr int kIdctWarps = 8;   // per warp: dequantised work tiles 3 x kWarpBuf floats
@@ -1446,7 +1445,7 @@ __global__ void __launch_bounds__(kIdctWarps * 32) k_dequant_idct(const BatchDev
     if (raw_t < 128) continue;
     const int t = raw_t & 127;
     const int cx = c_cov_x[t], cy = c_cov_y[t];
-    if (is_small_reg_type(t, B.reg_idct32 != 0)) continue;  // handled by k_idct_small
+    if (is_small_reg_type(t)) continue;  // handled by k_idct_small
     if (cx > 4 || cy > 4) {  // big varblock: handled cooperatively below
       if (lane == 0) {
         uint32_t i = atomicAdd(&s_nbig, 1u);
@@ -1753,33 +1752,21 @@ __device__ __forceinline__ void reg_dct_block(const RegBlockCtx& X, const float*
   }
 }
 
-// types handled in registers: 8x8-footprint {0,3,12,13} and plain DCTs up to 32x32 {4..11}
-__device__ __forceinline__ int reg_class(int t) {  // 0: 8 lanes, 1: 16 lanes, 2: 32 lanes, -1: not handled
-  switch (t) {
-    case 0: case 3: case 12: case 13: case 6: case 7: case 8: case 9: return 0;
-    case 4: case 10: case 11: return 1;
-    case 5: return 2;
-    default: return -1;
-  }
-}
-
 // KIND selects the coefficient-row length handled by this instantiation (register budget): 0: L = 8 (types
-// 0, 3, 12, 13), 1: L = 16 (6, 7, 4), 2: L = 32 (8, 9, 10, 11, 5).
+// 0, 3, 12, 13), 1: L = 16 (6, 7, 4).
 __device__ __forceinline__ int reg_kind(int t) {
   switch (t) {
     case 0: case 3: case 12: case 13: return 0;
     case 6: case 7: case 4: return 1;
-    case 8: case 9: case 10: case 11: case 5: return 2;
     default: return -1;
   }
 }
 
 // Shared memory for the coefficient tiles of the lane groups of one CTA: every class of a KIND needs 32 x 8 lanes x 3 x NC
-// words with NC = 64 / 128 / 256 coefficients per channel (the 16- and 32-lane classes hold 2x / 4x the coefficients in
-// half / a quarter of the groups).
+// words with NC = 64 / 128 coefficients per channel (the 16-lane class holds 2x the coefficients in half the groups).
 template <int KIND>
 __host__ __device__ constexpr size_t small_tile_bytes() {
-  return size_t(kSmallThreads / 8) * 3 * (KIND == 0 ? 64 : (KIND == 1 ? 128 : 256)) * sizeof(int32_t);
+  return size_t(kSmallThreads / 8) * 3 * (KIND == 0 ? 64 : 128) * sizeof(int32_t);
 }
 // Behind the tiles: the staged offset words (kOffWords) and the first kStageEntries entries of the group's list,
 // delivered by two bulk copies issued by thread 0 before the CTA sorts its varblocks.
@@ -1825,9 +1812,9 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
   }
   __syncthreads();
   if (threadIdx.x == 0) {
-    const int order[12] = {0, 3, 12, 13, 6, 7, 8, 9, 4, 10, 11, 5};
+    const int order[7] = {0, 3, 12, 13, 6, 7, 4};
     uint32_t acc = 0;
-    for (int i = 0; i < 12; i++) {
+    for (int i = 0; i < 7; i++) {
       s_start[order[i]] = acc;
       s_fill[order[i]] = acc;
       acc += s_cnt[order[i]];
@@ -1840,7 +1827,7 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
     if (raw_t >= 128 && reg_kind(raw_t & 127) == KIND) s_list[atomicAdd(&s_fill[raw_t & 127], 1u)] = uint16_t(bx | (by << 5));
   }
   __syncthreads();
-  const uint32_t begin8 = 0, begin16 = s_start[4], begin32 = s_start[5], end_all = s_start[5] + s_cnt[5];
+  const uint32_t begin8 = 0, begin16 = s_start[4], end_all = s_start[4] + s_cnt[4];
   // the staged list has landed (the sort above ran while the copies were in flight)
   mbar_wait(&s_bar[0], 0);
   mbar_wait(&s_bar[1], 0);
@@ -1886,7 +1873,7 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
       int t;
       uint32_t seq;
       setup_ctx(s_list[begin8 + (valid ? li : 0)], X, lfp, t, seq);
-      constexpr uint32_t NC = KIND == 0 ? 64 : (KIND == 1 ? 128 : 256);
+      constexpr uint32_t NC = KIND == 0 ? 64 : 128;
       float* tile = s_tiles + (threadIdx.x >> 3) * 3 * NC;
       gather_dequant_tile(B, F, g, seq, tile, NC, NC, deq_of(X), r, 8, valid, stage, [&] { __syncwarp(gmask); },
                           [](uint32_t pos) { return pos; });
@@ -1895,9 +1882,6 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
       if constexpr (KIND == 1) {
         if (t == 6) reg_dct_block<8, 16, true>(X, lfp, F.xb, r, gmask, valid);
         else reg_dct_block<8, 16, false>(X, lfp, F.xb, r, gmask, valid);
-      } else if constexpr (KIND == 2) {
-        if (t == 8) reg_dct_block<8, 32, true>(X, lfp, F.xb, r, gmask, valid);
-        else reg_dct_block<8, 32, false>(X, lfp, F.xb, r, gmask, valid);
       } else if (t == 0) {
         reg_dct_block<8, 8, true>(X, lfp, F.xb, r, gmask, valid);
       } else {
@@ -1979,7 +1963,7 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
   {
     const uint32_t r = threadIdx.x & 15;
     const uint32_t gmask = 0xffffu << (threadIdx.x & 16);
-    const uint32_t count = begin32 - begin16;
+    const uint32_t count = end_all - begin16;
     const uint32_t iters = (count + kSmallThreads / 16 - 1) / (kSmallThreads / 16);
     for (uint32_t it = 0; it < iters; it++) {
       const uint32_t li = it * (kSmallThreads / 16) + (threadIdx.x >> 4);
@@ -1989,42 +1973,14 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
       int t;
       uint32_t seq;
       setup_ctx(s_list[begin16 + (valid ? li : 0)], X, lfp, t, seq);
-      constexpr uint32_t NC = KIND == 1 ? 256 : 512;
-      if constexpr (KIND >= 1) {
+      if constexpr (KIND == 1) {
+        constexpr uint32_t NC = 256;
         float* tile = s_tiles + (threadIdx.x >> 4) * 3 * NC;
         gather_dequant_tile(B, F, g, seq, tile, NC, NC, deq_of(X), r, 16, valid, stage, [&] { __syncwarp(gmask); },
                             [](uint32_t pos) { return pos; });
         X.coeffs = tile;
         X.cstride = NC;
-      }
-      if constexpr (KIND == 1) {
         reg_dct_block<16, 16, true>(X, lfp, F.xb, r, gmask, valid);
-      } else if constexpr (KIND == 2) {
-        if (t == 10) reg_dct_block<16, 32, true>(X, lfp, F.xb, r, gmask, valid);
-        else reg_dct_block<16, 32, false>(X, lfp, F.xb, r, gmask, valid);
-      }
-    }
-  }
-  // ---------------- class 2: 32 lanes per block ----------------
-  {
-    const uint32_t r = threadIdx.x & 31;
-    const uint32_t count = end_all - begin32;
-    const uint32_t iters = (count + kSmallThreads / 32 - 1) / (kSmallThreads / 32);
-    for (uint32_t it = 0; it < iters; it++) {
-      const uint32_t li = it * (kSmallThreads / 32) + (threadIdx.x >> 5);
-      const bool valid = li < count;
-      RegBlockCtx X;
-      const float* lfp[3];
-      int t;
-      uint32_t seq;
-      setup_ctx(s_list[begin32 + (valid ? li : 0)], X, lfp, t, seq);
-      if constexpr (KIND == 2) {
-        float* tile = s_tiles + (threadIdx.x >> 5) * 3 * 1024;
-        gather_dequant_tile(B, F, g, seq, tile, 1024, 1024, deq_of(X), r, 32, valid, stage, [&] { __syncwarp(); },
-                            [](uint32_t pos) { return pos; });
-        X.coeffs = tile;
-        X.cstride = 1024;
-        reg_dct_block<32, 32, true>(X, lfp, F.xb, r, 0xffffffffu, valid);
       }
     }
   }
@@ -2930,13 +2886,12 @@ cudaError_t configure_kernels() {
   if ((e = configure_filters<true, 3>()) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(k_idct_small<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(small_smem_bytes<0>()))) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(k_idct_small<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(small_smem_bytes<1>()))) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(k_idct_small<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(small_smem_bytes<2>()))) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(k_dequant_idct, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kLargeSmemBytes))) != cudaSuccess) return e;
   return cudaSuccess;
 }
 
 int launch_pipeline(const BatchDev& B, cudaStream_t stream, int debug_stop, cudaEvent_t* ev, bool lean_all_420,
-                    uint32_t lean_S, uint32_t lean_ctas, bool lean_ctx_smem, cudaStream_t post_stream, cudaEvent_t handoff) {
+                    uint32_t lean_S, uint32_t lean_ctas, bool lean_ctx_smem) {
   // ev (optional, kNumStages + 1 events): ev[i] is recorded before stage i, ev[i+1] after it; stages that do not
   // run record nothing (the host pairs consecutive recorded events).
   int launches = 0;
@@ -2984,15 +2939,9 @@ int launch_pipeline(const BatchDev& B, cudaStream_t stream, int debug_stop, cuda
   }
   mark(2);
   if (debug_stop == 1) return launches;
-  if (post_stream != stream) {  // two-stage pipeline: the transforms and filters of this batch continue on the post stream
-    cudaEventRecord(handoff, stream);
-    cudaStreamWaitEvent(post_stream, handoff, 0);
-    stream = post_stream;
-  }
   k_idct_small<0><<<B.num_streams, kSmallThreads, small_smem_bytes<0>(), stream>>>(B);
   k_idct_small<1><<<B.num_streams, kSmallThreads, small_smem_bytes<1>(), stream>>>(B);
-  if (B.reg_idct32) k_idct_small<2><<<B.num_streams, kSmallThreads, small_smem_bytes<2>(), stream>>>(B);
-  launches += B.reg_idct32 ? 3 : 2;
+  launches += 2;
   k_dequant_idct<<<B.num_streams, kIdctWarps * 32, kLargeSmemBytes, stream>>>(B);
   launches++;
   mark(3);

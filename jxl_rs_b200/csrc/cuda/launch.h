@@ -9,11 +9,11 @@ namespace jxgpu {
 int sm_count();
 cudaError_t upload_constants(const float* wc, const float* rdct_scale);
 cudaError_t configure_kernels();
-// Enqueues the K1..K2 part of the pipeline: block plan + entropy kernels on `stream`, then (after `handoff`, when
-// post_stream differs) the transform kernels on `post_stream`; returns the number of kernel launches.
+// Enqueues the K1..K2 part of the pipeline on `stream`: block plan, entropy kernels, transform kernels; returns the
+// number of kernel launches.
 // debug_stop 1 stops after the entropy kernels, 2 after the transforms (as 0 does: the caller launches the filters).
 int launch_pipeline(const BatchDev& B, cudaStream_t stream, int debug_stop, cudaEvent_t* ev, bool lean_all_420,
-                    uint32_t lean_S, uint32_t lean_ctas, bool lean_ctx_smem, cudaStream_t post_stream, cudaEvent_t handoff);
+                    uint32_t lean_S, uint32_t lean_ctas, bool lean_ctx_smem);
 constexpr int kFusedTileW = 64, kFusedTileH = 32;
 int launch_filter_range(const BatchDev& B, const uint32_t* fused_prefix, uint32_t tile_begin, uint32_t tile_count,
                         uint32_t filter_cfg_mask, cudaStream_t stream);

@@ -550,7 +550,7 @@ void jxg_modular_parsed_free(void* parsed) { delete static_cast<jxg::ModularFram
 int jxg_modular_batch_begin(void* c, void** out_batch) {
   if (!c || !out_batch) return JXG_ERR_ARGUMENT;
   auto b = std::make_unique<ModularBatch>();
-  if (int r = batch_begin(*b, static_cast<Context*>(c), &b->ev_decode, cudaEventDefault)) return r;
+  if (int r = batch_begin(*b, static_cast<Context*>(c), &b->ev_decode)) return r;
   *out_batch = b.release();
   return JXG_OK;
 }
@@ -581,8 +581,7 @@ int jxg_modular_batch_run(void* bp, void* cuda_stream) {
   if (!b || b->frames.empty()) return JXG_ERR_ARGUMENT;
   Context* cx = b->ctx;
   CUDA_TRY(cudaSetDevice(cx->device));
-  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : cx->stream;
-  b->last_stream = s;
+  cudaStream_t s = batch_stream(*b, cuda_stream);
   b->h2d = b->d2h = 0;
   // streams without LZ77, then those with it (each group has its own decode launch); longest section first within
   // each (the decode kernel's queue is a longest-processing-time schedule)
@@ -633,8 +632,7 @@ int jxg_modular_batch_rerun_device(void* bp, void* cuda_stream) {
   ModularBatch* b = static_cast<ModularBatch*>(bp);
   if (!b || !b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch was never submitted");
   CUDA_TRY(cudaSetDevice(b->ctx->device));
-  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : b->ctx->stream;
-  b->last_stream = s;
+  cudaStream_t s = batch_stream(*b, cuda_stream);
   CUDA_TRY(cudaStreamWaitEvent(s, b->ev1, 0));  // the previous run of this batch still owns its device buffers
   if (int r = fill_pools(b->ctx, s, false)) return r;
   CUDA_TRY(cudaEventRecord(b->ev0, s));

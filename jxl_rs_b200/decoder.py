@@ -229,15 +229,6 @@ def decode_files(ctx: JxgContext, files, pixel_format: JxlPixelFormat = JxlPixel
     return outs
 
 
-def device_streams(device: int = 0):
-    """(entropy stream, post stream) of the device as raw cudaStream_t values (jxg_device_streams): the optional stage
-    streams (JXG_STAGE_STREAMS=1); by default every batch runs on its context's own stream."""
-    lib = abi.load_library()
-    e, p = C.c_void_p(), C.c_void_p()
-    abi.check(lib, lib.jxg_device_streams(device, C.byref(e), C.byref(p)))
-    return e.value, p.value
-
-
 def _parse_cpulist(text):
     cpus = set()
     for part in text.strip().split(","):

@@ -29,9 +29,6 @@ def install(setattr_fn, fail_e2e=False, gloo=False):
     setattr_fn(torch.cuda, "synchronize", lambda *a, **k: None)
     setattr_fn(torch.cuda, "Stream", _FakeStream)
     setattr_fn(torch.cuda, "Event", _FakeEvent)
-    setattr_fn(torch.cuda, "ExternalStream", lambda ptr, *a, **k: _FakeStream())
-    for mod in (decoder, j):
-        setattr_fn(mod, "device_streams", lambda device=0: (1, 2))
     setattr_fn(torch.cuda, "current_stream", lambda *a, **k: _FakeStream())
     setattr_fn(torch.cuda, "mem_get_info", lambda *a, **k: (150 << 30, 180 << 30))
     real_empty, real_tensor = torch.empty, torch.tensor

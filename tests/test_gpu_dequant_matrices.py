@@ -5,14 +5,9 @@ Every table index 0-16 carries a custom table in frames whose varblocks read it,
 from the frame's blob (F.dequant_off[qt] >= 0):
   - k_idct_small (is_small_reg_type): tables 0, 3, 4, 6 and 9;
   - the warp path of k_dequant_idct: the 32-row DCTs (tables 5, 7, 8) and IDENTITY, DCT2X2, AFV (tables 1, 2, 10);
-  - the CTA path of k_dequant_idct: tables 11-16;
-  - with JXG_REG_IDCT32=1 the 32-row DCTs move into k_idct_small (one case, in a subprocess).
+  - the CTA path of k_dequant_idct: tables 11-16.
 RAW tables with random entries sit at the square indices 0 and 11 and the non-square index 6. A mixed batch puts
 frames with different custom tables for the same index, library tables and a shared custom table side by side."""
-import os
-import subprocess
-import sys
-
 import pytest
 
 from tests import f64_quant as fq
@@ -20,7 +15,6 @@ from tests.gpu_stages import check_frames
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 # (width, height, seed) of profile-4 frames that place a varblock of every table index
 ALL_TABLES = [(512, 512, 14), (768, 512, 12)]
 
@@ -54,6 +48,7 @@ CASES = [
     (ALL_TABLES[0], 2, {4: fq.MODE_RAW, 12: fq.MODE_RAW, 15: fq.MODE_RAW}, 1, 0, 0, 7),  # RAW on 16x16, 32x64, 256x256
     (ALL_TABLES[1], 3, {0: fq.MODE_DCT, 1: fq.MODE_DCT, 2: fq.MODE_DCT, 3: fq.MODE_DCT, 9: fq.MODE_DCT,
                         10: fq.MODE_DCT, 16: fq.MODE_RAW}, 3, 1, 7, 0),                  # DCT mode on the 8x8 tables
+    (ALL_TABLES[0], 21, {5: fq.MODE_RAW}, 2, 1, 3, 2),                                    # RAW on 32x32
 ]
 
 
@@ -72,25 +67,3 @@ def test_mixed_batch_matches_f64(ctx):
     datas = [_frame(ALL_TABLES[0], ea), _frame(ALL_TABLES[0], eb), _frame(ALL_TABLES[0], None),
              _frame(ALL_TABLES[1], ea)]
     check_frames(ctx, datas, "mixed dequant batch", [ea, eb, None, ea])
-
-
-def reg_idct32_case():
-    """The 32-row DCT tables (5, 7, 8) and the others, custom, with the 32-row DCTs in k_idct_small; run in a
-    process started with JXG_REG_IDCT32=1."""
-    import jxl_rs_b200 as j
-    assert os.environ.get("JXG_REG_IDCT32") == "1"
-    encs = fq.profile4_encodings(21, {5: fq.MODE_RAW})
-    c = j.JxgContext(0)
-    try:
-        check_frames(c, [_frame(ALL_TABLES[0], encs)], "JXG_REG_IDCT32=1", [encs])
-    finally:
-        c.close()
-
-
-def test_reg_idct32_route_matches_f64():
-    code = "from tests.test_gpu_dequant_matrices import reg_idct32_case; reg_idct32_case()"
-    args = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code]
-    r = subprocess.run(args, cwd=ROOT, env=dict(os.environ, JXG_REG_IDCT32="1"), capture_output=True, text=True,
-                       timeout=900)
-    print(r.stdout)
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-4000:]

@@ -9,10 +9,9 @@ filled with 0xFF and on one filled with 0x7F, and every byte must agree:
       frames of test_vardct_ref in one batch per entropy route test_gpu_vardct_ref asserts (lean with and without the
       (4, 2, 0) form and the shared-memory context map, prefix, multi-pass / LZ77, all nineteen mixed), 8 lanes per
       warp and a two-pass frame of large varblocks (k_dequant_idct's CTA path adds the passes up in the planes); the
-      header-field sets of test_gpu_header_fields (one batch per filter path); the custom dequantisation
-      frames (also with JXG_REG_IDCT32=1 in a subprocess); the frames of test_gpu_f64_stages (all eight Gaborish / EPF
-      pairs, one-pixel edge tiles, profiles 0-3) and its real fixtures plus the multi-pass progressive_ac; every output
-      format at orientations 1-8. The float64 check (gpu_stages.check_frames) then runs on a poisoned context for one
+      header-field sets of test_gpu_header_fields (one batch per filter path); the custom dequantisation frames; the
+      frames of test_gpu_f64_stages (all eight Gaborish / EPF pairs, one-pixel edge tiles, profiles 0-3) and its real
+      fixtures plus the multi-pass progressive_ac; every output format at orientations 1-8. The float64 check (gpu_stages.check_frames) then runs on a poisoned context for one
       set per route: lean and prefix frames, an LZ77 frame, custom tables and header fields.
   (b) Modular: the token frames of test_modular_ref, test_modular_squeeze, test_modular_lz77 and
       test_modular_walk_table at 1, 2 and 4 lanes per warp, equal to the integer model, and the real Modular fixtures
@@ -31,8 +30,6 @@ Subsets: the token frames run as six batches rather than nineteen single frames,
 the kernels branch on; the output formats and orientations run on one 320x192 frame (test_gpu_output_stage's); the
 float64 check runs once per route, not per set, because the bit equality with the new context carries the rest."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -43,7 +40,6 @@ from tests import test_vardct_ref as T
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FILLS = (0xFF, 0x7F)
 U8, XYB = abi.FORMAT_RGB_U8, abi.FORMAT_XYB_F32_PLANAR
 
@@ -249,31 +245,6 @@ def test_custom_dequant_tables(poisoned):
     datas = [DQ._frame(size, fq.profile4_encodings(es, modes), epf, gab, xq, bq)
              for size, es, modes, epf, gab, xq, bq in DQ.CASES]
     same_on_every_context(poisoned, datas, "custom dequant tables")
-
-
-def reg_idct32_case():
-    """Custom tables with the 32-row DCTs in k_idct_small; run in a process started with JXG_REG_IDCT32=1."""
-    import jxl_rs_b200 as j
-    from tests import f64_quant as fq
-    from tests import test_gpu_dequant_matrices as DQ
-    assert os.environ.get("JXG_REG_IDCT32") == "1"
-    cs = {byte: j.JxgContext(0) for byte in FILLS}
-    try:
-        for byte, c in cs.items():
-            c.set_pool_fill(byte)
-        same_on_every_context(cs, [DQ._frame(DQ.ALL_TABLES[0], fq.profile4_encodings(21, {5: fq.MODE_RAW}))],
-                              "JXG_REG_IDCT32=1")
-    finally:
-        for c in cs.values():
-            c.close()
-
-
-def test_reg_idct32_route():
-    code = "from tests.test_gpu_pool_fill import reg_idct32_case; reg_idct32_case()"
-    args = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code]
-    r = subprocess.run(args, cwd=ROOT, env=dict(os.environ, JXG_REG_IDCT32="1"), capture_output=True, text=True,
-                       timeout=900)
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-4000:]
 
 
 def test_filter_pairs_profiles_and_entropy_codes(poisoned):
