@@ -267,6 +267,43 @@ int jxg_batch_add_parsed(void* batch, void* parsed, uint32_t output_format, void
 int jxg_parsed_desc(void* parsed, uint32_t output_format, JxgFrameDesc* desc, const uint8_t** hf_bytes,
                     const uint64_t** sec_off, const uint32_t** sec_len, uint32_t* n_sections);
 
+/* ---- Region decode of VarDCT frames ------------------------------------------------------------------------------
+ * A region is a rectangle of the OUTPUT image (display orientation, the JxgImageInfo width x height). Its pixels are
+ * defined as the pixels the whole-frame decode gives on that rectangle; the reference has no crop API. The bytes are
+ * the same when both outputs take the same store path. That holds in every case but one: Gaborish + EPF 2 frames with
+ * orientation 1 in RGB_U8, RGBA_U8 or RGB_F32. These filter their interior tiles with a vector path when the output
+ * row is aligned: for RGB_U8 a row stride (and, for a device output, a base address) that is a multiple of 4 bytes,
+ * otherwise a multiple of 16. The vector path differs from the scalar one by a few float ulps (1 LSB at most in U8).
+ * So the region and whole outputs are byte-identical when both are aligned or both are not. Only the HF
+ * groups the region needs are entropy-decoded, transformed and filtered: the 256x256 groups that hold a pixel the
+ * region's pixels depend on through Gaborish and EPF (within 1 + 2 / 3 / 6 pixels; with Gaborish + EPF 2, of the
+ * 64x32 filter tiles that meet the region), and only the region is stored. The output buffer holds region.height rows
+ * of region.width pixels; stride and alignment rules are those of jxg_batch_add_frame applied to that width. The
+ * region must be non-empty and inside the image, and the format must not be XYB_F32_PLANAR: JXG_ERR_ARGUMENT
+ * otherwise. jxg_batch_read_coeffs / jxg_batch_read_xyb refuse a region frame (JXG_ERR_ARGUMENT); jxg_batch_wait
+ * reports the group index of the whole frame. Each region is its own frame of the batch, also when regions of one
+ * frame overlap. */
+typedef struct JxgRegion {
+  uint32_t x, y, width, height;
+} JxgRegion;
+
+/* jxg_batch_add_frame for a region: desc and the sections describe the whole frame and are checked as
+ * jxg_batch_add_frame checks them. */
+int jxg_batch_add_frame_region(void* batch, const JxgFrameDesc* desc, const uint8_t* hf_bytes, const uint64_t* sec_off,
+                               const uint32_t* sec_len, uint32_t n_sections, const JxgRegion* region, void* out,
+                               size_t out_row_stride, int out_is_device);
+/* jxg_batch_add_parsed for a region. */
+int jxg_batch_add_parsed_region(void* batch, void* parsed, uint32_t output_format, const JxgRegion* region, void* out,
+                                size_t out_row_stride, int out_is_device);
+/* Parity tap, no device needed: the sub-frame a region decodes, as a self-contained (desc, sections) tuple that
+ * jxg_batch_add_frame would take. Its groups are the rectangle of whole groups the region needs (origin: the coded
+ * position of its top-left pixel, multiples of 256); section s = pass * G' + group of the sub-frame (G' its group count)
+ * is section pass * G + group of the frame. window: the top-left of the region inside the sub-frame's display-oriented
+ * output. The pointers stay valid until the next call on `parsed` or jxg_parsed_free. */
+int jxg_parsed_region_desc(void* parsed, uint32_t output_format, const JxgRegion* region, JxgFrameDesc* desc,
+                           const uint8_t** hf_bytes, const uint64_t** sec_off, const uint32_t** sec_len,
+                           uint32_t* n_sections, uint32_t origin[2], uint32_t window[2]);
+
 /* ---- Modular frames (BASELINE config 5; SURVEY §8 rows a18 / a19) ------------------------------------------------
  * Seam: FullModularImage::read_stream for ModularHF sections (jxl/src/frame/modular/mod.rs:567,
  * decode/bitstream.rs:134, decode/channel.rs:220) plus the inverse transforms (transforms/{rct,squeeze}.rs) and

@@ -64,6 +64,11 @@ class JxgImageInfo(C.Structure):
                 ("coded_width", C.c_uint32), ("coded_height", C.c_uint32), ("orientation", C.c_uint32)]
 
 
+class JxgRegion(C.Structure):
+    """A rectangle of the output image (display orientation)."""
+    _fields_ = [("x", C.c_uint32), ("y", C.c_uint32), ("width", C.c_uint32), ("height", C.c_uint32)]
+
+
 # every symbol include/jxg.h declares (tests check the .so exports all of them)
 EXPORTS = [
     "jxg_init", "jxg_shutdown", "jxg_context_set_pool_fill", "jxg_batch_begin", "jxg_batch_add_frame", "jxg_batch_run", "jxg_batch_wait",
@@ -74,7 +79,8 @@ EXPORTS = [
     "jxg_modular_parse_file", "jxg_modular_parsed_free", "jxg_modular_batch_begin", "jxg_modular_batch_add",
     "jxg_modular_batch_set_lanes", "jxg_modular_batch_run", "jxg_modular_batch_wait", "jxg_modular_batch_rerun_device",
     "jxg_modular_batch_read_planes", "jxg_modular_batch_stats", "jxg_modular_batch_end", "jxg_modular_walk_table",
-    "jxg_modular_batch_lz77_stats", "jxg_modular_batch_walk_stats",
+    "jxg_modular_batch_lz77_stats", "jxg_modular_batch_walk_stats", "jxg_batch_add_frame_region", "jxg_batch_add_parsed_region",
+    "jxg_parsed_region_desc",
 ]
 
 _LIB = None
@@ -144,6 +150,12 @@ def load_library():
     lib.jxg_parsed_desc.argtypes = [vp, C.c_uint32, C.POINTER(JxgFrameDesc), C.POINTER(vp), C.POINTER(vp),
                                     C.POINTER(vp), u32p]
     lib.jxg_batch_add_parsed.argtypes = [vp, vp, C.c_uint32, vp, C.c_size_t, C.c_int]
+    rp = C.POINTER(JxgRegion)
+    lib.jxg_batch_add_frame_region.argtypes = [vp, C.POINTER(JxgFrameDesc), vp, vp, vp, C.c_uint32, rp, vp, C.c_size_t,
+                                               C.c_int]
+    lib.jxg_batch_add_parsed_region.argtypes = [vp, vp, C.c_uint32, rp, vp, C.c_size_t, C.c_int]
+    lib.jxg_parsed_region_desc.argtypes = [vp, C.c_uint32, rp, C.POINTER(JxgFrameDesc), C.POINTER(vp), C.POINTER(vp),
+                                           C.POINTER(vp), u32p, u32p, u32p]
     _LIB = lib
     return lib
 

@@ -16,6 +16,7 @@
 
 #include "../../../include/jxg.h"
 #include "../host/frame.h"
+#include "../host/region.h"
 #include "device_types.h"
 #include "batch_common.h"
 #include "launch.h"
@@ -71,6 +72,10 @@ struct Batch : BatchCore {
   std::vector<uint2> lean_warps;  // per warp of k_entropy_lean: first stream (relative to its frame's list), lanes
   std::vector<uint32_t> fused_prefix{0};
   std::vector<FrameOut> outs;
+  // per frame: the slice of a region frame (its tables, sections and group map), nullptr for a whole frame; the slices
+  // are owned here until jxg_batch_end because a deferred copy reads their tables at jxg_batch_run
+  std::vector<const jxg::RegionSlice*> frame_region;
+  std::vector<std::unique_ptr<jxg::RegionSlice>> regions;
   uint64_t total_groups = 0, total_blocks = 0, total_plane_floats = 0, out_bytes = 0, orient_bytes = 0;
   uint32_t lz_windows = 0;
   uint32_t filter_cfg_mask = 0;  // bit (gab * 4 + min(epf_iters, 3))
@@ -334,9 +339,10 @@ int jxg_batch_set_debug_stop(void* bp, int stage) {
 
 // `trusted`: the descriptor comes from the in-tree front-end, which guarantees every invariant validate_desc checks by
 // construction (the scan costs ~0.45 ms per 4K frame, 30 ms per 64-frame batch on the dispatcher's critical path).
+// `region`: d is the sub-frame of a region (jxg::slice_region) and only its window is stored; nullptr: the whole frame.
 static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_bytes, const uint64_t* sec_off,
                           const uint32_t* sec_len, uint32_t n_sections, void* out, size_t out_row_stride,
-                          int out_is_device, bool trusted) {
+                          int out_is_device, bool trusted, const jxg::RegionSlice* region = nullptr) {
   Batch* b = static_cast<Batch*>(bp);
   if (!b || !d || !hf_bytes || !sec_off || !sec_len || !out) return JXG_ERR_ARGUMENT;
   if (d->abi_version != JXG_ABI_VERSION) return set_error(JXG_ERR_ARGUMENT, "ABI version mismatch");
@@ -364,7 +370,13 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
                : (d->output_format == JXG_FORMAT_RGB_U16 || d->output_format == JXG_FORMAT_RGB_F16) ? 6 : 4;
   if (d->orientation > 8) return set_error(JXG_ERR_ARGUMENT, "orientation must be 1..8");
   const uint32_t orientation = (d->orientation == 0 || d->output_format == JXG_FORMAT_XYB_F32_PLANAR) ? 1u : d->orientation;
-  const uint32_t disp_w = orientation >= 5 ? F.height : F.width, disp_h = orientation >= 5 ? F.width : F.height;
+  if (region && d->output_format == JXG_FORMAT_XYB_F32_PLANAR) return set_error(JXG_ERR_ARGUMENT, "XYB_F32_PLANAR has no region form");
+  // the stored window of the coded image
+  F.win_x = region ? region->coded_win[0] : 0;
+  F.win_y = region ? region->coded_win[1] : 0;
+  F.win_w = region ? region->coded_win[2] : F.width;
+  F.win_h = region ? region->coded_win[3] : F.height;
+  const uint32_t disp_w = orientation >= 5 ? F.win_h : F.win_w, disp_h = orientation >= 5 ? F.win_w : F.win_h;
   if (out_row_stride < size_t(disp_w) * bpp) return set_error(JXG_ERR_INVALID_OUTPUT, "output row stride too small");
   // The stores (and the orientation pass's word copies) write whole samples: rows, and a device buffer, must be
   // aligned to the sample size (include/jxg.h).
@@ -486,17 +498,17 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   fo.copy_bytes = (rows - 1) * out_row_stride + size_t(disp_w) * bpp;  // the last row of a user buffer may be unpadded
   fo.is_device = out_is_device != 0;
   fo.orientation = orientation;
-  fo.coded_w = F.width;
-  fo.coded_h = F.height;
+  fo.coded_w = F.win_w;
+  fo.coded_h = F.win_h;
   fo.bpp = uint32_t(bpp);
   if (!fo.is_device) {
     fo.dev_off = (b->out_bytes + 255) / 256 * 256;
     b->out_bytes = fo.dev_off + fo.bytes;
   }
-  if (orientation != 1) {  // coded image, tight rows (16-byte multiples: the vector store path stays usable)
-    fo.stage_stride = (size_t(F.width) * bpp + 15) / 16 * 16;
+  if (orientation != 1) {  // coded window, tight rows (16-byte multiples: the vector store path stays usable)
+    fo.stage_stride = (size_t(F.win_w) * bpp + 15) / 16 * 16;
     fo.stage_off = (b->orient_bytes + 255) / 256 * 256;
-    b->orient_bytes = fo.stage_off + fo.stage_stride * F.height;
+    b->orient_bytes = fo.stage_off + fo.stage_stride * F.win_h;
     F.out_row_stride = fo.stage_stride;
   }
   b->outs.push_back(fo);
@@ -532,8 +544,14 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   }
   F.tf_pq_mul = d->intensity_target * (1.0f / 10000.0f);
   b->filter_cfg_mask |= 1u << ((d->gab ? 4 : 0) + std::min<uint32_t>(d->epf_iters, 3));
-  b->fused_prefix.push_back(b->fused_prefix.back() + ((F.width + kFusedTileW - 1) / kFusedTileW) * ((F.height + kFusedTileH - 1) / kFusedTileH));
+  // filter tiles that meet the window
+  F.win_tx0 = F.win_x / kFusedTileW;
+  F.win_ty0 = F.win_y / kFusedTileH;
+  F.win_ntx = (F.win_x + F.win_w + kFusedTileW - 1) / kFusedTileW - F.win_tx0;
+  const uint32_t win_nty = (F.win_y + F.win_h + kFusedTileH - 1) / kFusedTileH - F.win_ty0;
+  b->fused_prefix.push_back(b->fused_prefix.back() + F.win_ntx * win_nty);
   b->frames.push_back(F);
+  b->frame_region.push_back(region);
   return JXG_OK;
 }
 
@@ -541,6 +559,32 @@ int jxg_batch_add_frame(void* bp, const JxgFrameDesc* d, const uint8_t* hf_bytes
                         const uint32_t* sec_len, uint32_t n_sections, void* out, size_t out_row_stride,
                         int out_is_device) {
   return add_frame_impl(bp, d, hf_bytes, sec_off, sec_len, n_sections, out, out_row_stride, out_is_device, false);
+}
+
+// A region of a frame: the full descriptor is checked as jxg_batch_add_frame checks it, sliced to the sub-frame of the
+// region, and the sub-frame is added as an ordinary frame that stores only the region.
+static int add_region_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_bytes, const uint64_t* sec_off,
+                           const uint32_t* sec_len, uint32_t n_sections, const JxgRegion* region, void* out,
+                           size_t out_row_stride, int out_is_device, bool trusted) {
+  Batch* b = static_cast<Batch*>(bp);
+  if (!b || !d || !hf_bytes || !sec_off || !sec_len || !out || !region) return JXG_ERR_ARGUMENT;
+  if (d->abi_version != JXG_ABI_VERSION) return set_error(JXG_ERR_ARGUMENT, "ABI version mismatch");
+  if (d->num_passes == 0 || d->num_passes > kMaxPasses) return set_error(JXG_ERR_ARGUMENT, "bad num_passes");
+  if (!trusted)
+    if (int r = validate_desc(d, sec_len, n_sections)) return r;
+  auto s = std::make_unique<jxg::RegionSlice>();
+  const char* why = "";
+  if (int r = jxg::slice_region(*d, sec_off, sec_len, n_sections, *region, s.get(), &why)) return set_error(r, why);
+  const int r = add_frame_impl(bp, &s->desc, hf_bytes, s->sec_off.data(), s->sec_len.data(), uint32_t(s->sec_off.size()), out,
+                               out_row_stride, out_is_device, /*trusted=*/true, s.get());
+  if (r == JXG_OK) b->regions.push_back(std::move(s));
+  return r;
+}
+
+int jxg_batch_add_frame_region(void* bp, const JxgFrameDesc* d, const uint8_t* hf_bytes, const uint64_t* sec_off,
+                               const uint32_t* sec_len, uint32_t n_sections, const JxgRegion* region, void* out,
+                               size_t out_row_stride, int out_is_device) {
+  return add_region_impl(bp, d, hf_bytes, sec_off, sec_len, n_sections, region, out, out_row_stride, out_is_device, false);
 }
 
 // Schedule of the persistent entropy lanes (k_entropy_lean). A stream's cost is proportional to its section length
@@ -794,7 +838,16 @@ int jxg_batch_wait(void* bp, uint32_t* first_bad_frame, uint32_t* first_bad_grou
   }
   CUDA_TRY(cudaGetLastError());
   cudaEventElapsedTime(&b->last_ms, b->ev0, b->ev1);
-  return batch_first_failure(*b, b->streams, "entropy decode failed in frame ", first_bad_frame, first_bad_group);
+  uint32_t f = 0, g = 0;
+  const int r = batch_first_failure(*b, b->streams, "entropy decode failed in frame ", &f, &g);
+  if (r == JXG_OK) return r;
+  if (const jxg::RegionSlice* rs = b->frame_region[f]) {  // a region frame reports the group of the full frame
+    g = rs->real_group[g];
+    set_error(r, "entropy decode failed in frame " + std::to_string(f) + " group " + std::to_string(g));
+  }
+  if (first_bad_frame) *first_bad_frame = f;
+  if (first_bad_group) *first_bad_group = g;
+  return r;
 }
 
 int jxg_batch_stats(void* bp, uint64_t* kernel_launches, uint64_t* h2d_bytes, uint64_t* d2h_bytes, float* last_device_ms) {
@@ -823,6 +876,7 @@ int jxg_batch_entropy_stats(void* bp, uint32_t* n_lean, uint32_t* n_fast, uint32
 int jxg_batch_read_coeffs(void* bp, uint32_t f, int32_t* out, size_t out_len) {
   Batch* b = static_cast<Batch*>(bp);
   if (!b || f >= b->frames.size() || !b->uploaded) return JXG_ERR_ARGUMENT;
+  if (b->frame_region[f]) return set_error(JXG_ERR_ARGUMENT, "the coefficient tap has no region form");
   const FrameDev& F = b->frames[f];
   size_t n = size_t(F.num_groups) * 3 * kGroupCoeffs;
   if (out_len < n) return JXG_ERR_ARGUMENT;
@@ -842,6 +896,7 @@ int jxg_batch_read_coeffs(void* bp, uint32_t f, int32_t* out, size_t out_len) {
 int jxg_batch_read_xyb(void* bp, uint32_t f, int stage, float* out, size_t out_len) {
   Batch* b = static_cast<Batch*>(bp);
   if (!b || f >= b->frames.size() || !b->uploaded || stage != 0) return JXG_ERR_ARGUMENT;
+  if (b->frame_region[f]) return set_error(JXG_ERR_ARGUMENT, "the XYB tap has no region form");
   const FrameDev& F = b->frames[f];
   size_t n = 3 * F.plane_size;
   if (out_len < n) return JXG_ERR_ARGUMENT;
@@ -903,6 +958,45 @@ int jxg_batch_add_parsed(void* batch, void* parsed, uint32_t output_format, void
   fs->fill_desc(&d, output_format);
   return add_frame_impl(batch, &d, fs->codestream.data(), fs->hf_off.data(), fs->hf_len.data(), uint32_t(fs->hf_off.size()), out,
                         out_row_stride, out_is_device, /*trusted=*/true);
+}
+
+int jxg_batch_add_parsed_region(void* batch, void* parsed, uint32_t output_format, const JxgRegion* region, void* out,
+                                size_t out_row_stride, int out_is_device) {
+  jxg::FrameState* fs = static_cast<jxg::FrameState*>(parsed);
+  if (!fs) return JXG_ERR_ARGUMENT;
+  JxgFrameDesc d;
+  fs->fill_desc(&d, output_format);
+  return add_region_impl(batch, &d, fs->codestream.data(), fs->hf_off.data(), fs->hf_len.data(), uint32_t(fs->hf_off.size()),
+                         region, out, out_row_stride, out_is_device, /*trusted=*/true);
+}
+
+int jxg_parsed_region_desc(void* parsed, uint32_t output_format, const JxgRegion* region, JxgFrameDesc* desc,
+                           const uint8_t** hf_bytes, const uint64_t** sec_off, const uint32_t** sec_len,
+                           uint32_t* n_sections, uint32_t origin[2], uint32_t window[2]) {
+  jxg::FrameState* fs = static_cast<jxg::FrameState*>(parsed);
+  if (!fs || !desc || !region) return JXG_ERR_ARGUMENT;
+  JxgFrameDesc d;
+  fs->fill_desc(&d, output_format);
+  auto s = std::make_unique<jxg::RegionSlice>();
+  const char* why = "";
+  if (int r = jxg::slice_region(d, fs->hf_off.data(), fs->hf_len.data(), uint32_t(fs->hf_off.size()), *region, s.get(), &why))
+    return set_error(r, why);
+  fs->region_tap = std::move(s);
+  const jxg::RegionSlice& rs = *fs->region_tap;
+  *desc = rs.desc;
+  if (hf_bytes) *hf_bytes = fs->codestream.data();
+  if (sec_off) *sec_off = rs.sec_off.data();
+  if (sec_len) *sec_len = rs.sec_len.data();
+  if (n_sections) *n_sections = uint32_t(rs.sec_off.size());
+  if (origin) {
+    origin[0] = rs.origin[0];
+    origin[1] = rs.origin[1];
+  }
+  if (window) {
+    window[0] = rs.window[0];
+    window[1] = rs.window[1];
+  }
+  return JXG_OK;
 }
 
 }  // extern "C"

@@ -87,7 +87,10 @@ struct FrameDev {
   uint64_t plane_size;        // plane_stride * plane_rows
   uint64_t out_off;           // byte offset into device output buffer (or absolute pointer if out_is_ptr)
   uint64_t out_row_stride;
-  void* out_ptr;              // device pointer for this frame's output
+  void* out_ptr;              // device pointer for this frame's output: pixel (win_x, win_y) of the coded image
+  // Window of the coded image the store writes (the whole frame, or a region of a sub-frame) and the 64x32 filter tiles
+  // that meet it: tiles win_tx0 .. win_tx0 + win_ntx - 1 across, from row win_ty0 down.
+  uint32_t win_x, win_y, win_w, win_h, win_tx0, win_ty0, win_ntx;
   // filters / colour
   uint32_t gab, epf_iters;
   float gab_k0[3], gab_k1[3], gab_k2[3];  // normalised weights (gaborish.rs:20-27)

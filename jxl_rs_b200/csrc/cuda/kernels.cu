@@ -20,6 +20,7 @@
 
 #include "../../../include/jxg.h"
 #include "device_types.h"
+#include "../host/region.h"
 
 namespace jxgpu {
 
@@ -2148,6 +2149,16 @@ struct FCfg {
   static constexpr int kMinCtas = EPF >= 3 ? 1 : 3;
 };
 
+// The region slicer (host/region.h) selects HF groups from this tile and halo: they must agree for every configuration.
+template <bool GAB, int EPF>
+constexpr bool region_geometry_matches() {
+  return FCfg<GAB, EPF>::H == int(jxg::filter_halo(GAB, EPF)) && kTW == int(jxg::kFilterTileW) && kTH == int(jxg::kFilterTileH);
+}
+static_assert(region_geometry_matches<false, 0>() && region_geometry_matches<false, 1>() && region_geometry_matches<false, 2>() &&
+                  region_geometry_matches<false, 3>() && region_geometry_matches<true, 0>() && region_geometry_matches<true, 1>() &&
+                  region_geometry_matches<true, 2>() && region_geometry_matches<true, 3>(),
+              "host/region.h filter_halo / kFilterTileW / kFilterTileH differ from the fused filter kernel");
+
 // Cell -> source position. INTERIOR tiles (window fully inside the image) skip every range / mirror computation.
 template <bool INTERIOR, int WW>
 __device__ __forceinline__ bool cell_source(int lx, int ly, int wx0, int wy0, int w, int h, int r, int& o, int& mx, int& my) {
@@ -2421,12 +2432,16 @@ __device__ __forceinline__ void filter_tile(const BatchDev& B, const FrameDev& F
     }
   }
   __syncthreads();
-  const int row_bytes = tw * bpp;
-  for (int ly = threadIdx.x >> 5; ly < th; ly += (blockDim.x >> 5)) {  // one warp per row
-    uint8_t* dst = out_base + size_t(y0 + ly) * F.out_row_stride + size_t(x0) * bpp;
-    const uint8_t* srow = stage_u8 + ly * kTW * bpp;
+  // the part of the tile inside the window (the whole tile of a full frame), stored at out + (y - win_y) * stride +
+  // (x - win_x) * bpp
+  const int lx0 = max(int(F.win_x) - x0, 0), lx1 = min(int(F.win_x + F.win_w) - x0, tw);
+  const int ly0 = max(int(F.win_y) - y0, 0), ly1 = min(int(F.win_y + F.win_h) - y0, th);
+  const int row_bytes = (lx1 - lx0) * bpp;
+  for (int ly = ly0 + (threadIdx.x >> 5); ly < ly1; ly += (blockDim.x >> 5)) {  // one warp per row
+    uint8_t* dst = out_base + size_t(y0 + ly - int(F.win_y)) * F.out_row_stride + size_t(x0 + lx0 - int(F.win_x)) * bpp;
+    const uint8_t* srow = stage_u8 + (ly * kTW + lx0) * bpp;
     const int lane = threadIdx.x & 31;
-    if (((reinterpret_cast<uintptr_t>(dst) | uintptr_t(row_bytes)) & 15) == 0) {
+    if (((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(srow) | uintptr_t(row_bytes)) & 15) == 0) {
       for (int i = lane; i < row_bytes / 16; i += 32) reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(srow)[i];
     } else {
       for (int i = lane; i < row_bytes; i += 32) dst[i] = srow[i];
@@ -2732,11 +2747,26 @@ __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev
         }
       }
       (void)w;
+      // Window-relative position of the quad. A quad fully inside the window at a multiple of 4 pixels from its left
+      // edge (every quad of a full frame) is stored with 16-byte / word stores; any other quad sample by sample, only
+      // its pixels inside the window. Both store the same values.
+      const int qx = gx - int(F.win_x), qy = gy - int(F.win_y);
+      uint8_t* out_row = out_base + size_t(qy) * F.out_row_stride;
+      const bool whole = (qx & 3) == 0 && qx >= 0 && qx + 4 <= int(F.win_w) && unsigned(qy) < F.win_h;
+      auto inside = [&](int i) { return unsigned(qx + i) < F.win_w && unsigned(qy) < F.win_h; };
       if (F.output_format == JXG_FORMAT_RGB_F32) {
-        float* d = reinterpret_cast<float*>(out_base + size_t(gy) * F.out_row_stride) + size_t(gx) * 3;
-        st4(d, make_float4(rgb[0][0], rgb[0][1], rgb[0][2], rgb[1][0]));
-        st4(d + 4, make_float4(rgb[1][1], rgb[1][2], rgb[2][0], rgb[2][1]));
-        st4(d + 8, make_float4(rgb[2][2], rgb[3][0], rgb[3][1], rgb[3][2]));
+        float* d = reinterpret_cast<float*>(out_row) + ptrdiff_t(qx) * 3;
+        if (whole) {
+          st4(d, make_float4(rgb[0][0], rgb[0][1], rgb[0][2], rgb[1][0]));
+          st4(d + 4, make_float4(rgb[1][1], rgb[1][2], rgb[2][0], rgb[2][1]));
+          st4(d + 8, make_float4(rgb[2][2], rgb[3][0], rgb[3][1], rgb[3][2]));
+        } else {
+#pragma unroll
+          for (int i = 0; i < 4; i++)
+            if (inside(i))
+#pragma unroll
+              for (int c = 0; c < 3; c++) d[i * 3 + c] = rgb[i][c];
+        }
         continue;
       }
       uint32_t b8[4][3];
@@ -2747,8 +2777,21 @@ __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev
           const float dth = g_dither[((gy + 13 * c) & 31) * 32 + ((gx + i + 23 * c) & 31)];
           b8[i][c] = uint32_t(__float2int_rn(fminf(fmaxf(fmaf(rgb[i][c], 255.0f, dth), 0.0f), 255.0f)));
         }
-      if (F.output_format == JXG_FORMAT_RGB_U8) {
-        uint32_t* d = reinterpret_cast<uint32_t*>(out_base + size_t(gy) * F.out_row_stride + size_t(gx) * 3);
+      if (!whole) {
+        const int bpp = F.output_format == JXG_FORMAT_RGB_U8 ? 3 : 4;
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+          if (inside(i)) {
+            uint8_t* d = out_row + ptrdiff_t(qx + i) * bpp;
+            if (bpp == 4) *reinterpret_cast<uint32_t*>(d) = b8[i][0] | (b8[i][1] << 8) | (b8[i][2] << 16) | 0xff000000u;
+            else {
+              d[0] = uint8_t(b8[i][0]);
+              d[1] = uint8_t(b8[i][1]);
+              d[2] = uint8_t(b8[i][2]);
+            }
+          }
+      } else if (F.output_format == JXG_FORMAT_RGB_U8) {
+        uint32_t* d = reinterpret_cast<uint32_t*>(out_row + size_t(qx) * 3);
         d[0] = b8[0][0] | (b8[0][1] << 8) | (b8[0][2] << 16) | (b8[1][0] << 24);
         d[1] = b8[1][1] | (b8[1][2] << 8) | (b8[2][0] << 16) | (b8[2][1] << 24);
         d[2] = b8[2][2] | (b8[3][0] << 8) | (b8[3][1] << 16) | (b8[3][2] << 24);
@@ -2758,7 +2801,7 @@ __device__ __forceinline__ void filter_tile_v4(const BatchDev& B, const FrameDev
         v.y = b8[1][0] | (b8[1][1] << 8) | (b8[1][2] << 16) | 0xff000000u;
         v.z = b8[2][0] | (b8[2][1] << 8) | (b8[2][2] << 16) | 0xff000000u;
         v.w = b8[3][0] | (b8[3][1] << 8) | (b8[3][2] << 16) | 0xff000000u;
-        *reinterpret_cast<uint4*>(out_base + size_t(gy) * F.out_row_stride + size_t(gx) * 4) = v;
+        *reinterpret_cast<uint4*>(out_row + size_t(qx) * 4) = v;
       }
     }
   }
@@ -2782,9 +2825,8 @@ __device__ __forceinline__ TileRef locate_tile(const BatchDev& B, const FusedTil
   if ((F.gab != 0) != GAB || int(min(F.epf_iters, 3u)) != EPF) return r;  // another instantiation handles this frame
   r.mine = true;
   const uint32_t local = tile_id - T.tile_prefix[lo];
-  const uint32_t tiles_x = (F.width + kTW - 1) / kTW;
-  r.x0 = int(local % tiles_x) * kTW;
-  r.y0 = int(local / tiles_x) * kTH;
+  r.x0 = int(F.win_tx0 + local % F.win_ntx) * kTW;
+  r.y0 = int(F.win_ty0 + local / F.win_ntx) * kTH;
   const bool interior = r.x0 - C::H >= 0 && r.y0 - C::H >= 0 && r.x0 + kTW + C::H <= int(F.width) && r.y0 + kTH + C::H <= int(F.height);
   // 16-byte accesses need an aligned output row (RGB8: stride and base multiples of 4, f32 / RGBA: of 16)
   const uintptr_t oa = reinterpret_cast<uintptr_t>(F.out_ptr) | uintptr_t(F.out_row_stride);
@@ -2867,6 +2909,7 @@ __global__ void __launch_bounds__(256) k_orient(const uint8_t* src, size_t src_s
 #include "launch.h"
 
 namespace jxgpu {
+static_assert(kFusedTileW == kTW && kFusedTileH == kTH, "launch.h tile size differs from the fused filter kernel");
 
 cudaError_t upload_constants(const float* wc, const float* rdct_scale) {
   cudaError_t e = cudaMemcpyToSymbol(c_wc, wc, sizeof(float) * 9 * 128);

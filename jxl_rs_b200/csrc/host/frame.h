@@ -13,6 +13,7 @@
 #include "entropy.h"
 #include "headers.h"
 #include "modular.h"
+#include "region.h"
 
 namespace jxg {
 
@@ -89,6 +90,9 @@ struct FrameState {
   // Section table for the HF groups (pass-major), offsets into codestream.
   std::vector<uint64_t> hf_off;
   std::vector<uint32_t> hf_len;
+
+  // the sub-frame jxg_parsed_region_desc handed out last (its pointers stay valid until the next call)
+  std::unique_ptr<RegionSlice> region_tap;
 
   size_t num_ac_contexts() const { return size_t(num_block_contexts) * (37 + 458); }
   void fill_desc(JxgFrameDesc* d, uint32_t output_format);

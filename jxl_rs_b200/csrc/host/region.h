@@ -1,0 +1,47 @@
+// Region decode of a VarDCT frame: the one place that decides which HF groups a display rectangle needs.
+// A region becomes a sub-frame — a self-contained JxgFrameDesc + section list over a rectangle of whole 256x256 groups
+// — and a window of that sub-frame to store. The sub-frame decode equals the full decode on the region because
+// * every pixel depends only on IDCT pixels within the filter halo H (Gaborish 1, EPF 2 / +1 / +3), and the sub-frame
+//   holds all of them or shares the frame edge they are mirrored at;
+// * its origin is a multiple of 256, which keeps the phase of everything tied to coordinates: 8x8 blocks, 64x64 CfL
+//   tiles, the 32x32 dither table and the 64x32 filter tiles;
+// * with Gaborish + EPF 2 (the only configuration with a vector filter path) the halo is taken around the filter tiles
+//   that meet the region, so that each of them is interior in the sub-frame exactly when it is interior in the frame and
+//   takes the same path.
+#pragma once
+#include <cstdint>
+#include <vector>
+
+#include "../../../include/jxg.h"
+
+namespace jxg {
+
+struct RegionSlice {
+  JxgFrameDesc desc;                     // the sub-frame; its table pointers point into the vectors below
+  std::vector<uint64_t> sec_off;         // sections of the sub-frame (pass-major, sub-frame group order)
+  std::vector<uint32_t> sec_len;
+  std::vector<uint32_t> real_group;      // sub-frame group -> group of the full frame
+  uint32_t origin[2];                    // coded origin of the sub-frame in the frame (multiples of 256)
+  uint32_t coded_win[4];                 // the region in the sub-frame's coded coordinates: x, y, width, height
+  uint32_t window[2];                    // the region's top-left in the sub-frame's display-oriented output
+  std::vector<float> lf[3];
+  std::vector<uint8_t> transform_map, epf_map, quant_lf;
+  std::vector<int32_t> raw_quant_map;
+  std::vector<int8_t> ytox_map, ytob_map;
+};
+
+// Geometry of the fused filter kernel the selection depends on: its 64x32 tile (kTW x kTH, launch.h kFusedTileW / H)
+// and its halo in pixels, Gaborish 1 + EPF 2 / +1 / +3 (FCfg<GAB, EPF>::H). kernels.cu checks both against the kernel's
+// own constants at compile time.
+constexpr uint32_t kFilterTileW = 64, kFilterTileH = 32;
+constexpr uint32_t filter_halo(bool gab, uint32_t epf_iters) {
+  return (gab ? 1 : 0) + (epf_iters >= 1 ? 2 : 0) + (epf_iters >= 2 ? 1 : 0) + (epf_iters >= 3 ? 3 : 0);
+}
+
+// Slices `full` (and its n_sections sections) to the region r, given in display coordinates (the frame's orientation
+// applied; XYB output has none). Returns 0, or JXG_ERR_ARGUMENT with *why set when the region is empty or leaves the
+// image, or the output format is XYB_F32_PLANAR.
+int slice_region(const JxgFrameDesc& full, const uint64_t* sec_off, const uint32_t* sec_len, uint32_t n_sections,
+                 const JxgRegion& r, RegionSlice* out, const char** why);
+
+}  // namespace jxg

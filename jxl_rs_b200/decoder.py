@@ -58,10 +58,32 @@ class ParsedFrame:
                                                        C.byref(ln), C.byref(n)))
         return d, hf, off, ln, n.value
 
+    def region_desc(self, output_format, region):
+        """The sub-frame a region (x, y, w, h in output coordinates) decodes (jxg_parsed_region_desc): (desc, hf, off,
+        len, n_sections, origin, window); origin is the sub-frame's coded top-left, window the region's top-left in
+        the sub-frame's display-oriented output. Valid until the next call on this frame."""
+        d = abi.JxgFrameDesc()
+        hf, off, ln, n = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_uint32()
+        origin, window = (C.c_uint32 * 2)(), (C.c_uint32 * 2)()
+        abi.check(self._lib, self._lib.jxg_parsed_region_desc(self._h, output_format, C.byref(_region(region)), C.byref(d),
+                                                              C.byref(hf), C.byref(off), C.byref(ln), C.byref(n),
+                                                              origin, window))
+        return d, hf, off, ln, n.value, tuple(origin), tuple(window)
+
     def __del__(self):
         if getattr(self, "_h", None) and self._h.value:
             self._lib.jxg_parsed_free(self._h)
             self._h = C.c_void_p()
+
+
+def _region(region):
+    x, y, w, h = (int(v) for v in region)
+    return abi.JxgRegion(x, y, w, h)
+
+
+def _out_size(frame, region):
+    """(height, width) of the output of a frame, or of a region (x, y, w, h) of it."""
+    return (frame.height, frame.width) if region is None else (int(region[3]), int(region[2]))
 
 
 class JxgContext:
@@ -134,9 +156,15 @@ class Batch(_BatchHandle):
         if staging_threads > 0:
             abi.check(self._lib, self._lib.jxg_batch_set_deferred_copy(self._h, staging_threads))
 
-    def add(self, frame: ParsedFrame, out_ptr: int, row_stride: int, fmt: int, out_is_device: bool):
-        abi.check(self._lib, self._lib.jxg_batch_add_parsed(self._h, frame._h, fmt, C.c_void_p(out_ptr), row_stride,
-                                                            1 if out_is_device else 0))
+    def add(self, frame: ParsedFrame, out_ptr: int, row_stride: int, fmt: int, out_is_device: bool, region=None):
+        """region: None for the whole frame, or (x, y, w, h) in output coordinates: only that rectangle is decoded
+        and stored, into a buffer of h rows of w pixels (jxg_batch_add_parsed_region)."""
+        dev = 1 if out_is_device else 0
+        if region is None:
+            abi.check(self._lib, self._lib.jxg_batch_add_parsed(self._h, frame._h, fmt, C.c_void_p(out_ptr), row_stride, dev))
+        else:
+            abi.check(self._lib, self._lib.jxg_batch_add_parsed_region(self._h, frame._h, fmt, C.byref(_region(region)),
+                                                                       C.c_void_p(out_ptr), row_stride, dev))
         self.frames.append(frame)
 
     def add_desc(self, desc, hf, off, ln, n, out_ptr, row_stride, out_is_device):
@@ -197,9 +225,12 @@ class Batch(_BatchHandle):
         return out.reshape(3, pr, ps)
 
 
-def decode_files(ctx: JxgContext, files, pixel_format: JxlPixelFormat = JxlPixelFormat(), to_host: bool = True):
+def decode_files(ctx: JxgContext, files, pixel_format: JxlPixelFormat = JxlPixelFormat(), to_host: bool = True,
+                 regions=None):
     """Decodes a list of .jxl byte strings; returns a list of torch tensors
-    (H x W x C). Host results land in pinned memory (JxlOutputBuffer analogue)."""
+    (H x W x C). Host results land in pinned memory (JxlOutputBuffer analogue).
+    regions: None, or one entry per file: None (the whole image) or (x, y, w, h) in output coordinates, which decodes
+    only that rectangle into an h x w x C tensor."""
     import torch
     fmt = pixel_format.abi_format()
     cpus = effective_cpus()
@@ -210,18 +241,23 @@ def decode_files(ctx: JxgContext, files, pixel_format: JxlPixelFormat = JxlPixel
             frames = list(ex.map(lambda f: ParsedFrame(f, per_file), files))
     else:
         frames = [ParsedFrame(f, per_file) for f in files]
+    if regions is None:
+        regions = [None] * len(frames)
+    if len(regions) != len(frames):
+        raise ValueError("regions: one entry per file")
     batch = Batch(ctx, len(frames))
     outs = []
     try:  # a corrupt frame must not leave the context with a live batch
-        for fr in frames:
+        for fr, reg in zip(frames, regions):
             ch = 4 if fmt == abi.FORMAT_RGBA_U8 else 3
             dt = {abi.FORMAT_RGB_F32: torch.float32, abi.FORMAT_RGB_U16: torch.uint16, abi.FORMAT_RGB_F16: torch.float16}.get(fmt, torch.uint8)
+            h, w = _out_size(fr, reg)
             if to_host:
-                t = torch.empty((fr.height, fr.width, ch), dtype=dt).pin_memory()
+                t = torch.empty((h, w, ch), dtype=dt).pin_memory()
             else:
-                t = torch.empty((fr.height, fr.width, ch), dtype=dt, device=f"cuda:{ctx.device}")
+                t = torch.empty((h, w, ch), dtype=dt, device=f"cuda:{ctx.device}")
             outs.append(t)
-            batch.add(fr, t.data_ptr(), fr.width * ch * t.element_size(), fmt, not to_host)
+            batch.add(fr, t.data_ptr(), w * ch * t.element_size(), fmt, not to_host, reg)
         batch.run()
         batch.wait()
     finally:
@@ -352,7 +388,7 @@ class PipelinedDecoder:
         if self.trace is not None:  # ("retire", start, event wait, stats + marks, close)
             self.retire_trace.append((t0, t1 - t0, t2 - t1, time.perf_counter() - t2))
 
-    def _launch(self, futs, outs, fmt, out_is_device):
+    def _launch(self, futs, outs, fmt, out_is_device, regions):
         import time
         t0 = time.perf_counter()
         if len(self.inflight) == self.depth:
@@ -366,8 +402,11 @@ class PipelinedDecoder:
         try:
             frames = [fut.result() for fut in futs]
             t2 = time.perf_counter()
-            for fr, (ptr, stride) in zip(frames, outs):
-                b.add(fr, ptr, stride, fmt, out_is_device)
+            for fr, (ptr, stride), reg in zip(frames, outs, regions):
+                if reg is None:  # the five-argument call whole frames always made (stand-in batches implement only it)
+                    b.add(fr, ptr, stride, fmt, out_is_device)
+                else:
+                    b.add(fr, ptr, stride, fmt, out_is_device, reg)
             t3 = time.perf_counter()
             b.run()
         except Exception:
@@ -401,14 +440,19 @@ class PipelinedDecoder:
             finally:
                 self._jobs.task_done()
 
-    def submit(self, files, outs, fmt: int = abi.FORMAT_RGB_U8, out_is_device: bool = False):
+    def submit(self, files, outs, fmt: int = abi.FORMAT_RGB_U8, out_is_device: bool = False, regions=None):
         """files: list of .jxl byte strings; outs: list of (data_ptr, row_stride). Returns once the batch is
-        queued; its outputs are complete after drain() (or once `depth` later batches have been launched)."""
+        queued; its outputs are complete after drain() (or once `depth` later batches have been launched).
+        regions: None, or one entry per file: None (the whole image) or (x, y, w, h), the output rectangle that is
+        decoded into that file's buffer."""
+        regions = [None] * len(files) if regions is None else list(regions)
+        if len(regions) != len(files):
+            raise ValueError("regions: one entry per file")
         self._ahead.acquire()
         # fewer files than workers (one large image): the spare workers decode LF groups inside each file
         per_file = max(1, self.workers // max(1, len(files)))
         futs = [self.pool.submit(ParsedFrame, f, per_file) for f in files]
-        self._jobs.put((futs, list(outs), fmt, out_is_device))
+        self._jobs.put((futs, list(outs), fmt, out_is_device, regions))
 
     def drain(self):
         import threading
@@ -419,8 +463,8 @@ class PipelinedDecoder:
             e, self._error = self._error, None
             raise e
 
-    def decode(self, files, outs, fmt: int = abi.FORMAT_RGB_U8, out_is_device: bool = False):
-        self.submit(files, outs, fmt, out_is_device)
+    def decode(self, files, outs, fmt: int = abi.FORMAT_RGB_U8, out_is_device: bool = False, regions=None):
+        self.submit(files, outs, fmt, out_is_device, regions)
         self.drain()
 
     def close(self):
