@@ -700,6 +700,10 @@ __global__ void __launch_bounds__(128, 6) k_entropy_lean(const BatchDev B) {
   const uint32_t* const ucfg = reinterpret_cast<const uint32_t*>(B.blob + P.code.cfg_off);
   const uint2* const ans = reinterpret_cast<const uint2*>(B.blob + P.code.ans_off);
   const uint32_t log_alpha = P.code.log_alpha, log_bucket = 12 - P.code.log_alpha, bucket_mask = (1u << (12 - P.code.log_alpha)) - 1;
+  // Coefficient orders: read once here, not by every channel's set-up (the stores of the loop keep the compiler from
+  // hoisting the loads of P itself).
+  const bool custom_orders = P.custom_orders != 0;
+  const uint32_t* const order_base = custom_orders ? reinterpret_cast<const uint32_t*>(B.blob + P.order_off) : B.natural_orders;
   // ---- per-stream state (re-initialised by the set-up path when a lane takes a new stream) ----
   uint32_t gsid = 0, nblk = 0, bi = 0;
   const uint4* desc = B.desc;
@@ -796,10 +800,9 @@ __global__ void __launch_bounds__(128, 6) k_entropy_lean(const BatchDev B) {
       if (!done) {
         const int c = ci == 0 ? 1 : (ci == 1 ? 0 : 2);  // Y, X, B
         const uint8_t* nzc_col = nz + c * 32;
-        uint32_t predicted;
-        if (bx == 0) predicted = by == 0 ? 32u : nzc_col[0];
-        else if (by == 0) predicted = nzc_col[bx - 1];
-        else predicted = (uint32_t(nzc_col[bx]) + uint32_t(nzc_col[bx - 1]) + 1u) >> 1;
+        // both neighbours read, the prediction selected: no branches inside the (divergent) set-up path
+        const uint32_t up = nzc_col[bx], left = nzc_col[bx ? bx - 1 : 0];
+        const uint32_t predicted = bx == 0 ? (by == 0 ? 32u : up) : (by == 0 ? left : (up + left + 1u) >> 1);
         block_context = (bctx3 >> (8 * ci)) & 0xff;
         const uint32_t nzc = predicted < 8 ? predicted : (predicted < 64 ? 4 + predicted / 2 : 36);
         cluster = ctx_cluster(nzc * nbc + block_context + context_offset);
@@ -876,11 +879,11 @@ __global__ void __launch_bounds__(128, 6) k_entropy_lean(const BatchDev B) {
       uint8_t* nzc_col = nz + c * 32;
       const uint8_t nzv = uint8_t((nonzeros + num_blocks - 1) >> lnb);
       const uint32_t cx = cxy & 0xff;
-      for (uint32_t ix = 0; ix < cx; ix++) nzc_col[bx + ix] = nzv;
+#pragma unroll 1
+      for (uint32_t ix = 0; ix < cx; ix++) nzc_col[bx + ix] = nzv;  // a rolled loop: most varblocks are one block wide
       histo_offset = nbc * 37 + 458 * block_context + context_offset;
       k = num_blocks;
-      order = P.custom_orders ? reinterpret_cast<const uint32_t*>(B.blob + P.order_off) + P.order_offset[shape * 3 + c]
-                              : B.natural_orders + s_order_off[shape];
+      order = order_base + (custom_orders ? P.order_offset[shape * 3 + c] : s_order_off[shape]);
       list[kOffBase + (bi - 1) * 3 + ci] = nlist;  // first entry of this varblock's channel ci (Y, X, B)
       mode_nnz = false;
       if (nonzeros == 0) {
