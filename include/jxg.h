@@ -167,6 +167,14 @@ void jxg_shutdown(void* ctx);
  * NULL context or a byte outside -1..255. */
 int jxg_context_set_pool_fill(void* ctx, int byte);
 
+/* Test hook, off by default: with n >= 1 every scheduling decision of the context's later batches (VarDCT and Modular)
+ * takes n in place of the device's SM count: the lean entropy kernel's lanes per warp, lanes per frame and queued
+ * streams, the fast entropy kernel's streams per warp, the Modular decode grid and the grid-stride grids of the Modular
+ * transforms. n = 0 restores the device's own count. Outputs do not depend on it, only which schedule produces them:
+ * a small n reaches the queued streams and wide warps of very large batches with small ones. JXG_ERR_ARGUMENT for a
+ * NULL context or a negative n. */
+int jxg_context_set_sm_budget(void* ctx, int n);
+
 /* Batch of frames decoded together (one kernel pipeline over all groups of
  * all frames). Replaces N calls of decode_and_render_hf_groups. */
 int jxg_batch_begin(void* ctx, uint32_t n_frames_hint, void** batch);
@@ -235,6 +243,22 @@ int jxg_batch_stats(void* batch, uint64_t* kernel_launches, uint64_t* h2d_bytes,
  * schedule (4 or 8), 0 before jxg_batch_run or without lean streams. Any pointer may be NULL. */
 int jxg_batch_entropy_stats(void* batch, uint32_t* n_lean, uint32_t* n_fast, uint32_t* n_slow, int* lean_all_420,
                             int* lean_ctx_smem, uint32_t* lean_S);
+
+/* The entropy schedule of the last jxg_batch_run. For frame f: its lean streams (lean_count), the lanes that start on
+ * them (lean_lanes; the other lean_count - lean_lanes streams are queued and taken by whichever of the frame's lanes
+ * ends first) and its CTAs of k_entropy_lean. With f = JXG_ALL_FRAMES: the batch's lean streams, the sum of the lanes
+ * and the grid k_entropy_lean is launched with. fast_S: streams per warp of k_entropy_fast (1, 2, 4 or 8; 0 without
+ * such streams). lean_pulls (waits for the last run): how often the frame's lanes pulled from its stream queue, once
+ * per queued stream and once more per lane when the queue was empty, so lean_count when every queued stream was
+ * taken exactly once. JXG_ERR_ARGUMENT before jxg_batch_run or for a frame out of range. Any output pointer may be
+ * NULL. */
+#define JXG_ALL_FRAMES 0xffffffffu
+int jxg_batch_entropy_schedule(void* batch, uint32_t f, uint32_t* lean_count, uint32_t* lean_lanes, uint32_t* lean_ctas,
+                               uint32_t* fast_S, uint32_t* lean_pulls);
+/* The status word of each group of frame f after the last run (0, or the JXG_ERR_* its entropy stream or block plan
+ * ended with; groups of a region frame are those of its sub-frame), out[0 .. num_groups). Waits for the last run.
+ * JXG_ERR_ARGUMENT before jxg_batch_run, for a frame out of range or when n < the frame's group count. */
+int jxg_batch_stream_status(void* batch, uint32_t f, int32_t* out, uint32_t n);
 
 /* ---------------- convenience front-end (host parse + batch) ----------------
  * Parses complete .jxl files (container or bare codestream) on the host with

@@ -68,6 +68,7 @@ struct Batch : BatchCore {
   bool lean_all_420 = true;
   bool lean_ctx_smem = true;  // every lean frame's context map (+64 spill) fits k_entropy_lean's 16 KB staging area
   uint32_t lean_S = 1, lean_ctas = 0;  // k_entropy_lean schedule (see schedule_lean)
+  uint32_t fast_S = 0;                 // streams per warp of k_entropy_fast (see schedule_fast), 0: no such streams
   std::vector<uint32_t> lean_cta_first;
   std::vector<uint2> lean_warps;  // per warp of k_entropy_lean: first stream (relative to its frame's list), lanes
   std::vector<uint32_t> fused_prefix{0};
@@ -252,6 +253,13 @@ int jxg_context_set_pool_fill(void* c, int byte) {
   Context* cx = static_cast<Context*>(c);
   if (!cx || byte < -1 || byte > 255) return set_error(JXG_ERR_ARGUMENT, "pool fill: a context and a byte in -1..255");
   cx->pool_fill = byte;
+  return JXG_OK;
+}
+
+int jxg_context_set_sm_budget(void* c, int n) {
+  Context* cx = static_cast<Context*>(c);
+  if (!cx || n < 0) return set_error(JXG_ERR_ARGUMENT, "SM budget: a context and a count >= 0");
+  cx->sm_budget = n;
   return JXG_OK;
 }
 
@@ -614,7 +622,7 @@ static void schedule_lean(Batch* b) {
   }
   // The kernel keeps 6 CTAs per SM resident (register bound); a grid beyond one resident wave would start its last
   // CTAs only when the first ones end, so the packing is made denser until the grid fits.
-  const uint32_t max_ctas = uint32_t(sm_count()) * 6;
+  const uint32_t max_ctas = schedule_sms(b->ctx) * 6;
   // 4 lanes per warp are the fastest schedule for a batch that has the device to itself; 8 lanes halve the kernel's
   // warp-instructions, which is what counts once several batches share the SMs (on 64 x 4K frames 8 lanes lose alone and
   // win with three or more resident batches; 16 and 32 lanes lose again). Three or more live contexts on the device are taken as "batches share the SMs".
@@ -624,6 +632,7 @@ static void schedule_lean(Batch* b) {
   for (int attempt = 0; attempt < 12; attempt++) {
     warps.clear();
     uint32_t ctas = 0;
+    bool one_cta_each = true;  // every frame with lean streams is down to one CTA
     for (size_t f = 0; f < nf; f++) {
       FrameDev& F = b->frames[f];
       F.lean_cta_first = ctas;
@@ -637,9 +646,12 @@ static void schedule_lean(Batch* b) {
       F.lean_lanes = lanes;
       F.lean_ctas = uint32_t(warps.size() - w0) / 4;
       ctas += F.lean_ctas;
+      one_cta_each &= F.lean_ctas == 1;
     }
     b->lean_ctas = ctas;
-    if (ctas <= max_ctas) break;
+    // A frame never shares a CTA, so with one CTA per frame the grid cannot shrink: denser packing would only queue
+    // streams behind lanes that fit already.
+    if (ctas <= max_ctas || one_cta_each) break;
     // denser: first 8 lanes per warp, then more streams per lane
     if (S < 8) S = 8;
     else per_lane *= 1.3f;
@@ -648,6 +660,14 @@ static void schedule_lean(Batch* b) {
   b->lean_warps = std::move(warps);
   b->lean_cta_first.assign(nf, 0);
   for (size_t f = 0; f < nf; f++) b->lean_cta_first[f] = b->frames[f].lean_cta_first;
+}
+
+// Streams per warp of k_entropy_fast (1, 2, 4 or 8): the fewest that keep the grid within about one resident wave of
+// 16 warps per SM (4 schedulers x 4 warps).
+static void schedule_fast(Batch* b) {
+  const uint32_t n = uint32_t(b->streams_fast.size()), wave = schedule_sms(b->ctx) * 16;
+  const uint32_t per = (n + wave - 1) / wave;
+  b->fast_S = n == 0 ? 0 : per <= 1 ? 1 : per <= 2 ? 2 : per <= 4 ? 4 : 8;
 }
 
 static BatchDev make_batch_dev(Batch* b) {
@@ -686,7 +706,8 @@ static BatchDev make_batch_dev(Batch* b) {
 static int launch(Batch* b, cudaStream_t s, bool copy_to_host) {
   const BatchDev B = make_batch_dev(b);
   cudaEvent_t* ev = b->profile ? b->stage_ev : nullptr;
-  b->launches = uint64_t(launch_pipeline(B, s, b->debug_stop, ev, b->lean_all_420, b->lean_S, b->lean_ctas, b->lean_ctx_smem));
+  b->launches =
+      uint64_t(launch_pipeline(B, s, b->debug_stop, ev, b->lean_all_420, b->lean_S, b->lean_ctas, b->lean_ctx_smem, b->fast_S));
   if (b->debug_stop == 0) {
     // Fused filter + colour + store, launched per range of frames; each finished range is copied to the host on the
     // device's D2H stream while the next range is being filtered.
@@ -757,6 +778,7 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
   cudaStream_t s = batch_stream(*b, cuda_stream);
   b->h2d = b->d2h = 0;
   schedule_lean(b);
+  schedule_fast(b);
   // device allocations
   // one coefficient list per HF section (pass x group), worst-case capacity (every coefficient non-zero)
   if (int r = b->d_coeffs.ensure(b->sections.size() * size_t(kListStride) * 4)) return r;
@@ -773,7 +795,8 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
     if (fo.orientation != 1) b->frames[f].out_ptr = static_cast<uint8_t*>(b->ctx->d_orient.p) + fo.stage_off;
     else b->frames[f].out_ptr = fo.is_device ? fo.user_ptr : static_cast<uint8_t*>(b->d_out.p) + fo.dev_off;
   }
-  if (int r = batch_status(*b, b->streams.size())) return r;
+  // the status word of each stream, then k_entropy_lean's queue counter of each frame (jxg_batch_entropy_schedule)
+  if (int r = batch_status(*b, b->streams.size() + b->frames.size())) return r;
   if (!batch_table(b->blob, b->frames, b->tab.frames) || !batch_table(b->blob, b->sections, b->tab.sections) ||
       !batch_table(b->blob, b->streams, b->tab.streams) || !batch_table(b->blob, b->lean_cta_first, b->tab.lean_cta) ||
       !batch_table(b->blob, b->lean_warps, b->tab.lean_warp) || !batch_table(b->blob, b->streams_lean, b->tab.streams_lean) ||
@@ -870,6 +893,46 @@ int jxg_batch_entropy_stats(void* bp, uint32_t* n_lean, uint32_t* n_fast, uint32
   if (lean_all_420) *lean_all_420 = b->lean_all_420 ? 1 : 0;
   if (lean_ctx_smem) *lean_ctx_smem = b->lean_ctx_smem ? 1 : 0;
   if (lean_S) *lean_S = b->lean_ctas ? b->lean_S : 0;
+  return JXG_OK;
+}
+
+int jxg_batch_entropy_schedule(void* bp, uint32_t f, uint32_t* lean_count, uint32_t* lean_lanes, uint32_t* lean_ctas,
+                               uint32_t* fast_S, uint32_t* lean_pulls) {
+  Batch* b = static_cast<Batch*>(bp);
+  if (!b || !b->uploaded || (f >= b->frames.size() && f != JXG_ALL_FRAMES)) return JXG_ERR_ARGUMENT;
+  const size_t nf = b->frames.size();
+  if (lean_pulls)
+    if (int r = batch_wait_last_run(*b)) return r;
+  // the queue counters follow the status words; they are cleared by the run only when it has lean streams
+  auto pulls = [&](size_t i) { return b->lean_ctas ? uint32_t(b->status_host[b->streams.size() + i]) : 0u; };
+  uint32_t count = 0, lanes = 0, ctas = 0, taken = 0;
+  if (f == JXG_ALL_FRAMES) {
+    count = uint32_t(b->streams_lean.size());
+    for (size_t i = 0; i < nf; i++) {
+      lanes += b->frames[i].lean_lanes;
+      taken += pulls(i);
+    }
+    ctas = b->lean_ctas;  // the launched grid
+  } else {
+    count = b->frames[f].lean_count;
+    lanes = b->frames[f].lean_lanes;
+    ctas = b->frames[f].lean_ctas;
+    taken = pulls(f);
+  }
+  if (lean_count) *lean_count = count;
+  if (lean_lanes) *lean_lanes = lanes;
+  if (lean_ctas) *lean_ctas = ctas;
+  if (fast_S) *fast_S = b->fast_S;
+  if (lean_pulls) *lean_pulls = taken;
+  return JXG_OK;
+}
+
+int jxg_batch_stream_status(void* bp, uint32_t f, int32_t* out, uint32_t n) {
+  Batch* b = static_cast<Batch*>(bp);
+  if (!b || !out || !b->uploaded || f >= b->frames.size() || n < b->frames[f].num_groups) return JXG_ERR_ARGUMENT;
+  if (int r = batch_wait_last_run(*b)) return r;
+  const FrameDev& F = b->frames[f];
+  memcpy(out, b->status_host + F.first_stream, size_t(F.num_groups) * 4);
   return JXG_OK;
 }
 

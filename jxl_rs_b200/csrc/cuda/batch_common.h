@@ -13,6 +13,8 @@
 #include "../../../include/jxg.h"
 
 namespace jxgpu {
+int sm_count();  // kernels.cu
+
 namespace detail {
 
 extern thread_local std::string g_error;
@@ -133,12 +135,18 @@ struct Context {
   DevBuf d_blob, d_coeffs, d_block_off, d_planes_a, d_status, d_out, d_desc, d_nblk, d_orient, d_lzwin,
       d_modular_lzwin, d_modular_wp;
   int pool_fill = -1;  // test hook (jxg_context_set_pool_fill): byte written over the pools before each run, -1: off
+  int sm_budget = 0;   // test hook (jxg_context_set_sm_budget): SMs every schedule of the context assumes, 0: the device's
   bool batch_live = false;
   // pinned status readback buffer, owned by the context: cudaHostAlloc / cudaFreeHost synchronise the whole
   // device, so they must not happen per batch when batches of several contexts are in flight
   int32_t* status_host = nullptr;
   size_t status_cap = 0;
 };
+
+// SMs the launch schedules of the context's batches are sized for: the device's count, or the test hook's budget.
+inline uint32_t schedule_sms(const Context* cx) {
+  return cx->sm_budget > 0 ? uint32_t(cx->sm_budget) : uint32_t(sm_count());
+}
 
 // What a batch of either engine holds besides its frames. ev0: before the upload; ev1: behind everything of the last run.
 struct BatchCore {
@@ -206,10 +214,11 @@ inline int batch_status(BatchCore& b, size_t n) {
   return 0;
 }
 
-// The first non-zero status word as the batch's error: "<what><frame> group <group>" of the stream it belongs to.
+// The first non-zero status word of a stream as the batch's error: "<what><frame> group <group>" of that stream. The
+// words after the streams' (status_n may count more) are not statuses.
 template <typename Stream>
 int batch_first_failure(const BatchCore& b, const std::vector<Stream>& streams, const char* what, uint32_t* frame, uint32_t* group) {
-  for (size_t i = 0; i < b.status_n; i++)
+  for (size_t i = 0; i < std::min(b.status_n, streams.size()); i++)
     if (b.status_host[i] != 0) {
       if (frame) *frame = streams[i].frame;
       if (group) *group = streams[i].group;

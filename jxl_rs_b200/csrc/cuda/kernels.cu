@@ -2937,7 +2937,7 @@ cudaError_t configure_kernels() {
 }
 
 int launch_pipeline(const BatchDev& B, cudaStream_t stream, int debug_stop, cudaEvent_t* ev, bool lean_all_420,
-                    uint32_t lean_S, uint32_t lean_ctas, bool lean_ctx_smem) {
+                    uint32_t lean_S, uint32_t lean_ctas, bool lean_ctx_smem, uint32_t fast_S) {
   // ev (optional, kNumStages + 1 events): ev[i] is recorded before stage i, ev[i+1] after it; stages that do not
   // run record nothing (the host pairs consecutive recorded events).
   int launches = 0;
@@ -2971,11 +2971,10 @@ int launch_pipeline(const BatchDev& B, cudaStream_t stream, int debug_stop, cuda
     launches++;
   }
   if (B.num_fast) {
-    // streams per warp: aim at about one resident wave (592 schedulers x ~4 warps)
-    const uint32_t per = (B.num_fast + 2367) / 2368;
-    if (per <= 1) k_entropy_fast<1><<<(B.num_fast + 3) / 4, 128, 0, stream>>>(B);
-    else if (per <= 2) k_entropy_fast<2><<<(B.num_fast + 7) / 8, 128, 0, stream>>>(B);
-    else if (per <= 4) k_entropy_fast<4><<<(B.num_fast + 15) / 16, 128, 0, stream>>>(B);
+    // streams per warp chosen by the host (batch.cc schedule_fast): about one resident wave of warps
+    if (fast_S <= 1) k_entropy_fast<1><<<(B.num_fast + 3) / 4, 128, 0, stream>>>(B);
+    else if (fast_S == 2) k_entropy_fast<2><<<(B.num_fast + 7) / 8, 128, 0, stream>>>(B);
+    else if (fast_S == 4) k_entropy_fast<4><<<(B.num_fast + 15) / 16, 128, 0, stream>>>(B);
     else k_entropy_fast<8><<<(B.num_fast + 31) / 32, 128, 0, stream>>>(B);
     launches++;
   }

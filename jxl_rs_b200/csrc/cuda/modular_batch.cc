@@ -486,7 +486,8 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
     if (f.host_planes_elems)
       CUDA_TRY(cudaMemcpyAsync(B.planes + f.arena_base, B.blob + f.host_planes_blob, f.host_planes_elems * 4,
                                cudaMemcpyDeviceToDevice, s));
-  b->launches = uint64_t(launch_modular_decode(B, b->num_plain, b->lanes_per_warp, uint32_t(b->rct_streams.size()), s));
+  b->launches = uint64_t(
+      launch_modular_decode(B, b->num_plain, b->lanes_per_warp, uint32_t(b->rct_streams.size()), schedule_sms(cx), s));
   CUDA_TRY(cudaEventRecord(b->ev_decode, s));
   const MJobDev* jobs = reinterpret_cast<const MJobDev*>(B.blob + b->tab.jobs);  // the levels in order, then the stores
   auto launch_jobs = [&](jxg::ModularJobKind kind, const std::vector<MJobDev>& level) {
@@ -495,7 +496,7 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
       mw = std::max(mw, j.w);
       mh = std::max(mh, j.h);
     }
-    launch_modular_jobs(kind, jobs, uint32_t(level.size()), mw, mh, B.planes, s);
+    launch_modular_jobs(kind, jobs, uint32_t(level.size()), mw, mh, B.planes, schedule_sms(cx), s);
     jobs += level.size();
     b->launches++;
   };

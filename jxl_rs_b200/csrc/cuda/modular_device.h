@@ -74,12 +74,14 @@ struct MBatchDev {
 };
 
 // The first num_plain entries of B.order are streams without LZ77, the remaining B.num_streams - num_plain use it: each
-// group is decoded by its own launch of k_modular_decode (B.queue[0] / B.queue[1]), then the local RCTs run.
+// group is decoded by its own launch of k_modular_decode (B.queue[0] / B.queue[1]), then the local RCTs run. `sms`: the SMs
+// the grids are sized for (schedule_sms, batch_common.h): the decode grid is capped at 8 CTAs per SM, the grid-stride
+// job grids at 16.
 int launch_modular_decode(const MBatchDev& B, uint32_t num_plain, uint32_t lanes_per_warp, uint32_t num_rct_streams,
-                          cudaStream_t stream);
+                          uint32_t sms, cudaStream_t stream);
 // kind: a jxg::ModularJobKind (host/modular_frame.h): 0 RCT, 1 horizontal unsqueeze, 2 vertical unsqueeze, 3 store,
 // 4 palette look-up
 void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint32_t max_w, uint32_t max_h, int32_t* planes,
-                         cudaStream_t stream);
+                         uint32_t sms, cudaStream_t stream);
 
 }  // namespace jxgpu

@@ -770,10 +770,10 @@ __global__ void __launch_bounds__(256) k_modular_store(const MJobDev* jobs, cons
 // host-side launchers
 // ---------------------------------------------------------------------------
 template <bool LZ>
-void launch_decode(const MBatchDev& B, uint32_t lanes_per_warp, cudaStream_t stream) {
+void launch_decode(const MBatchDev& B, uint32_t lanes_per_warp, uint32_t sms, cudaStream_t stream) {
   const uint32_t S = lanes_per_warp <= 1 ? 1 : (lanes_per_warp <= 2 ? 2 : 4);
   const uint32_t warps = (B.num_streams + S - 1) / S;
-  const uint32_t grid = min((warps + 3) / 4, uint32_t(sm_count()) * 8u);
+  const uint32_t grid = min((warps + 3) / 4, sms * 8u);
   const uint32_t total_lanes = grid * 4 * S;
   if (S == 1) k_modular_decode<1, LZ><<<grid, 128, 0, stream>>>(B, total_lanes);
   else if (S == 2) k_modular_decode<2, LZ><<<grid, 128, 0, stream>>>(B, total_lanes);
@@ -781,13 +781,13 @@ void launch_decode(const MBatchDev& B, uint32_t lanes_per_warp, cudaStream_t str
 }
 
 int launch_modular_decode(const MBatchDev& B, uint32_t num_plain, uint32_t lanes_per_warp, uint32_t num_rct_streams,
-                          cudaStream_t stream) {
+                          uint32_t sms, cudaStream_t stream) {
   int launches = 0;
   if (B.num_streams) cudaMemsetAsync(B.queue, 0, 2 * sizeof(uint32_t), stream);
   if (num_plain) {
     MBatchDev P = B;
     P.num_streams = num_plain;
-    launch_decode<false>(P, lanes_per_warp, stream);
+    launch_decode<false>(P, lanes_per_warp, sms, stream);
     launches++;
   }
   if (B.num_streams > num_plain) {  // longest first among the LZ77 streams too, with their own queue counter
@@ -795,7 +795,7 @@ int launch_modular_decode(const MBatchDev& B, uint32_t num_plain, uint32_t lanes
     L.order = B.order + num_plain;
     L.num_streams = B.num_streams - num_plain;
     L.queue = B.queue + 1;
-    launch_decode<true>(L, lanes_per_warp, stream);
+    launch_decode<true>(L, lanes_per_warp, sms, stream);
     launches++;
   }
   if (num_rct_streams) {
@@ -860,20 +860,20 @@ __global__ void __launch_bounds__(256) k_modular_palette(const MJobDev* jobs, in
 }
 
 void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint32_t max_w, uint32_t max_h, int32_t* planes,
-                         cudaStream_t stream) {
+                         uint32_t sms, cudaStream_t stream) {
   if (!num_jobs) return;
   if (kind == 0) {
-    const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sm_count()) * 16));
+    const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sms) * 16));
     k_modular_rct<<<dim3(max(gx, 1u), num_jobs), 256, 0, stream>>>(jobs, planes);
   } else if (kind == 1) {  // a level can hold only empty channels (a squeeze of a zero-height residual): one idle block
     k_unsqueeze_h<<<dim3(max((max_h + 127) / 128, 1u), num_jobs), 128, 0, stream>>>(jobs, planes);
   } else if (kind == 2) {
     k_unsqueeze_v<<<dim3(max((max_w + 127) / 128, 1u), num_jobs), 128, 0, stream>>>(jobs, planes);
   } else if (kind == 4) {
-    const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sm_count()) * 16));
+    const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sms) * 16));
     k_modular_palette<<<dim3(max(gx, 1u), num_jobs), 256, 0, stream>>>(jobs, planes);
   } else {
-    const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sm_count()) * 16));
+    const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sms) * 16));
     k_modular_store<<<dim3(max(gx, 1u), num_jobs), 256, 0, stream>>>(jobs, planes);
   }
 }

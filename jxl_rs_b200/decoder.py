@@ -101,6 +101,12 @@ class JxgContext:
         there; -1 (the default) turns it off. Each begin, run and rerun uses the byte in force when it is called."""
         abi.check(self._lib, self._lib.jxg_context_set_pool_fill(self._h, int(byte)))
 
+    def set_sm_budget(self, n: int):
+        """Test hook (jxg_context_set_sm_budget): with n >= 1 the context's later batches are scheduled as if the device
+        had n SMs (entropy lanes per warp and per frame, queued streams, Modular grids); 0 (the default) uses the
+        device's own count. Outputs do not depend on it."""
+        abi.check(self._lib, self._lib.jxg_context_set_sm_budget(self._h, int(n)))
+
     def close(self):
         if self._h.value:
             self._lib.jxg_shutdown(self._h)
@@ -210,6 +216,31 @@ class Batch(_BatchHandle):
                                                                C.byref(a420), C.byref(smem), C.byref(s)))
         return {"lean": nl.value, "fast": nf.value, "slow": ns.value, "lean_all_420": bool(a420.value),
                 "lean_ctx_smem": bool(smem.value), "lean_S": s.value}
+
+    def entropy_schedule(self):
+        """The entropy schedule of the last run() (jxg_batch_entropy_schedule): the lean kernel's lanes per warp
+        ("lean_S", 0 without lean streams) and grid ("lean_ctas"), the fast kernel's streams per warp ("fast_S", 0
+        without such streams), and per frame ("frames") a dict of its lean streams ("count"), the lanes that start on
+        them ("lanes"; the rest are queued), its CTAs ("ctas") and the pulls of its lanes from its stream queue
+        ("pulls": "count" when every queued stream was taken once). Waits for the run."""
+        def one(f):
+            v = [C.c_uint32() for _ in range(5)]
+            abi.check(self._lib, self._lib.jxg_batch_entropy_schedule(self._h, f, *(C.byref(x) for x in v)))
+            return [x.value for x in v]
+        count, lanes, ctas, fast_s, pulls = one(abi.ALL_FRAMES)
+        frames = []
+        for f in range(len(self.frames)):
+            c, la, ct, _, p = one(f)
+            frames.append({"count": c, "lanes": la, "ctas": ct, "pulls": p})
+        return {"lean_S": self.entropy_stats()["lean_S"], "lean_count": count, "lean_lanes": lanes, "lean_ctas": ctas,
+                "fast_S": fast_s, "lean_pulls": pulls, "frames": frames}
+
+    def stream_status(self, f: int):
+        """Status word of each group of whole frame f after wait() (jxg_batch_stream_status): 0 or a JXG_ERR_* code."""
+        n = self.frames[f].info.num_groups
+        out = np.empty(n, np.int32)
+        abi.check(self._lib, self._lib.jxg_batch_stream_status(self._h, f, out.ctypes.data_as(C.POINTER(C.c_int32)), n))
+        return out
 
     def read_coeffs(self, f: int):
         n = self.frames[f].info.num_groups * 3 * 65536

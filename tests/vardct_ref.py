@@ -222,11 +222,14 @@ class Frame:
         self.passes = passes
         self.hist = hist
 
-    def decode(self, chooser):
+    def decode(self, chooser, per_group=False):
         """Runs the decode forward. chooser(ev) returns, for ev = dict(pass, group, c, bx, by, t, num_blocks,
         num_coeffs, shift, predicted, ...), (nonzeros, [values from k = num_blocks on]). Sets .tokens, .coeffs,
-        .reach, .error (None or the first refusal)."""
+        .reach, .error (None or the first refusal). A refusal ends the whole decode; with `per_group` it ends only its
+        group, whose stream stops at the refused token, and the decode goes on with the next group: .group_errors
+        then holds each group's refusal (None for a good group; None throughout without `per_group`)."""
         self.error = None
+        self.group_errors = [None] * self.num_groups
         bcm = self.bcm
         nac = bcm.num_ctx * 495
         first = {}
@@ -241,91 +244,102 @@ class Frame:
                   for p in self.passes]
         try:
             for g in range(self.num_groups):
-                gx, gy = g % self.xg, g // self.xg
-                bx0, by0 = gx * 32, gy * 32
-                gw, gh = min(32, self.xb - bx0), min(32, self.yb - by0)
-                nzmap = [[[0] * 1024 for _ in range(3)] for _ in self.passes]
-                hidx = []
-                for p in range(len(self.passes)):
-                    h = self.hist[p * self.num_groups + g]
-                    if h >= self.num_histograms:
-                        raise DecodeError("InvalidHistogramIndex")
-                    hidx.append(h)
-                    reach["hist"].add(h)
-                offset = 0
-                for by in range(gh):
-                    for bx in range(gw):
-                        vb = first.get((by0 + by, bx0 + bx))
-                        if vb is None:
-                            continue
-                        t, rq = vb[2], vb[3]
-                        cx, cy = COV_X[t], COV_Y[t]
-                        nb, nc = cx * cy, cx * cy * 64
-                        lnb = ceil_log2(nb)
-                        reach["lnb"].add(lnb)
-                        o = ORDER_OF[t]
-                        qx, qy, qb = (int(self.lf[c, by0 + by, bx0 + bx]) for c in range(3))
-                        lf_idx = bcm.lf_index(qx, qy, qb) if bcm.num_lf > 1 else 0
-                        qf_idx = bcm.qf_index(rq)
-                        for p, ps in enumerate(self.passes):
-                            shift = ps["shift"]
-                            reach["shifts"].add(shift)
-                            toks = self.tokens[p * self.num_groups + g]
-                            ctx_off = hidx[p] * nac
-                            for c in (1, 0, 2):
-                                nz = nzmap[p][c]
-                                if bx == 0:
-                                    pred = 32 if by == 0 else nz[(by - 1) * 32]
-                                elif by == 0:
-                                    pred = nz[bx - 1]
-                                else:
-                                    pred = (nz[(by - 1) * 32 + bx] + nz[by * 32 + bx - 1] + (0 if F.pred_no_round else 1)) // 2
-                                bctx, cell = bcm.block_context(c, o, qf_idx, lf_idx)
-                                reach["cells"].add(cell)
-                                nzctx, bucket = bcm.nonzero_context(pred, bctx)
-                                reach["nz_buckets"].add(bucket)
-                                ev = dict(p=p, g=g, c=c, bx=bx0 + bx, by=by0 + by, t=t, num_blocks=nb, num_coeffs=nc,
-                                          shift=shift, predicted=pred)
-                                nonzeros, vals = chooser(ev)
-                                toks.append((nzctx + ctx_off, nonzeros))
-                                if nonzeros + nb > nc:
-                                    raise DecodeError("InvalidNumNonZeros")
-                                if nonzeros == nc - nb:
-                                    reach["full"] += 1
-                                if nonzeros == 0:
-                                    reach["empty"] += 1
-                                store = (nonzeros >> lnb) if F.nz_store_floor else shrc(nonzeros, lnb)
-                                for iy in range(cy):
-                                    for ix in range(cx):
-                                        nz[(by + iy) * 32 + bx + ix] = store
-                                histo = bcm.num_ctx * 37 + 458 * bctx + ctx_off
-                                prev = 0 if (nonzeros >= nc // 16 if F.prev_ge else nonzeros > nc // 16) else 1
-                                order = orders[p][3 * o + c]
-                                reach["orders"].add((p, 3 * o + c, id(order)))
-                                k = nb
-                                vi = 0
-                                while k < nc and nonzeros:
-                                    v = vals[vi]
-                                    vi += 1
-                                    toks.append((histo + bcm.zero_density_context(nonzeros, k, lnb, prev), pack_signed(v)))
-                                    coeff = wrap32(v << shift)
-                                    if v != 0 and coeff == 0:
-                                        reach["wrapped"] += 1
-                                    prev = int((v if F.shift_after_prev else coeff) != 0)
-                                    nonzeros -= prev
-                                    pos = offset + int(order[k])
-                                    self.coeffs[g, c, pos] = wrap32(self.coeffs[g, c, pos] + coeff)
-                                    reach["max_abs"] = max(reach["max_abs"], abs(int(coeff)))
-                                    if nonzeros == 0 and k == nc - 1:
-                                        reach["last_k"] += 1
-                                    k += 1
-                                if nonzeros:
-                                    raise DecodeError("EndOfBlockResidualNonZeros")
-                        offset += nb * 64
+                try:
+                    self._decode_group(g, chooser, orders, nac, first, reach)
+                except DecodeError as e:
+                    if not per_group:
+                        raise
+                    self.group_errors[g] = e.kind
+                    self.error = self.error or e.kind
         except DecodeError as e:
             self.error = e.kind
         self.coeffs = self.coeffs.astype(np.int32)
         return self
+
+    def _decode_group(self, g, chooser, orders, nac, first, reach):
+        """One group of decode(): every pass, varblocks in raster order; raises DecodeError at a refusal."""
+        bcm = self.bcm
+        gx, gy = g % self.xg, g // self.xg
+        bx0, by0 = gx * 32, gy * 32
+        gw, gh = min(32, self.xb - bx0), min(32, self.yb - by0)
+        nzmap = [[[0] * 1024 for _ in range(3)] for _ in self.passes]
+        hidx = []
+        for p in range(len(self.passes)):
+            h = self.hist[p * self.num_groups + g]
+            if h >= self.num_histograms:
+                raise DecodeError("InvalidHistogramIndex")
+            hidx.append(h)
+            reach["hist"].add(h)
+        offset = 0
+        for by in range(gh):
+            for bx in range(gw):
+                vb = first.get((by0 + by, bx0 + bx))
+                if vb is None:
+                    continue
+                t, rq = vb[2], vb[3]
+                cx, cy = COV_X[t], COV_Y[t]
+                nb, nc = cx * cy, cx * cy * 64
+                lnb = ceil_log2(nb)
+                reach["lnb"].add(lnb)
+                o = ORDER_OF[t]
+                qx, qy, qb = (int(self.lf[c, by0 + by, bx0 + bx]) for c in range(3))
+                lf_idx = bcm.lf_index(qx, qy, qb) if bcm.num_lf > 1 else 0
+                qf_idx = bcm.qf_index(rq)
+                for p, ps in enumerate(self.passes):
+                    shift = ps["shift"]
+                    reach["shifts"].add(shift)
+                    toks = self.tokens[p * self.num_groups + g]
+                    ctx_off = hidx[p] * nac
+                    for c in (1, 0, 2):
+                        nz = nzmap[p][c]
+                        if bx == 0:
+                            pred = 32 if by == 0 else nz[(by - 1) * 32]
+                        elif by == 0:
+                            pred = nz[bx - 1]
+                        else:
+                            pred = (nz[(by - 1) * 32 + bx] + nz[by * 32 + bx - 1] + (0 if F.pred_no_round else 1)) // 2
+                        bctx, cell = bcm.block_context(c, o, qf_idx, lf_idx)
+                        reach["cells"].add(cell)
+                        nzctx, bucket = bcm.nonzero_context(pred, bctx)
+                        reach["nz_buckets"].add(bucket)
+                        ev = dict(p=p, g=g, c=c, bx=bx0 + bx, by=by0 + by, t=t, num_blocks=nb, num_coeffs=nc,
+                                  shift=shift, predicted=pred)
+                        nonzeros, vals = chooser(ev)
+                        toks.append((nzctx + ctx_off, nonzeros))
+                        if nonzeros + nb > nc:
+                            raise DecodeError("InvalidNumNonZeros")
+                        if nonzeros == nc - nb:
+                            reach["full"] += 1
+                        if nonzeros == 0:
+                            reach["empty"] += 1
+                        store = (nonzeros >> lnb) if F.nz_store_floor else shrc(nonzeros, lnb)
+                        for iy in range(cy):
+                            for ix in range(cx):
+                                nz[(by + iy) * 32 + bx + ix] = store
+                        histo = bcm.num_ctx * 37 + 458 * bctx + ctx_off
+                        prev = 0 if (nonzeros >= nc // 16 if F.prev_ge else nonzeros > nc // 16) else 1
+                        order = orders[p][3 * o + c]
+                        reach["orders"].add((p, 3 * o + c, id(order)))
+                        k = nb
+                        vi = 0
+                        while k < nc and nonzeros:
+                            v = vals[vi]
+                            vi += 1
+                            toks.append((histo + bcm.zero_density_context(nonzeros, k, lnb, prev), pack_signed(v)))
+                            coeff = wrap32(v << shift)
+                            if v != 0 and coeff == 0:
+                                reach["wrapped"] += 1
+                            prev = int((v if F.shift_after_prev else coeff) != 0)
+                            nonzeros -= prev
+                            pos = offset + int(order[k])
+                            self.coeffs[g, c, pos] = wrap32(self.coeffs[g, c, pos] + coeff)
+                            reach["max_abs"] = max(reach["max_abs"], abs(int(coeff)))
+                            if nonzeros == 0 and k == nc - 1:
+                                reach["last_k"] += 1
+                            k += 1
+                        if nonzeros:
+                            raise DecodeError("EndOfBlockResidualNonZeros")
+                offset += nb * 64
 
     @property
     def spec(self):
