@@ -260,6 +260,16 @@ int jxg_batch_entropy_schedule(void* batch, uint32_t f, uint32_t* lean_count, ui
  * JXG_ERR_ARGUMENT before jxg_batch_run, for a frame out of range or when n < the frame's group count. */
 int jxg_batch_stream_status(void* batch, uint32_t f, int32_t* out, uint32_t n);
 
+/* The transform-class partition of the block plan for each group of frame f after the last run: counts[g * 8 + c] =
+ * varblocks of class c of group g, entries[g * 1024 ..] = one word per varblock, class after class: its ordinal in the
+ * raster order of the group's varblocks | bx << 10 | by << 15 (its first block inside the group) | transform type << 20.
+ * Classes: 0 DCT8X8 / DCT4X4 / DCT4X8 / DCT8X4, 1 DCT16X8 / DCT8X16, 2 DCT16X16, 3 the other types of at most 4 x 4
+ * blocks, 4 larger varblocks; words 5..7 are 0. Classes 0..2 are grouped by transform type in the order
+ * 0, 3, 12, 13 / 6, 7 / 4, raster order within a type; classes 3 and 4 are in raster order. A group whose block plan
+ * failed has all counts 0. Slots of entries behind the group's varblocks are not written. Waits for the last run;
+ * JXG_ERR_ARGUMENT before jxg_batch_run, for a frame out of range or when n < the frame's group count. */
+int jxg_batch_read_transform_plan(void* batch, uint32_t f, uint32_t* counts, uint32_t* entries, uint32_t n);
+
 /* ---------------- convenience front-end (host parse + batch) ----------------
  * Parses complete .jxl files (container or bare codestream) on the host with
  * the in-tree C++ front-end (the stand-in for the Rust host: headers, TOC,

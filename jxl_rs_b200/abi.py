@@ -81,6 +81,7 @@ EXPORTS = [
     "jxg_modular_batch_read_planes", "jxg_modular_batch_stats", "jxg_modular_batch_end", "jxg_modular_walk_table",
     "jxg_modular_batch_lz77_stats", "jxg_modular_batch_walk_stats", "jxg_batch_add_frame_region", "jxg_batch_add_parsed_region",
     "jxg_parsed_region_desc", "jxg_context_set_sm_budget", "jxg_batch_entropy_schedule", "jxg_batch_stream_status",
+    "jxg_batch_read_transform_plan",
 ]
 
 ALL_FRAMES = 0xFFFFFFFF  # JXG_ALL_FRAMES
@@ -148,6 +149,7 @@ def load_library():
     lib.jxg_batch_entropy_stats.argtypes = [vp, u32p, u32p, u32p, C.POINTER(C.c_int), C.POINTER(C.c_int), u32p]
     lib.jxg_batch_entropy_schedule.argtypes = [vp, C.c_uint32, u32p, u32p, u32p, u32p, u32p]
     lib.jxg_batch_stream_status.argtypes = [vp, C.c_uint32, C.POINTER(C.c_int32), C.c_uint32]
+    lib.jxg_batch_read_transform_plan.argtypes = [vp, C.c_uint32, vp, vp, C.c_uint32]
     lib.jxg_parse_file.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(vp), C.POINTER(JxgImageInfo)]
     lib.jxg_parse_file_mt.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.POINTER(vp), C.POINTER(JxgImageInfo)]
     lib.jxg_parsed_free.argtypes = [vp]

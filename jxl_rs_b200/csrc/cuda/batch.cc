@@ -60,8 +60,7 @@ struct FrameOut {
 struct Batch : BatchCore {
   PinnedArena& blob;
   explicit Batch(Context* c)
-      : blob(c->blob), d_blob(c->d_blob), d_coeffs(c->d_coeffs), d_block_off(c->d_block_off),
-        d_planes_a(c->d_planes_a), d_status(c->d_status), d_out(c->d_out) {}
+      : blob(c->blob), d_blob(c->d_blob), d_coeffs(c->d_coeffs), d_planes_a(c->d_planes_a), d_status(c->d_status), d_out(c->d_out) {}
   std::vector<FrameDev> frames;
   std::vector<SectionDev> sections;
   std::vector<StreamDev> streams, streams_lean, streams_fast, streams_slow;
@@ -77,12 +76,12 @@ struct Batch : BatchCore {
   // are owned here until jxg_batch_end because a deferred copy reads their tables at jxg_batch_run
   std::vector<const jxg::RegionSlice*> frame_region;
   std::vector<std::unique_ptr<jxg::RegionSlice>> regions;
-  uint64_t total_groups = 0, total_blocks = 0, total_plane_floats = 0, out_bytes = 0, orient_bytes = 0;
+  uint64_t total_groups = 0, total_plane_floats = 0, out_bytes = 0, orient_bytes = 0;
   uint32_t lz_windows = 0;
   uint32_t filter_cfg_mask = 0;  // bit (gab * 4 + min(epf_iters, 3))
   int debug_stop = 0;
   // device
-  DevBuf &d_blob, &d_coeffs, &d_block_off, &d_planes_a, &d_status, &d_out;
+  DevBuf &d_blob, &d_coeffs, &d_planes_a, &d_status, &d_out;
   // byte offsets of the batch tables inside the blob (they ride on the one pinned H2D copy: a cudaMemcpyAsync from
   // pageable std::vector storage blocks the calling thread until earlier device work drains, which takes long with
   // other batches in flight)
@@ -491,8 +490,6 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   }
   F.coeff_group_base = b->total_groups;
   b->total_groups += F.num_groups;
-  F.block_base = b->total_blocks;
-  b->total_blocks += nb;
   F.plane_size = size_t(F.plane_stride) * F.plane_rows;
   F.plane_base = b->total_plane_floats;
   b->total_plane_floats += 3 * F.plane_size;
@@ -687,7 +684,6 @@ static BatchDev make_batch_dev(Batch* b) {
   B.num_fast = uint32_t(b->streams_fast.size());
   B.num_slow = uint32_t(b->streams_slow.size());
   B.nzlist = static_cast<uint32_t*>(b->d_coeffs.p);  // the pool that held the dense coefficients now holds the lists
-  B.block_off = static_cast<uint32_t*>(b->d_block_off.p);
   B.lzwin = static_cast<uint32_t*>(b->ctx->d_lzwin.p);
   B.planes_a = static_cast<float*>(b->d_planes_a.p);
   B.status = static_cast<int32_t*>(b->d_status.p);
@@ -696,6 +692,8 @@ static BatchDev make_batch_dev(Batch* b) {
   B.lean_warp = reinterpret_cast<const uint2*>(tab(b->tab.lean_warp));
   B.desc = static_cast<uint4*>(b->ctx->d_desc.p);
   B.nblk = static_cast<uint32_t*>(b->ctx->d_nblk.p);
+  B.cls_n = static_cast<uint32_t*>(b->ctx->d_cls_n.p);
+  B.cls_list = static_cast<uint32_t*>(b->ctx->d_cls_list.p);
   B.dequant_default = static_cast<const float*>(b->ctx->dequant_default.p);
   B.dequant_default_off = static_cast<const uint32_t*>(b->ctx->dequant_default_off.p);
   B.natural_orders = static_cast<const uint32_t*>(b->ctx->natural_orders.p);
@@ -782,13 +780,14 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
   // device allocations
   // one coefficient list per HF section (pass x group), worst-case capacity (every coefficient non-zero)
   if (int r = b->d_coeffs.ensure(b->sections.size() * size_t(kListStride) * 4)) return r;
-  if (int r = b->d_block_off.ensure(b->total_blocks * 4)) return r;
   if (int r = b->ctx->d_lzwin.ensure(std::max<size_t>(size_t(b->lz_windows) * kLzWindow * 4, 16))) return r;
   if (int r = b->d_planes_a.ensure(b->total_plane_floats * 4)) return r;
   if (int r = b->d_status.ensure((b->streams.size() + b->frames.size() + 4) * 4)) return r;
   if (int r = b->d_out.ensure(std::max<size_t>(b->out_bytes, 16))) return r;
   if (int r = b->ctx->d_desc.ensure(std::max<size_t>(b->streams.size() * 1024 * 16, 16))) return r;
   if (int r = b->ctx->d_nblk.ensure(std::max<size_t>(b->streams.size() * 4, 16))) return r;
+  if (int r = b->ctx->d_cls_n.ensure(std::max<size_t>(b->streams.size() * kClassWords * 4, 16))) return r;
+  if (int r = b->ctx->d_cls_list.ensure(std::max<size_t>(b->streams.size() * 1024 * 4, 16))) return r;
   if (int r = b->ctx->d_orient.ensure(std::max<size_t>(b->orient_bytes, 16))) return r;
   for (size_t f = 0; f < b->frames.size(); f++) {
     const FrameOut& fo = b->outs[f];
@@ -933,6 +932,20 @@ int jxg_batch_stream_status(void* bp, uint32_t f, int32_t* out, uint32_t n) {
   if (int r = batch_wait_last_run(*b)) return r;
   const FrameDev& F = b->frames[f];
   memcpy(out, b->status_host + F.first_stream, size_t(F.num_groups) * 4);
+  return JXG_OK;
+}
+
+int jxg_batch_read_transform_plan(void* bp, uint32_t f, uint32_t* counts, uint32_t* entries, uint32_t n) {
+  Batch* b = static_cast<Batch*>(bp);
+  if (!b || !counts || !entries || !b->uploaded || f >= b->frames.size() || n < b->frames[f].num_groups) return JXG_ERR_ARGUMENT;
+  if (int r = batch_wait_last_run(*b)) return r;
+  const FrameDev& F = b->frames[f];
+  cudaStream_t s = b->last_stream ? b->last_stream : b->ctx->stream;
+  CUDA_TRY(cudaMemcpyAsync(counts, static_cast<const uint32_t*>(b->ctx->d_cls_n.p) + size_t(F.first_stream) * kClassWords,
+                           size_t(F.num_groups) * kClassWords * 4, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(entries, static_cast<const uint32_t*>(b->ctx->d_cls_list.p) + size_t(F.first_stream) * 1024,
+                           size_t(F.num_groups) * 1024 * 4, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   return JXG_OK;
 }
 

@@ -132,7 +132,7 @@ struct Context {
   // intermediates and the pinned staging arena survive jxg_batch_end so that a
   // steady-state decode loop does no cudaMalloc / cudaHostAlloc.
   PinnedArena blob;
-  DevBuf d_blob, d_coeffs, d_block_off, d_planes_a, d_status, d_out, d_desc, d_nblk, d_orient, d_lzwin,
+  DevBuf d_blob, d_coeffs, d_planes_a, d_status, d_out, d_desc, d_nblk, d_cls_n, d_cls_list, d_orient, d_lzwin,
       d_modular_lzwin, d_modular_wp;
   int pool_fill = -1;  // test hook (jxg_context_set_pool_fill): byte written over the pools before each run, -1: off
   int sm_budget = 0;   // test hook (jxg_context_set_sm_budget): SMs every schedule of the context assumes, 0: the device's
@@ -240,8 +240,8 @@ bool batch_table(PinnedArena& blob, const std::vector<T>& v, uint64_t& off) {
 // earlier batch left there. A run fills d_blob as well (the upload then overwrites its own part); a rerun keeps it.
 inline int fill_pools(Context* cx, cudaStream_t s, bool with_blob) {
   if (cx->pool_fill < 0) return 0;
-  for (DevBuf* d : {&cx->d_blob, &cx->d_coeffs, &cx->d_block_off, &cx->d_planes_a, &cx->d_status, &cx->d_out, &cx->d_desc,
-                    &cx->d_nblk, &cx->d_orient, &cx->d_lzwin, &cx->d_modular_lzwin, &cx->d_modular_wp})
+  for (DevBuf* d : {&cx->d_blob, &cx->d_coeffs, &cx->d_planes_a, &cx->d_status, &cx->d_out, &cx->d_desc, &cx->d_nblk,
+                    &cx->d_cls_n, &cx->d_cls_list, &cx->d_orient, &cx->d_lzwin, &cx->d_modular_lzwin, &cx->d_modular_wp})
     if (d->p && (with_blob || d != &cx->d_blob)) CUDA_TRY(cudaMemsetAsync(d->p, cx->pool_fill, d->cap, s));
   return 0;
 }

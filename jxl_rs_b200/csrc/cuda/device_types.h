@@ -33,6 +33,20 @@ constexpr uint32_t kListStride = kOffBase + kOffWords;  // u32 words per list
 
 // One entropy code (decode.rs:36-58) of a VarDCT pass (PassDev::code) or a Modular stream (MBatchDev::codes), tables in
 // the blob.
+// Transform classes of the block plan (BatchDev::cls_n): which kernel and lane layout each varblock goes through.
+constexpr uint32_t kClassReg8 = 0;    // k_idct_small<0>, 8 lanes: DCT8X8, DCT4X4, DCT4X8, DCT8X4 (types 0, 3, 12, 13)
+constexpr uint32_t kClassReg16_8 = 1; // k_idct_small<1>, 8 lanes: DCT16X8, DCT8X16 (types 6, 7)
+constexpr uint32_t kClassReg16 = 2;   // k_idct_small<1>, 16 lanes: DCT16X16 (type 4)
+constexpr uint32_t kClassWarp = 3;    // k_dequant_idct, one warp: the other types of at most 4 x 4 blocks
+constexpr uint32_t kClassCta = 4;     // k_dequant_idct, the whole CTA: varblocks wider or taller than 4 blocks
+constexpr uint32_t kClassWords = 8;   // words per stream in cls_n (the last three are 0)
+// Class-list entry of a varblock: everything a transform kernel needs to find it, in one word (no dependent descriptor
+// load): ordinal in the group (index into desc and the coefficient list's offset words) | bx << 10 | by << 15 (first
+// block inside the group) | transform type << 20.
+__host__ __device__ constexpr uint32_t cls_entry(uint32_t seq, uint32_t bx, uint32_t by, uint32_t t) {
+  return seq | (bx << 10) | (by << 15) | (t << 20);
+}
+
 struct CodeDev {
   uint32_t use_prefix, log_alpha, num_clusters;
   // LZ77 (decode.rs:36-45): tokens >= lz_min_symbol start a copy of hybrid(lz_len_cfg) + lz_min_length symbols, whose
@@ -82,7 +96,6 @@ struct FrameDev {
   uint32_t has_lz, lz_win_base;
   // device-only buffers (element offsets)
   uint64_t coeff_group_base;  // group index base into coeffs
-  uint64_t block_base;        // block index base into block_off
   uint64_t plane_base;        // float index base into plane sets (per channel: + c * plane_size)
   uint64_t plane_size;        // plane_stride * plane_rows
   uint64_t out_off;           // byte offset into device output buffer (or absolute pointer if out_is_ptr)
@@ -126,7 +139,6 @@ struct BatchDev {
   uint32_t num_frames, num_streams, num_lean, num_fast, num_slow;
   uint32_t* nzlist;     // [sections][kListStride]: list of section (pass * num_groups + group) of a frame, see above
   uint32_t* lzwin;      // [lz sections][kLzWindow] LZ77 windows (decode.rs:86-146), frames with has_lz only
-  uint32_t* block_off;  // per 8x8 block: ordinal (raster order) of the varblock starting there within its group
   float* planes_a;
   int32_t* status;      // per stream
   uint32_t* queue;      // [frames] work-queue cursors of the persistent entropy kernel
@@ -134,6 +146,11 @@ struct BatchDev {
   const uint2* lean_warp;          // [lean CTAs * 4] per warp: first stream (relative to the frame's list), lanes
   uint4* desc;           // [num_streams][1024] varblock descriptors written by k_block_plan, read by every entropy kernel
   uint32_t* nblk;        // [num_streams] varblocks per stream (0xffffffff: the plan failed, JXG_ERR_INVALID_TRANSFORM)
+  // Transform-class partition of each stream's varblocks, written by k_block_plan and read by the transform kernels:
+  // cls_n[s * kClassWords + c] = varblocks of class c (kClass*), cls_list[s * 1024 ..] = their entries (cls_entry),
+  // class after class in kClass* order, each class grouped by transform type, raster order within a type.
+  uint32_t* cls_n;       // [num_streams][kClassWords]
+  uint32_t* cls_list;    // [num_streams][1024]
   // context-wide tables
   const float* dequant_default;       // 17 tables concatenated
   const uint32_t* dequant_default_off;  // [17] float offsets

@@ -5,7 +5,8 @@
 //   k_entropy_fast       entropy_coding/*.rs): persistent lanes for single-pass ANS frames (lean), packed lanes for
 //   k_entropy            prefix-coded or shifted single-pass frames (fast), one lane per warp for multi-pass and LZ77 frames
 //   k_idct_small     K2  one CTA per group: dequant + chroma-from-luma + LLF + inverse variable-block DCT
-//   k_dequant_idct       (group.rs:100-250, jxl_transforms/src/transform.rs); small and large varblocks
+//   k_dequant_idct       (group.rs:100-250, jxl_transforms/src/transform.rs); each kernel walks the varblocks of its
+//                        transform classes in the block plan's partition
 //   k_filters_store  K3-K5 fused Gaborish -> EPF 0/1/2 -> XYB -> output transfer curve -> store
 //                    (render/stages/{gaborish,epf/*,xyb,from_linear,convert}.rs, color/tf.rs)
 //   k_orient         orientation post-pass of frames with orientation != 1
@@ -542,14 +543,23 @@ __global__ void __launch_bounds__(128, 8) k_entropy_fast(const BatchDev B) {
 // corrupt stream cannot walk out of the blob (the over-read is reported from bitpos at the end).
 // ---------------------------------------------------------------------------
 // ---------------------------------------------------------------------------
-// K0: block plan of the entropy kernels. One warp per (frame, group) stream walks the group's 32x32 transform map
+// K0: block plan of the entropy and transform kernels. One warp per (frame, group) stream walks the group's 32x32 transform map
 // in raster order and writes, for every varblock, a 16-byte descriptor
 //   x: bx | by << 5 | cx << 10 | cy << 16 | shape << 22 | log2(cx * cy) << 26
 //   y: block contexts of Y, X, B (block_context_map.rs:128-150), one byte each
 //   z: offset of the block's coefficients inside the group's dense decode-order array (group.rs:455; parity tap only)
-// plus the block count and block_off[] = the varblock's ordinal (read by the transform kernels to find its entries). This is everything the serial decode lanes
-// needed several dependent loads and a scan loop for, computed here fully in parallel.
+//   w: transform type (HfTransformType)
+// plus the block count. This is everything the serial decode lanes needed several dependent loads and a scan loop for,
+// computed here fully in parallel. Then the same warp partitions the varblocks into the transform classes (kClass*,
+// BatchDev::cls_n / cls_list), so that each transform kernel walks only its own varblocks.
 // ---------------------------------------------------------------------------
+// Bucket of each transform type in the class partition: the classes in kClass* order, and inside the register classes
+// one bucket per type (lanes of a warp then mostly share a type). kNumBuckets buckets.
+constexpr uint32_t kNumBuckets = 9;
+__constant__ uint8_t c_bucket[27] = {0, 7, 7, 1, 6, 7, 4, 5, 7, 7, 7, 7, 2, 3, 7, 7, 7, 7, 8, 8, 8, 8, 8, 8, 8, 8, 8};
+// first bucket of each class, and kNumBuckets
+__constant__ uint8_t c_class_bucket[6] = {0, 4, 6, 7, 8, kNumBuckets};
+
 __global__ void __launch_bounds__(128) k_block_plan(const BatchDev B) {
   const uint32_t sidx = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (sidx >= B.num_streams) return;
@@ -563,7 +573,6 @@ __global__ void __launch_bounds__(128) k_block_plan(const BatchDev B) {
   const int32_t* rq = reinterpret_cast<const int32_t*>(B.blob + F.raw_quant_off) + goff;
   const uint8_t* qlf = B.blob + F.quant_lf_off + goff;
   const uint8_t* bcm = B.blob + F.block_ctx_map_off;
-  uint32_t* block_off = B.block_off + F.block_base + goff;
   uint4* desc = B.desc + size_t(sidx) * 1024;
   uint32_t seq = 0, coeffs_offset = 0;
   bool bad = false;
@@ -602,15 +611,59 @@ __global__ void __launch_bounds__(128) k_block_plan(const BatchDev B) {
       d.x = lane | (by << 5) | (cx << 10) | (cy << 16) | (shape << 22) | ((31u - __clz(cx * cy)) << 26);
       d.y = cy_ctx | (cx_ctx << 8) | (cb_ctx << 16);
       d.z = off;
-      d.w = 0;
+      d.w = tt;
       desc[seq + rank] = d;
-      block_off[bidx] = seq + rank;
     }
     seq += __popc(mask);
     coeffs_offset += row_total;
   }
   bad = __any_sync(0xffffffffu, bad);
   if (lane == 0) B.nblk[sidx] = bad ? 0xffffffffu : seq;
+
+  // Class partition: a counting sort of the descriptors by bucket, read back in raster (ordinal) order. A failed plan
+  // has empty classes (its stream reports the error and no transform touches it).
+  uint32_t* cls_n = B.cls_n + size_t(sidx) * kClassWords;
+  if (bad) {
+    if (lane < kClassWords) cls_n[lane] = 0;
+    return;
+  }
+  uint32_t* cls_list = B.cls_list + size_t(sidx) * 1024;
+  const uint32_t* dw = reinterpret_cast<const uint32_t*>(desc);  // x and w words, written above by this warp
+  __syncwarp();
+  uint32_t cnt = 0;  // lane k < kNumBuckets: varblocks of bucket k
+  for (uint32_t i0 = 0; i0 < seq; i0 += 32) {
+    const uint32_t bk = i0 + lane < seq ? c_bucket[dw[size_t(i0 + lane) * 4 + 3]] : kNumBuckets;
+#pragma unroll
+    for (uint32_t k = 0; k < kNumBuckets; k++) {
+      const uint32_t m = __ballot_sync(0xffffffffu, bk == k);
+      if (lane == k) cnt += __popc(m);
+    }
+  }
+  uint32_t start = cnt;  // exclusive prefix sum over the buckets
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t v = __shfl_up_sync(0xffffffffu, start, d);
+    if (int(lane) >= d) start += v;
+  }
+  start -= cnt;
+  // class c covers buckets c_class_bucket[c] .. c_class_bucket[c + 1] - 1 (lane kNumBuckets holds the total); lane c < 5
+  // stores its count
+  const uint32_t s0 = __shfl_sync(0xffffffffu, start, c_class_bucket[min(lane, 5u)]);
+  const uint32_t s1 = __shfl_sync(0xffffffffu, start, c_class_bucket[min(lane + 1, 5u)]);
+  if (lane < kClassWords) cls_n[lane] = lane < 5 ? s1 - s0 : 0u;
+  uint32_t fill = start;  // lane k: next slot of bucket k
+  for (uint32_t i0 = 0; i0 < seq; i0 += 32) {
+    const uint32_t i = i0 + lane;
+    const uint32_t x = i < seq ? dw[size_t(i) * 4] : 0u, t = i < seq ? dw[size_t(i) * 4 + 3] : 0u;
+    const uint32_t bk = i < seq ? c_bucket[t] : kNumBuckets;
+#pragma unroll
+    for (uint32_t k = 0; k < kNumBuckets; k++) {
+      const uint32_t m = __ballot_sync(0xffffffffu, bk == k);
+      const uint32_t at = __shfl_sync(0xffffffffu, fill, k);
+      if (bk == k) cls_list[at + __popc(m & ((1u << lane) - 1u))] = cls_entry(i, x & 31, (x >> 5) & 31, t);
+      if (lane == k) fill += __popc(m);
+    }
+  }
 }
 
 // Loads the compiler must not sink below the token computation (it would re-serialise the chain).
@@ -1328,12 +1381,10 @@ __device__ __noinline__ void warp_col_pass(float* ch, int lane_col, int stride) 
   for (int i = 0; i < N; i++) ch[i * stride + lane_col] = v[i];
 }
 
-// Types transformed in registers by k_idct_small: 8x8-footprint transforms and plain DCTs with rows of <= 16
-// coefficients. Rows of 32 (32x8 ... 32x32) unroll into ~300 KB of code and starve on instruction fetch, so they take the compact shared-memory path of k_dequant_idct.
-__device__ __forceinline__ bool is_small_reg_type(int t) {
-  return (t == 0) || (t >= 3 && t <= 13 && !(t == 5 || (t >= 8 && t <= 11)));
-}
-
+// k_dequant_idct takes the varblocks of the classes kClassWarp and kClassCta (k_block_plan). Types transformed in
+// registers by k_idct_small are the 8x8-footprint transforms and plain DCTs with rows of <= 16 coefficients. Rows of 32
+// (32x8 ... 32x32) unroll into ~300 KB of code and starve on instruction fetch, so they take the compact shared-memory
+// path here.
 constexpr int kIdctWarps = 8;   // per warp: dequantised work tiles 3 x kWarpBuf floats
 constexpr size_t kLargeSmemBytes = size_t(kIdctWarps) * (3 * (32 * 33)) * sizeof(float);
 constexpr int kWarpBuf = 32 * 33;  // floats per channel per warp
@@ -1388,21 +1439,22 @@ __device__ __forceinline__ void warp_dct_block(float* wbuf, int lane, const floa
 __global__ void __launch_bounds__(kIdctWarps * 32) k_dequant_idct(const BatchDev B) {
   extern __shared__ float smem[];
   __shared__ uint32_t s_next;
-  __shared__ uint32_t s_nbig;
-  __shared__ uint16_t s_big[64];
   const uint32_t stream = blockIdx.x;
   if (B.status[stream] != 0) return;
+  // this kernel's varblocks, from the block plan: the warp class, then the CTA class
+  const uint32_t* cn = B.cls_n + size_t(stream) * kClassWords;
+  const uint32_t nwarp = cn[kClassWarp], nbig = cn[kClassCta];
+  if (nwarp + nbig == 0) return;
+  const uint32_t* wlist = B.cls_list + size_t(stream) * 1024 + (cn[kClassReg8] + cn[kClassReg16_8] + cn[kClassReg16]);
+  const uint32_t* blist = wlist + nwarp;
   const StreamDev sd = B.streams[stream];
   const FrameDev& F = B.frames[sd.frame];
   const uint32_t g = sd.group;
   const uint32_t gx = g % F.xg, gy = g / F.xg;
   const uint32_t bx0 = gx * 32, by0 = gy * 32;
-  const uint32_t gw = min(32u, F.xb - bx0), gh = min(32u, F.yb - by0);
-  const uint8_t* tmap = B.blob + F.transform_off;
   const int32_t* rq = reinterpret_cast<const int32_t*>(B.blob + F.raw_quant_off);
   const int8_t* ytox = reinterpret_cast<const int8_t*>(B.blob + F.ytox_off);
   const int8_t* ytob = reinterpret_cast<const int8_t*>(B.blob + F.ytob_off);
-  const uint32_t* block_off = B.block_off + F.block_base;
   float* planes[3] = {B.planes_a + F.plane_base, B.planes_a + F.plane_base + F.plane_size,
                       B.planes_a + F.plane_base + 2 * F.plane_size};
   const float* lfp[3] = {reinterpret_cast<const float*>(B.blob + F.lf_off[0]),
@@ -1410,10 +1462,7 @@ __global__ void __launch_bounds__(kIdctWarps * 32) k_dequant_idct(const BatchDev
                          reinterpret_cast<const float*>(B.blob + F.lf_off[2])};
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float* wbuf = smem + warp * (3 * kWarpBuf);
-  if (threadIdx.x == 0) {
-    s_next = 0;
-    s_nbig = 0;
-  }
+  if (threadIdx.x == 0) s_next = 0;
   __syncthreads();
 
   // everything of the dequantisation context but the coefficient pointers (set by the callers)
@@ -1437,26 +1486,16 @@ __global__ void __launch_bounds__(kIdctWarps * 32) k_dequant_idct(const BatchDev
     dq.bias3 = F.quant_biases[3];
   };
 
-  // ---- warp path: each warp grabs the next block position of the group ----
+  // ---- warp path: each warp grabs the next varblock of the warp class ----
   for (;;) {
-    uint32_t pos = 0;
-    if (lane == 0) pos = atomicAdd(&s_next, 1u);
-    pos = __shfl_sync(0xffffffffu, pos, 0);
-    if (pos >= gw * gh) break;
-    const uint32_t bx = pos % gw, by = pos / gw;
-    const size_t bidx = size_t(by0 + by) * F.xb + bx0 + bx;
-    const uint32_t raw_t = tmap[bidx];
-    if (raw_t < 128) continue;
-    const int t = raw_t & 127;
+    uint32_t li = 0;
+    if (lane == 0) li = atomicAdd(&s_next, 1u);
+    li = __shfl_sync(0xffffffffu, li, 0);
+    if (li >= nwarp) break;
+    const uint32_t e = wlist[li];
+    const uint32_t seq = e & 1023, bx = (e >> 10) & 31, by = (e >> 15) & 31;
+    const int t = int(e >> 20);
     const int cx = c_cov_x[t], cy = c_cov_y[t];
-    if (is_small_reg_type(t)) continue;  // handled by k_idct_small
-    if (cx > 4 || cy > 4) {  // big varblock: handled cooperatively below
-      if (lane == 0) {
-        uint32_t i = atomicAdd(&s_nbig, 1u);
-        if (i < 64) s_big[i] = uint16_t(pos);
-      }
-      continue;
-    }
     DequantCtx dq;
     setup(bx, by, t, dq);
     const int R = 8 * cy, C = 8 * cx;
@@ -1467,7 +1506,7 @@ __global__ void __launch_bounds__(kIdctWarps * 32) k_dequant_idct(const BatchDev
       const bool wide_l = R < C;
       const DeqParams D{dq.mat, dq.num_coeffs, dq.sx, dq.sy, dq.sb, dq.x_cc, dq.b_cc, dq.bias0, dq.bias1, dq.bias2, dq.bias3};
       const uint32_t zero_floats = is_dct ? uint32_t((R * (C + 1) + 3) & ~3) : 64u;
-      gather_dequant_tile(B, F, g, block_off[bidx], wbuf, uint32_t(kWarpBuf), zero_floats, D, uint32_t(lane), 32, true,
+      gather_dequant_tile(B, F, g, seq, wbuf, uint32_t(kWarpBuf), zero_floats, D, uint32_t(lane), 32, true,
                           ListStage{nullptr, nullptr, 0}, [] { __syncwarp(); },
                           [=](uint32_t k) {
                             if (!is_dct) return k;
@@ -1539,12 +1578,10 @@ __global__ void __launch_bounds__(kIdctWarps * 32) k_dequant_idct(const BatchDev
   __syncthreads();
 
   // ---- big varblocks (a dimension >= 64): CTA-cooperative, in place in HBM ----
-  const uint32_t nbig = min(s_nbig, 64u);
   for (uint32_t bi = 0; bi < nbig; bi++) {
-    const uint32_t pos = s_big[bi];
-    const uint32_t bx = pos % gw, by = pos / gw;
-    const size_t bidx = size_t(by0 + by) * F.xb + bx0 + bx;
-    const int t = tmap[bidx] & 127;
+    const uint32_t e = blist[bi];
+    const uint32_t seq = e & 1023, bx = (e >> 10) & 31, by = (e >> 15) & 31;
+    const int t = int(e >> 20);
     const int cx = c_cov_x[t], cy = c_cov_y[t];
     const int R = 8 * cy, C = 8 * cx;
     DequantCtx dq;
@@ -1566,7 +1603,7 @@ __global__ void __launch_bounds__(kIdctWarps * 32) k_dequant_idct(const BatchDev
       planes[2][o] = 0.0f;
     }
     __syncthreads();
-    const uint32_t seq = block_off[bidx], lnc = 31 - __clz(dq.num_coeffs);
+    const uint32_t lnc = 31 - __clz(dq.num_coeffs);
     if (F.num_passes == 1) {
       const uint32_t* base = list_base(B, F.section_base + g);
       const uint32_t* ow = base + kOffBase + seq * 3;
@@ -1756,15 +1793,8 @@ __device__ __forceinline__ void reg_dct_block(const RegBlockCtx& X, const float*
   }
 }
 
-// KIND selects the coefficient-row length handled by this instantiation (register budget): 0: L = 8 (types
-// 0, 3, 12, 13), 1: L = 16 (6, 7, 4).
-__device__ __forceinline__ int reg_kind(int t) {
-  switch (t) {
-    case 0: case 3: case 12: case 13: return 0;
-    case 6: case 7: case 4: return 1;
-    default: return -1;
-  }
-}
+// KIND selects the coefficient-row length handled by this instantiation (register budget): 0: L = 8 (class kClassReg8:
+// types 0, 3, 12, 13), 1: L = 16 (kClassReg16_8 and kClassReg16: types 6, 7, 4).
 
 // Shared memory for the coefficient tiles of the lane groups of one CTA: every class of a KIND needs 32 x 8 lanes x 3 x NC
 // words with NC = 64 / 128 coefficients per channel (the 16-lane class holds 2x the coefficients in half the groups).
@@ -1773,7 +1803,7 @@ __host__ __device__ constexpr size_t small_tile_bytes() {
   return size_t(kSmallThreads / 8) * 3 * (KIND == 0 ? 64 : 128) * sizeof(int32_t);
 }
 // Behind the tiles: the staged offset words (kOffWords) and the first kStageEntries entries of the group's list,
-// delivered by two bulk copies issued by thread 0 before the CTA sorts its varblocks.
+// delivered by two bulk copies issued by thread 0. A CTA whose group has no varblock of its KIND issues none.
 constexpr uint32_t kStageEntries = 8192;
 template <int KIND>
 constexpr size_t small_smem_bytes() {
@@ -1783,11 +1813,14 @@ constexpr size_t small_smem_bytes() {
 template <int KIND>
 __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small(const BatchDev B) {
   extern __shared__ __align__(16) float s_tiles[];
-  __shared__ uint16_t s_list[1024];
-  __shared__ uint32_t s_cnt[28], s_start[28], s_fill[28];
   __shared__ __align__(8) uint64_t s_bar[2];
   const uint32_t stream = blockIdx.x;
   if (B.status[stream] != 0) return;
+  // this kernel's varblocks, from the block plan: KIND 0: the 8-lane class; KIND 1: its 8-lane class, then the 16-lane one
+  const uint32_t* cn = B.cls_n + size_t(stream) * kClassWords;
+  const uint32_t n8 = KIND == 0 ? cn[kClassReg8] : cn[kClassReg16_8], n16 = KIND == 0 ? 0u : cn[kClassReg16];
+  if (n8 + n16 == 0) return;  // before the staging copies: most groups have no varblock of one of the two kinds
+  const uint32_t* list = B.cls_list + size_t(stream) * 1024 + (KIND == 0 ? 0u : cn[kClassReg8]);
   const StreamDev sd = B.streams[stream];
   const FrameDev& F = B.frames[sd.frame];
   const uint32_t g = sd.group;
@@ -1804,50 +1837,20 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
     bulk_load(s_ent, base, kStageEntries * 4, &s_bar[1]);
   }
   const uint32_t bx0 = (g % F.xg) * 32, by0 = (g / F.xg) * 32;
-  const uint32_t gw = min(32u, F.xb - bx0), gh = min(32u, F.yb - by0);
-  const uint8_t* tmap = B.blob + F.transform_off;
-  if (threadIdx.x < 28) s_cnt[threadIdx.x] = 0;
-  __syncthreads();
-  // counting sort of the group's first-blocks by (lane class, transform type): lanes of a warp mostly share a type
-  for (uint32_t pos = threadIdx.x; pos < gw * gh; pos += blockDim.x) {
-    const uint32_t by = pos / gw, bx = pos - by * gw;
-    const uint32_t raw_t = tmap[size_t(by0 + by) * F.xb + bx0 + bx];
-    if (raw_t >= 128 && reg_kind(raw_t & 127) == KIND) atomicAdd(&s_cnt[raw_t & 127], 1u);
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const int order[7] = {0, 3, 12, 13, 6, 7, 4};
-    uint32_t acc = 0;
-    for (int i = 0; i < 7; i++) {
-      s_start[order[i]] = acc;
-      s_fill[order[i]] = acc;
-      acc += s_cnt[order[i]];
-    }
-  }
-  __syncthreads();
-  for (uint32_t pos = threadIdx.x; pos < gw * gh; pos += blockDim.x) {
-    const uint32_t by = pos / gw, bx = pos - by * gw;
-    const uint32_t raw_t = tmap[size_t(by0 + by) * F.xb + bx0 + bx];
-    if (raw_t >= 128 && reg_kind(raw_t & 127) == KIND) s_list[atomicAdd(&s_fill[raw_t & 127], 1u)] = uint16_t(bx | (by << 5));
-  }
-  __syncthreads();
-  const uint32_t begin8 = 0, begin16 = s_start[4], end_all = s_start[4] + s_cnt[4];
-  // the staged list has landed (the sort above ran while the copies were in flight)
+  __syncthreads();  // the barriers are initialised
   mbar_wait(&s_bar[0], 0);
   mbar_wait(&s_bar[1], 0);
   const ListStage stage{s_off, s_ent, kStageEntries};
   const int32_t* rq = reinterpret_cast<const int32_t*>(B.blob + F.raw_quant_off);
   const int8_t* ytox = reinterpret_cast<const int8_t*>(B.blob + F.ytox_off);
   const int8_t* ytob = reinterpret_cast<const int8_t*>(B.blob + F.ytob_off);
-  const uint32_t* block_off = B.block_off + F.block_base;
   const float bias0 = F.quant_biases[0], bias1 = F.quant_biases[1], bias2 = F.quant_biases[2], bias3 = F.quant_biases[3];
 
-  auto setup_ctx = [&](uint32_t e, RegBlockCtx& X, const float* (&lfp)[3], int& t, uint32_t& seq) {
-    const uint32_t bx = e & 31, by = e >> 5;
+  auto setup_ctx = [&](uint32_t e, RegBlockCtx& X, const float* (&lfp)[3], int& t) {
+    const uint32_t bx = (e >> 10) & 31, by = (e >> 15) & 31;
     const size_t bidx = size_t(by0 + by) * F.xb + bx0 + bx;
-    t = tmap[bidx] & 127;
+    t = int(e >> 20);
     const int qt = c_qtable[t];
-    seq = block_off[bidx];
     X.mat = F.dequant_off[qt] >= 0 ? reinterpret_cast<const float*>(B.blob + F.dequant_off[qt]) : B.dequant_default + B.dequant_default_off[qt];
     X.num_coeffs = uint32_t(c_cov_x[t]) * c_cov_y[t] * 64;
     const size_t cidx = size_t((by0 + by) >> 3) * F.cxb + ((bx0 + bx) >> 3);
@@ -1867,16 +1870,20 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
   {
     const uint32_t r = threadIdx.x & 7;
     const uint32_t gmask = 0xffu << (threadIdx.x & 24);
-    const uint32_t count = begin16 - begin8;
+    const uint32_t count = n8;
     const uint32_t iters = (count + kSmallThreads / 8 - 1) / (kSmallThreads / 8);
+    // class-list entries are loaded one iteration ahead: the varblock's set-up loads then start at once
+    uint32_t e_next = iters ? list[((threadIdx.x >> 3) < count ? (threadIdx.x >> 3) : 0u)] : 0u;
     for (uint32_t it = 0; it < iters; it++) {
       const uint32_t li = it * (kSmallThreads / 8) + (threadIdx.x >> 3);
       const bool valid = li < count;
+      const uint32_t e = e_next;  // invalid lanes hold the class's first entry
+      if (it + 1 < iters) e_next = list[(li + kSmallThreads / 8 < count ? li + kSmallThreads / 8 : 0u)];
       RegBlockCtx X;
       const float* lfp[3];
       int t;
-      uint32_t seq;
-      setup_ctx(s_list[begin8 + (valid ? li : 0)], X, lfp, t, seq);
+      const uint32_t seq = e & 1023;
+      setup_ctx(e, X, lfp, t);
       constexpr uint32_t NC = KIND == 0 ? 64 : 128;
       float* tile = s_tiles + (threadIdx.x >> 3) * 3 * NC;
       gather_dequant_tile(B, F, g, seq, tile, NC, NC, deq_of(X), r, 8, valid, stage, [&] { __syncwarp(gmask); },
@@ -1964,28 +1971,30 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
     }
   }
   // ---------------- class 1: 16 lanes per block ----------------
-  {
+  if constexpr (KIND == 1) {
     const uint32_t r = threadIdx.x & 15;
     const uint32_t gmask = 0xffffu << (threadIdx.x & 16);
-    const uint32_t count = end_all - begin16;
+    const uint32_t count = n16;
     const uint32_t iters = (count + kSmallThreads / 16 - 1) / (kSmallThreads / 16);
+    // class-list entries are loaded one iteration ahead: the varblock's set-up loads then start at once
+    uint32_t e_next = iters ? list[n8 + ((threadIdx.x >> 4) < count ? (threadIdx.x >> 4) : 0u)] : 0u;
     for (uint32_t it = 0; it < iters; it++) {
       const uint32_t li = it * (kSmallThreads / 16) + (threadIdx.x >> 4);
       const bool valid = li < count;
+      const uint32_t e = e_next;  // invalid lanes hold the class's first entry
+      if (it + 1 < iters) e_next = list[n8 + (li + kSmallThreads / 16 < count ? li + kSmallThreads / 16 : 0u)];
       RegBlockCtx X;
       const float* lfp[3];
       int t;
-      uint32_t seq;
-      setup_ctx(s_list[begin16 + (valid ? li : 0)], X, lfp, t, seq);
-      if constexpr (KIND == 1) {
-        constexpr uint32_t NC = 256;
-        float* tile = s_tiles + (threadIdx.x >> 4) * 3 * NC;
-        gather_dequant_tile(B, F, g, seq, tile, NC, NC, deq_of(X), r, 16, valid, stage, [&] { __syncwarp(gmask); },
-                            [](uint32_t pos) { return pos; });
-        X.coeffs = tile;
-        X.cstride = NC;
-        reg_dct_block<16, 16, true>(X, lfp, F.xb, r, gmask, valid);
-      }
+      const uint32_t seq = e & 1023;
+      setup_ctx(e, X, lfp, t);
+      constexpr uint32_t NC = 256;
+      float* tile = s_tiles + (threadIdx.x >> 4) * 3 * NC;
+      gather_dequant_tile(B, F, g, seq, tile, NC, NC, deq_of(X), r, 16, valid, stage, [&] { __syncwarp(gmask); },
+                          [](uint32_t pos) { return pos; });
+      X.coeffs = tile;
+      X.cstride = NC;
+      reg_dct_block<16, 16, true>(X, lfp, F.xb, r, gmask, valid);
     }
   }
 }

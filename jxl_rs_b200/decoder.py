@@ -242,6 +242,17 @@ class Batch(_BatchHandle):
         abi.check(self._lib, self._lib.jxg_batch_stream_status(self._h, f, out.ctypes.data_as(C.POINTER(C.c_int32)), n))
         return out
 
+    def transform_plan(self, f: int, num_groups: int = 0):
+        """Transform-class partition of the block plan of whole frame f (jxg_batch_read_transform_plan): counts
+        [groups, 8] u32 (classes 0..4, then zeros) and the varblock entries [groups, 1024] u32 (ordinal | bx << 10 |
+        by << 15 | transform type << 20), class after class.
+        num_groups: the frame's group count, needed for frames added with add_desc."""
+        n = num_groups or self.frames[f].info.num_groups
+        counts = np.zeros((n, 8), np.uint32)
+        seqs = np.zeros((n, 1024), np.uint32)
+        abi.check(self._lib, self._lib.jxg_batch_read_transform_plan(self._h, f, counts.ctypes.data, seqs.ctypes.data, n))
+        return counts, seqs
+
     def read_coeffs(self, f: int):
         n = self.frames[f].info.num_groups * 3 * 65536
         out = np.empty(n, np.int32)
