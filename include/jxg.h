@@ -353,12 +353,38 @@ int jxg_parsed_region_desc(void* parsed, uint32_t output_format, const JxgRegion
  * RGB u8 (grey replicated). Frames of one batch must agree on the kind of each inverse-transform step they share: one
  * frame's step list may be a prefix of another's, in either order of adding. A frame jxg_modular_batch_add refuses
  * leaves the batch as it was (no stream of it decodes, no statistic counts it); a group-local Squeeze is refused with
- * JXG_ERR_UNSUPPORTED. */
+ * JXG_ERR_UNSUPPORTED. A rectangle of a frame can be decoded alone (jxg_modular_batch_add_region). */
 int jxg_modular_parse_file(const uint8_t* data, size_t size, void** parsed, JxgImageInfo* info);
 void jxg_modular_parsed_free(void* parsed);
 int jxg_modular_batch_begin(void* ctx, void** batch);
 /* `parsed` must stay alive until jxg_modular_batch_end. */
 int jxg_modular_batch_add(void* batch, void* parsed, void* out, size_t out_row_stride, int out_is_device);
+
+/* ---- Region decode of Modular frames ----------------------------------------------------------------------------
+ * A region is a JxgRegion rectangle of the OUTPUT image (display orientation, the JxgImageInfo width x height of
+ * jxg_modular_parse_file). Its pixels are defined as the pixels of the whole-frame decode on that rectangle, and they
+ * are byte-identical to them for every orientation, host and device outputs and any valid stride: everything up to the
+ * u8 store is integer arithmetic. The output holds region.height rows of region.width RGB u8 pixels; the stride rule
+ * is that of jxg_modular_batch_add applied to the region's width (JXG_ERR_INVALID_OUTPUT). An empty region or one
+ * outside the image returns JXG_ERR_ARGUMENT; a frame jxg_modular_batch_add refuses is refused with the same code, and
+ * a refused region leaves the batch as it was. Only the group streams the region depends on are uploaded and decoded,
+ * and the global inverse transforms and the store run only on the rectangles it depends on (the dependency cone):
+ * RCT mixes the same position of its three channels, a palette look-up needs the palette whole, and an unsqueeze
+ * output depends on the outputs to its left (horizontal) or above (vertical), so on Squeeze frames the cone reaches the
+ * top-left corner of each squeeze level and a crop far from it needs most of the frame's streams. The plane memory of
+ * the frame is sized to the cone. jxg_modular_batch_wait reports the failing group by its index in the whole frame;
+ * jxg_modular_batch_read_planes refuses a region frame (JXG_ERR_ARGUMENT). Each region is its own frame of the batch,
+ * also when regions of one parsed frame overlap. */
+int jxg_modular_batch_add_region(void* batch, void* parsed, const JxgRegion* region, void* out, size_t out_row_stride,
+                                 int out_is_device);
+/* Parity tap, no device needed: the cone of a region as jxg_modular_batch_add_region computes it, after the same
+ * checks. groups[0 .. *n_groups): the ModularHF groups decoded (whole-frame indices, ascending). rects: 8 words per
+ * buffer of the frame's inverse plan (its coded channels first, then the outputs of the plan's steps in plan order):
+ * the rectangle the frame's plane memory holds of it, then the rectangle the region needs of it, each as
+ * x0, y0, x1, y1 (half-open; all zero when empty). groups and rects may be NULL; *n_groups and *n_buffers are always
+ * written, and JXG_ERR_ARGUMENT is returned when max_groups or max_buffers is smaller than they say. */
+int jxg_modular_parsed_region_plan(void* parsed, const JxgRegion* region, uint32_t* groups, uint32_t max_groups,
+                                   uint32_t* n_groups, uint32_t* rects, uint32_t max_buffers, uint32_t* n_buffers);
 /* Streams per warp of the decode kernel (1, 2 or 4; default 1). */
 int jxg_modular_batch_set_lanes(void* batch, int lanes_per_warp);
 int jxg_modular_batch_run(void* batch, void* cuda_stream);
@@ -366,7 +392,7 @@ int jxg_modular_batch_wait(void* batch, uint32_t* first_bad_frame, uint32_t* fir
 /* Ordered after the batch's own last run, whichever stream that ran on. */
 int jxg_modular_batch_rerun_device(void* batch, void* cuda_stream);
 /* Parity tap: final colour planes of frame f (3 x H x W i32, before the u8 conversion), after waiting for the
- * batch's own last run on whichever stream it ran. */
+ * batch's own last run on whichever stream it ran. JXG_ERR_ARGUMENT for a region frame. */
 int jxg_modular_batch_read_planes(void* batch, uint32_t f, int32_t* out, size_t out_len);
 /* ms[0]: whole batch on the device, ms[1]: group-stream decode kernel (+ local RCT). */
 int jxg_modular_batch_stats(void* batch, uint64_t* h2d_bytes, uint64_t* d2h_bytes, uint64_t* kernel_launches, float* ms);

@@ -81,7 +81,7 @@ EXPORTS = [
     "jxg_modular_batch_read_planes", "jxg_modular_batch_stats", "jxg_modular_batch_end", "jxg_modular_walk_table",
     "jxg_modular_batch_lz77_stats", "jxg_modular_batch_walk_stats", "jxg_batch_add_frame_region", "jxg_batch_add_parsed_region",
     "jxg_parsed_region_desc", "jxg_context_set_sm_budget", "jxg_batch_entropy_schedule", "jxg_batch_stream_status",
-    "jxg_batch_read_transform_plan",
+    "jxg_batch_read_transform_plan", "jxg_modular_batch_add_region", "jxg_modular_parsed_region_plan",
 ]
 
 ALL_FRAMES = 0xFFFFFFFF  # JXG_ALL_FRAMES
@@ -163,6 +163,8 @@ def load_library():
     lib.jxg_batch_add_parsed_region.argtypes = [vp, vp, C.c_uint32, rp, vp, C.c_size_t, C.c_int]
     lib.jxg_parsed_region_desc.argtypes = [vp, C.c_uint32, rp, C.POINTER(JxgFrameDesc), C.POINTER(vp), C.POINTER(vp),
                                            C.POINTER(vp), u32p, u32p, u32p]
+    lib.jxg_modular_batch_add_region.argtypes = [vp, vp, rp, vp, C.c_size_t, C.c_int]
+    lib.jxg_modular_parsed_region_plan.argtypes = [vp, rp, u32p, C.c_uint32, u32p, u32p, C.c_uint32, u32p]
     _LIB = lib
     return lib
 

@@ -14,6 +14,7 @@
 
 #include "../../../include/jxg.h"
 #include "../host/modular_frame.h"
+#include "../host/modular_region.h"
 #include "batch_common.h"
 #include "modular_device.h"
 
@@ -27,8 +28,10 @@ struct MFrame {
   void* out;
   size_t out_stride;
   bool out_is_device;
+  bool region = false;             // a region of the frame (jxg_modular_batch_add_region)
+  jxg::ModularRegionPlan plan;     // the cone: per buffer the rectangle the arena holds, the streams decoded
   uint64_t arena_base = 0;         // element offset of this frame's planes
-  std::vector<uint64_t> buf_off;   // per plan buffer, element offset in the arena
+  std::vector<uint64_t> buf_off;   // per plan buffer, element offset in the arena of its arena rectangle's top-left
   uint64_t host_planes_blob = 0;   // blob offset of the packed host-decoded planes
   uint64_t host_planes_elems = 0;
   size_t dev_out_off = 0;
@@ -107,7 +110,7 @@ uint64_t add_tree(ModularBatch* b, const jxg::ModularTree& t) {
       nodes[i * 4 + 2] = int32_t(n.left);
       nodes[i * 4 + 3] = 0;
     } else {
-      if (n.ctx >= (1u << 27)) throw jxg::Error(JXG_ERR_UNSUPPORTED, "MA tree too large for the device encoding");
+      if (n.ctx >= (1u << 27)) throw jxg::Error(JXG_ERR_UNSUPPORTED, "MA tree too large for the device encoding");  // check_tree
       nodes[i * 4 + 2] = int32_t(n.left | (n.ctx << 4));  // predictor | ctx << 4
       nodes[i * 4 + 3] = int32_t(n.right);                // multiplier
     }
@@ -244,33 +247,69 @@ struct BatchMark {
   }
 };
 
-// Plane arena: host-decoded coded channels first (one contiguous copy from the blob), then the rest.
+// Element index of pixel (x, y) of plan buffer i: its arena rectangle starts at buf_off[i], rows of the rectangle's width.
+uint32_t buf_stride(const MFrame& f, size_t i) { return f.plan.arena[i].w(); }
+int64_t buf_origin(const MFrame& f, size_t i) {  // the index of pixel (0, 0), outside the rectangle unless it starts there
+  const jxg::PlaneRect& r = f.plan.arena[i];
+  return int64_t(f.buf_off[i]) - int64_t(r.y0) * r.w() - int64_t(r.x0);
+}
+uint64_t buf_index(const MFrame& f, size_t i, uint32_t x, uint32_t y) { return uint64_t(buf_origin(f, i) + int64_t(y) * buf_stride(f, i) + x); }
+
+// Plane arena: per plan buffer its arena rectangle (the whole plane for a whole frame); host-decoded coded channels first
+// (one contiguous copy from the blob of their rectangles), then the rest.
 void add_arena(ModularBatch* b, MFrame& f) {
   const jxg::ModularFrameState* ms = f.ms;
+  const std::vector<jxg::PlaneRect>& ar = f.plan.arena;
   f.arena_base = b->arena_elems;
   f.buf_off.assign(ms->bufs.size(), 0);
   uint64_t cursor = f.arena_base;
   for (size_t c = 0; c < ms->coded.size(); c++)
     if (ms->host_decoded[c]) {
       f.buf_off[c] = cursor;
-      cursor += uint64_t(ms->bufs[c].w) * ms->bufs[c].h;
+      cursor += uint64_t(ar[c].w()) * ar[c].h();
     }
   f.host_planes_elems = cursor - f.arena_base;
   for (size_t i = 0; i < ms->bufs.size(); i++)
     if (i >= ms->coded.size() || !ms->host_decoded[i]) {
       cursor = (cursor + 3) & ~uint64_t(3);
       f.buf_off[i] = cursor;
-      cursor += uint64_t(ms->bufs[i].w) * ms->bufs[i].h;
+      cursor += uint64_t(ar[i].w()) * ar[i].h();
     }
   b->arena_elems = (cursor + 63) & ~uint64_t(63);
   if (f.host_planes_elems) {
     f.host_planes_blob = blob_append(b, nullptr, 0, 16);
-    for (size_t c = 0; c < ms->coded.size(); c++)
-      if (ms->host_decoded[c] && !ms->coded[c].data.empty()) blob_append(b, ms->coded[c].data.data(), ms->coded[c].data.size() * 4, 4);
+    for (size_t c = 0; c < ms->coded.size(); c++) {
+      const jxg::ModularChannel& ch = ms->coded[c];
+      if (!ms->host_decoded[c] || ar[c].empty() || ch.data.empty()) continue;
+      if (ar[c].w() == ch.w) {
+        blob_append(b, ch.row(ar[c].y0), size_t(ch.w) * ar[c].h() * 4, 4);
+      } else {
+        for (uint32_t y = ar[c].y0; y < ar[c].y1; y++) blob_append(b, ch.row(y) + ar[c].x0, size_t(ar[c].w()) * 4, 4);
+      }
+    }
   }
 }
 
-// Codes / trees, and per coded group stream its MStreamDev, rects, reference channels, local RCTs and LZ77 window.
+// What jxg_modular_batch_add refuses in any group stream, whether or not a region decodes it.
+void check_tree(const jxg::ModularTree& t) {
+  for (const jxg::TreeNode& n : t.nodes)
+    if (n.property < 0 && n.ctx >= (1u << 27)) throw jxg::Error(JXG_ERR_UNSUPPORTED, "MA tree too large for the device encoding");
+}
+void check_streams(const jxg::ModularFrameState* ms) {
+  for (const jxg::ModularGroupStream& st : ms->hf) {
+    if (st.empty) continue;
+    check_tree(st.local_tree ? *st.local_tree : ms->global_tree);
+    for (const jxg::ModularTransform& t : st.header.transforms) {
+      if (t.id != 0) throw jxg::Error(JXG_ERR_UNSUPPORTED, "only RCT is implemented as a group-local transform on the device path");
+      if (t.begin_channel + 3 > st.rects.size()) throw jxg::Error(jxg::kErrBitstream, "RCT channel range");
+      const jxg::ModularRect &r0 = st.rects[t.begin_channel], &r1 = st.rects[t.begin_channel + 1], &r2 = st.rects[t.begin_channel + 2];
+      if (r0.w != r1.w || r0.w != r2.w || r0.h != r1.h || r0.h != r2.h) throw jxg::Error(jxg::kErrBitstream, "RCT on channels of different size");
+    }
+  }
+}
+
+// Codes / trees, and per group stream the cone selects its MStreamDev, rects, reference channels, local RCTs and LZ77
+// window. The rects address the channels' arena rectangles; the stream keeps its whole-frame group index.
 void add_streams(ModularBatch* b, MFrame& f) {
   const jxg::ModularFrameState* ms = f.ms;
   uint32_t global_code = 0;
@@ -278,8 +317,9 @@ void add_streams(ModularBatch* b, MFrame& f) {
   bool have_global = false;
   std::map<WalkKey, WalkInfo> walk_cache;
   std::map<uint64_t, bool> inner_static;
-  for (const jxg::ModularGroupStream& st : ms->hf) {
-    if (st.empty) continue;
+  for (size_t g = 0; g < ms->hf.size(); g++) {
+    const jxg::ModularGroupStream& st = ms->hf[g];
+    if (!f.plan.selected[g]) continue;
     const jxg::ModularTree* tree = st.local_tree ? st.local_tree.get() : &ms->global_tree;
     MStreamDev d;
     memset(&d, 0, sizeof(d));
@@ -311,8 +351,8 @@ void add_streams(ModularBatch* b, MFrame& f) {
     for (size_t ri = 0; ri < st.rects.size(); ri++) {
       const jxg::ModularRect& r = st.rects[ri];
       MRectDev rd;
-      rd.stride = ms->coded[r.chan].w;
-      rd.base = f.buf_off[r.chan] + uint64_t(r.y0) * rd.stride + r.x0;
+      rd.stride = buf_stride(f, r.chan);
+      rd.base = buf_index(f, r.chan, r.x0, r.y0);
       rd.w = r.w;
       rd.h = r.h;
       rd.walk = kWalkGeneric;
@@ -362,13 +402,7 @@ void add_streams(ModularBatch* b, MFrame& f) {
       b->wp_bytes += (size_t(max_w + 1) * (8 + 2) * 4 + 63) & ~size_t(63);
     }
     d.first_rct = uint32_t(b->rcts.size());
-    for (const jxg::ModularTransform& t : st.header.transforms) {
-      if (t.id != 0) throw jxg::Error(JXG_ERR_UNSUPPORTED, "only RCT is implemented as a group-local transform on the device path");
-      if (t.begin_channel + 3 > st.rects.size()) throw jxg::Error(jxg::kErrBitstream, "RCT channel range");
-      const jxg::ModularRect &r0 = st.rects[t.begin_channel], &r1 = st.rects[t.begin_channel + 1], &r2 = st.rects[t.begin_channel + 2];
-      if (r0.w != r1.w || r0.w != r2.w || r0.h != r1.h || r0.h != r2.h) throw jxg::Error(jxg::kErrBitstream, "RCT on channels of different size");
-      b->rcts.push_back(MRctDev{t.begin_channel, t.rct_type});
-    }
+    for (const jxg::ModularTransform& t : st.header.transforms) b->rcts.push_back(MRctDev{t.begin_channel, t.rct_type});  // check_streams
     d.num_rct = uint32_t(b->rcts.size()) - d.first_rct;
     if (d.num_rct) b->rct_streams.push_back(uint32_t(b->streams.size()));
     if (tree->code.lz77_enabled) {
@@ -384,9 +418,17 @@ void add_streams(ModularBatch* b, MFrame& f) {
   }
 }
 
-// Global inverse plan -> jobs per level. A frame with fewer steps than the batch has levels has no jobs in the last
-// ones; levels are launched in order and the store runs after all of them, so only the kinds of the common steps must
-// agree, whatever the order of adding.
+void set_rect(MJobDev& j, const jxg::PlaneRect& r) {
+  j.x0 = r.x0;
+  j.y0 = r.y0;
+  j.x1 = r.x1;
+  j.y1 = r.y1;
+}
+
+// Global inverse plan -> jobs per level, each on the rectangle the cone gives its step; a step the region does not
+// need has no job. A frame with fewer steps than the batch has levels has no jobs in the last ones; levels are launched
+// in order and the store runs after all of them, so only the kinds of the common steps must agree, whatever the order
+// of adding.
 void add_plan(ModularBatch* b, const MFrame& f) {
   const jxg::ModularFrameState* ms = f.ms;
   for (size_t si = 0; si < ms->steps.size(); si++) {
@@ -399,9 +441,12 @@ void add_plan(ModularBatch* b, const MFrame& f) {
       throw jxg::Error(JXG_ERR_UNSUPPORTED, "frames of one Modular batch must share the global transform structure");
     MJobDev j;
     memset(&j, 0, sizeof(j));
-    j.a = f.buf_off[s.a];
-    j.b = f.buf_off[s.b];
-    j.c = f.buf_off[s.c];
+    j.a = buf_origin(f, s.a);
+    j.b = buf_origin(f, s.b);
+    j.c = buf_origin(f, s.c);
+    j.sa = buf_stride(f, s.a);
+    j.sb = buf_stride(f, s.b);
+    j.sc = buf_stride(f, s.c);
     j.w = ms->bufs[s.a].w;
     j.h = ms->bufs[s.a].h;
     j.rw = s.kind == jxg::kJobHSqueeze ? ms->bufs[s.b].w : (s.kind == jxg::kJobVSqueeze ? ms->bufs[s.b].h : 0);
@@ -409,50 +454,81 @@ void add_plan(ModularBatch* b, const MFrame& f) {
     if (s.kind == jxg::kJobPalette) {  // one job per colour channel: a index plane, b palette plane (row c = component c), c output
       if (ms->bufs[s.b].h < s.n || ms->bufs[s.b].w < s.num_colors) throw jxg::Error(jxg::kErrBitstream, "palette channel smaller than its header says");
       for (uint32_t c = 0; c < s.n; c++) {
-        j.c = f.buf_off[s.c + c];
+        if (f.plan.need[s.c + c].empty()) continue;
+        j.c = buf_origin(f, s.c + c);
+        j.sc = buf_stride(f, s.c + c);
+        set_rect(j, f.plan.need[s.c + c]);
         j.rw = s.num_colors;
         j.op = c;
-        j.out_stride = ms->bufs[s.b].w;  // palette row stride
         b->levels[si].push_back(j);
       }
       continue;
     }
+    if (f.plan.step[si].empty()) continue;
+    set_rect(j, f.plan.step[si]);
     b->levels[si].push_back(j);
   }
 }
 
-// Store job: the final colour planes -> the u8 output, in the file's orientation (render/save.rs).
+// Store job: the coded window of the final colour planes -> the u8 output, in the file's orientation (render/save.rs).
 void add_store(ModularBatch* b, MFrame& f) {
   const jxg::ModularFrameState* ms = f.ms;
   const uint32_t W = ms->header.xsize(), H = ms->header.ysize();
   MJobDev sj;
   memset(&sj, 0, sizeof(sj));
   const uint32_t nc = ms->num_color_channels;
-  sj.a = f.buf_off[ms->out_buf[0]];
-  sj.b = f.buf_off[ms->out_buf[nc > 1 ? 1 : 0]];
-  sj.c = f.buf_off[ms->out_buf[nc > 2 ? 2 : 0]];
+  const uint32_t ob[3] = {ms->out_buf[0], ms->out_buf[nc > 1 ? 1 : 0], ms->out_buf[nc > 2 ? 2 : 0]};
+  sj.a = buf_origin(f, ob[0]);
+  sj.b = buf_origin(f, ob[1]);
+  sj.c = buf_origin(f, ob[2]);
+  sj.sa = buf_stride(f, ob[0]);
+  sj.sb = buf_stride(f, ob[1]);
+  sj.sc = buf_stride(f, ob[2]);
+  set_rect(sj, f.plan.coded);
   sj.w = W;
   sj.h = H;
   sj.op = ms->file.orientation;
-  for (uint32_t c = 0; c < nc; c++)
-    if (ms->bufs[ms->out_buf[c]].w != W || ms->bufs[ms->out_buf[c]].h != H)
-      throw jxg::Error(jxg::kErrBitstream, "unexpected output channel size");
+  sj.out_x = f.plan.out_x;
+  sj.out_y = f.plan.out_y;
   if (!f.out_is_device) {
     f.dev_out_off = b->out_bytes;
-    b->out_bytes += (size_t(W) * H * 3 + 255) & ~size_t(255);
+    b->out_bytes += (size_t(f.plan.out_w) * f.plan.out_h * 3 + 255) & ~size_t(255);
   }
   b->store_jobs.push_back(sj);
 }
 
-void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, void* out, size_t stride, bool is_device) {
+// The frame checks of jxg_modular_batch_add, for the whole frame and for any region of it alike.
+void check_frame(const jxg::ModularFrameState* ms) {
   if (!ms->device_plan_ok)
     throw jxg::Error(JXG_ERR_UNSUPPORTED, "palette transforms with delta entries or a predictor are not implemented on the device path");
   if (ms->toc.offsets.size() == 1 && !ms->hf[0].empty)
     throw jxg::Error(JXG_ERR_UNSUPPORTED, "single-section Modular frames with a coded group are not on the device path");
+}
+void check_plan(const jxg::ModularFrameState* ms) {
+  check_streams(ms);
+  for (const jxg::ModularStep& s : ms->steps)
+    if (s.kind == jxg::kJobPalette && (ms->bufs[s.b].h < s.n || ms->bufs[s.b].w < s.num_colors))
+      throw jxg::Error(jxg::kErrBitstream, "palette channel smaller than its header says");
   const uint32_t W = ms->header.xsize(), H = ms->header.ysize();
-  if (stride < size_t(ms->file.orientation >= 5 ? H : W) * 3) throw jxg::Error(JXG_ERR_INVALID_OUTPUT, "output row stride too small");
+  for (uint32_t c = 0; c < ms->num_color_channels; c++)
+    if (ms->bufs[ms->out_buf[c]].w != W || ms->bufs[ms->out_buf[c]].h != H)
+      throw jxg::Error(jxg::kErrBitstream, "unexpected output channel size");
+}
+
+// The cone of `region` (nullptr: the whole frame), after the frame checks; throws what jxg_modular_batch_add refuses.
+void plan_frame(const jxg::ModularFrameState* ms, const JxgRegion* region, jxg::ModularRegionPlan& plan) {
+  const char* why = "";
+  if (int r = jxg::plan_modular_region(*ms, region, plan, &why)) throw jxg::Error(r, why);
+  check_frame(ms);
+}
+
+void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, const JxgRegion* region, void* out, size_t stride, bool is_device) {
   MFrame f;
+  plan_frame(ms, region, f.plan);
+  if (stride < size_t(f.plan.out_w) * 3) throw jxg::Error(JXG_ERR_INVALID_OUTPUT, "output row stride too small");
+  check_plan(ms);
   f.ms = ms;
+  f.region = region != nullptr;
   f.out = out;
   f.out_stride = stride;
   f.out_is_device = is_device;
@@ -493,8 +569,8 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
   auto launch_jobs = [&](jxg::ModularJobKind kind, const std::vector<MJobDev>& level) {
     uint32_t mw = 0, mh = 0;
     for (const MJobDev& j : level) {
-      mw = std::max(mw, j.w);
-      mh = std::max(mh, j.h);
+      mw = std::max(mw, j.x1 - j.x0);
+      mh = std::max(mh, j.y1 - j.y0);
     }
     launch_modular_jobs(kind, jobs, uint32_t(level.size()), mw, mh, B.planes, schedule_sms(cx), s);
     jobs += level.size();
@@ -505,8 +581,7 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
   if (copy_to_host) {
     for (const MFrame& f : b->frames)
       if (!f.out_is_device) {
-        const bool tr = f.ms->file.orientation >= 5;  // display size
-        const uint32_t W = tr ? f.ms->header.ysize() : f.ms->header.xsize(), H = tr ? f.ms->header.xsize() : f.ms->header.ysize();
+        const uint32_t W = f.plan.out_w, H = f.plan.out_h;  // display size of the frame or region
         CUDA_TRY(cudaMemcpy2DAsync(f.out, f.out_stride, static_cast<uint8_t*>(cx->d_out.p) + f.dev_out_off, size_t(W) * 3,
                                    size_t(W) * 3, H, cudaMemcpyDeviceToHost, s));
         b->d2h += size_t(W) * 3 * H;
@@ -562,10 +637,53 @@ int jxg_modular_batch_add(void* bp, void* parsed, void* out, size_t out_row_stri
   if (b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch already submitted");
   const BatchMark mark(b);
   try {
-    add_frame(b, static_cast<jxg::ModularFrameState*>(parsed), out, out_row_stride, out_is_device != 0);
+    add_frame(b, static_cast<jxg::ModularFrameState*>(parsed), nullptr, out, out_row_stride, out_is_device != 0);
     return JXG_OK;
   } catch (jxg::Error& e) {
     mark.restore(b);  // a refused frame leaves nothing behind: no streams decode for it, no stats count it
+    return set_error(e.code, e.what());
+  }
+}
+
+int jxg_modular_batch_add_region(void* bp, void* parsed, const JxgRegion* region, void* out, size_t out_row_stride,
+                                 int out_is_device) {
+  ModularBatch* b = static_cast<ModularBatch*>(bp);
+  if (!b || !parsed || !region || !out) return JXG_ERR_ARGUMENT;
+  if (b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch already submitted");
+  const BatchMark mark(b);
+  try {
+    add_frame(b, static_cast<jxg::ModularFrameState*>(parsed), region, out, out_row_stride, out_is_device != 0);
+    return JXG_OK;
+  } catch (jxg::Error& e) {
+    mark.restore(b);
+    return set_error(e.code, e.what());
+  }
+}
+
+int jxg_modular_parsed_region_plan(void* parsed, const JxgRegion* region, uint32_t* groups, uint32_t max_groups,
+                                   uint32_t* n_groups, uint32_t* rects, uint32_t max_buffers, uint32_t* n_buffers) {
+  if (!parsed || !region || !n_groups || !n_buffers) return JXG_ERR_ARGUMENT;
+  const jxg::ModularFrameState* ms = static_cast<const jxg::ModularFrameState*>(parsed);
+  try {
+    jxg::ModularRegionPlan plan;
+    plan_frame(ms, region, plan);
+    check_plan(ms);
+    std::vector<uint32_t> sel;
+    for (size_t g = 0; g < plan.selected.size(); g++)
+      if (plan.selected[g]) sel.push_back(ms->hf[g].group);
+    *n_groups = uint32_t(sel.size());
+    *n_buffers = uint32_t(plan.need.size());
+    if ((groups && max_groups < sel.size()) || (rects && max_buffers < plan.need.size()))
+      return set_error(JXG_ERR_ARGUMENT, "region plan: output arrays too small");
+    if (groups) std::copy(sel.begin(), sel.end(), groups);
+    if (rects)
+      for (size_t i = 0; i < plan.need.size(); i++) {
+        const jxg::PlaneRect &a = plan.arena[i], &n = plan.need[i];
+        const uint32_t v[8] = {a.x0, a.y0, a.x1, a.y1, n.x0, n.y0, n.x1, n.y1};
+        std::copy(v, v + 8, rects + i * 8);
+      }
+    return JXG_OK;
+  } catch (jxg::Error& e) {
     return set_error(e.code, e.what());
   }
 }
@@ -605,8 +723,7 @@ int jxg_modular_batch_run(void* bp, void* cuda_stream) {
   for (size_t i = 0; i < b->frames.size(); i++) {
     MFrame& f = b->frames[i];
     b->store_jobs[i].out = f.out_is_device ? f.out : static_cast<uint8_t*>(cx->d_out.p) + f.dev_out_off;
-    b->store_jobs[i].out_stride =
-        f.out_is_device ? f.out_stride : size_t(f.ms->file.orientation >= 5 ? f.ms->header.ysize() : f.ms->header.xsize()) * 3;
+    b->store_jobs[i].out_stride = f.out_is_device ? f.out_stride : size_t(f.plan.out_w) * 3;
   }
   if (int r = batch_status(*b, b->streams.size())) return r;
   std::vector<MJobDev> all_jobs;
@@ -654,8 +771,9 @@ int jxg_modular_batch_wait(void* bp, uint32_t* bad_frame, uint32_t* bad_group) {
 int jxg_modular_batch_read_planes(void* bp, uint32_t f, int32_t* out, size_t out_len) {
   ModularBatch* b = static_cast<ModularBatch*>(bp);
   if (!b || !b->uploaded || f >= b->frames.size() || !out) return JXG_ERR_ARGUMENT;
+  if (b->frames[f].region) return set_error(JXG_ERR_ARGUMENT, "read_planes: a region frame holds no whole planes");
   if (int r = batch_wait_last_run(*b)) return r;
-  const MJobDev& j = b->store_jobs[f];
+  const MJobDev& j = b->store_jobs[f];  // a whole frame: the planes are whole, rows of width w
   const size_t n = size_t(j.w) * j.h;
   if (out_len < 3 * n) return set_error(JXG_ERR_ARGUMENT, "plane buffer too small");
   const int32_t* planes = static_cast<const int32_t*>(b->ctx->d_planes_a.p);

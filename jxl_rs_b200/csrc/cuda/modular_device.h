@@ -49,11 +49,18 @@ struct MRctDev {
   uint32_t begin, type;
 };
 
-struct MJobDev {  // one global transform / store job (element offsets into the plane arena)
-  uint64_t a, b, c;
+// One global transform / store job. A buffer's pixel (x, y) is planes[a + y * sa + x] (b, c alike): a is the element
+// index of the buffer's pixel (0, 0), outside the arena when the buffer's arena rectangle does not start there (a region
+// frame); only pixels inside that rectangle are touched. The job's rectangle [x0, x1) x [y0, y1), in the coordinates
+// of the buffers it writes, is the whole frame's planes for a whole frame (see each kernel).
+struct MJobDev {
+  int64_t a, b, c;
+  uint32_t sa, sb, sc;
+  uint32_t x0, y0, x1, y1;
   uint32_t w, h, rw, op;
   void* out;
   uint64_t out_stride;
+  uint32_t out_x, out_y;  // store: display coordinates of the output's top-left pixel
 };
 
 struct MBatchDev {
@@ -80,7 +87,7 @@ struct MBatchDev {
 int launch_modular_decode(const MBatchDev& B, uint32_t num_plain, uint32_t lanes_per_warp, uint32_t num_rct_streams,
                           uint32_t sms, cudaStream_t stream);
 // kind: a jxg::ModularJobKind (host/modular_frame.h): 0 RCT, 1 horizontal unsqueeze, 2 vertical unsqueeze, 3 store,
-// 4 palette look-up
+// 4 palette look-up. max_w / max_h: the largest x1 - x0 / y1 - y0 of the jobs.
 void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint32_t max_w, uint32_t max_h, int32_t* planes,
                          uint32_t sms, cudaStream_t stream);
 

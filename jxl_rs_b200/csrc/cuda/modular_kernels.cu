@@ -5,7 +5,8 @@
 //                      streams with LZ77 in a launch of their own        predict.rs:148-527, decode/common.rs:85,
 //                                                                        entropy_coding/decode.rs:286-330
 //   k_modular_local_rct  inverse RCT of a group's local transforms     <- transforms/rct.rs:9-40 (apply_local.rs)
-//   k_modular_rct / k_unsqueeze_h / k_unsqueeze_v  global inverse transforms over full planes
+//   k_modular_rct / k_unsqueeze_h / k_unsqueeze_v  global inverse transforms over the job rectangles (full planes for
+//                                                    a whole frame, the dependency cone of a region, host/modular_region.h)
 //                                                                     <- transforms/rct.rs, squeeze.rs:144-195,390,577
 //   k_modular_store    i32 planes -> interleaved RGB u8                <- render/stages/convert.rs:642-690
 // Integer work throughout: results are bit-exact against the CPU path (tests/test_gpu_modular.py).
@@ -667,16 +668,21 @@ __global__ void __launch_bounds__(256) k_modular_local_rct(const MBatchDev B) {
   }
 }
 
-// Global RCT over full planes, in place (the permutation is applied by the host to the buffer ids).
+// Global RCT over the job rectangle, in place (the permutation is applied by the host to the buffer ids): rows
+// grid-strided over the CTAs, columns over the threads.
 __global__ void __launch_bounds__(256) k_modular_rct(const MJobDev* jobs, int32_t* planes) {
   const MJobDev j = jobs[blockIdx.y];
-  const size_t n = size_t(j.w) * j.h;
-  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
-    int32_t v0 = planes[j.a + i], v1 = planes[j.b + i], v2 = planes[j.c + i];
-    inv_rct_op(j.op, v0, v1, v2);
-    planes[j.a + i] = v0;
-    planes[j.b + i] = v1;
-    planes[j.c + i] = v2;
+  for (uint32_t y = j.y0 + blockIdx.x; y < j.y1; y += gridDim.x) {
+    int32_t* const pa = planes + (j.a + int64_t(y) * j.sa);
+    int32_t* const pb = planes + (j.b + int64_t(y) * j.sb);
+    int32_t* const pc = planes + (j.c + int64_t(y) * j.sc);
+    for (uint32_t x = j.x0 + threadIdx.x; x < j.x1; x += blockDim.x) {
+      int32_t v0 = pa[x], v1 = pb[x], v2 = pc[x];
+      inv_rct_op(j.op, v0, v1, v2);
+      pa[x] = v0;
+      pb[x] = v1;
+      pc[x] = v2;
+    }
   }
 }
 
@@ -696,17 +702,18 @@ __device__ __forceinline__ int64_t smooth_tendency(int64_t b, int64_t a, int64_t
 }
 
 // Horizontal unsqueeze (squeeze.rs:390): one thread per output row, serial along x (each output depends on the one
-// to its left). job: a = avg (w x h), b = residual (rw x h), c = out ((w + rw) x h).
+// to its left). job: a = avg (w x h), b = residual (rw x h), c = out ((w + rw) x h); rows [y0, y1), output columns
+// [0, x1): x1 / 2 pairs from column 0, then the tail column (the last average) when x1 is odd (x1 = w + rw).
 __global__ void __launch_bounds__(128) k_unsqueeze_h(const MJobDev* jobs, int32_t* planes) {
   const MJobDev j = jobs[blockIdx.y];
-  const uint32_t y = blockIdx.x * blockDim.x + threadIdx.x;
-  if (y >= j.h) return;
-  const uint32_t aw = j.w, rw = j.rw, ow = aw + rw;
-  const int32_t* a = planes + j.a + size_t(y) * aw;
-  const int32_t* r = planes + j.b + size_t(y) * rw;
-  int32_t* o = planes + j.c + size_t(y) * ow;
+  const uint32_t y = j.y0 + blockIdx.x * blockDim.x + threadIdx.x;
+  if (y >= j.y1) return;
+  const uint32_t aw = j.w, pairs = j.x1 >> 1;
+  const int32_t* a = planes + (j.a + int64_t(y) * j.sa);
+  const int32_t* r = planes + (j.b + int64_t(y) * j.sb);
+  int32_t* o = planes + (j.c + int64_t(y) * j.sc);
   int64_t av = aw ? a[0] : 0, left = av;
-  for (uint32_t x = 0; x < rw; x++) {
+  for (uint32_t x = 0; x < pairs; x++) {
     const int64_t next_avg = x + 1 < aw ? a[x + 1] : av;
     const int64_t diff = int64_t(r[x]) + smooth_tendency(left, av, next_avg);
     const int64_t A = av + diff / 2;
@@ -716,53 +723,57 @@ __global__ void __launch_bounds__(128) k_unsqueeze_h(const MJobDev* jobs, int32_
     left = int32_t(left);
     av = next_avg;
   }
-  if (ow & 1) o[ow - 1] = a[aw - 1];
+  if (j.x1 & 1) o[j.x1 - 1] = a[aw - 1];
 }
 
 // Vertical unsqueeze (squeeze.rs:577): one thread per column, serial along y, coalesced across x.
-// job: a = avg (w x h), b = residual (w x rh), c = out (w x (h + rh)); rw holds rh.
+// job: a = avg (w x h), b = residual (w x rh), c = out (w x (h + rh)); rw holds rh. Columns [x0, x1), output rows
+// [0, y1): y1 / 2 pairs from row 0, then the tail row when y1 is odd (y1 = h + rh).
 __global__ void __launch_bounds__(128) k_unsqueeze_v(const MJobDev* jobs, int32_t* planes) {
   const MJobDev j = jobs[blockIdx.y];
-  const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-  if (x >= j.w) return;
-  const uint32_t w = j.w, ah = j.h, rh = j.rw, oh = ah + rh;
-  const int32_t* a = planes + j.a + x;
-  const int32_t* r = planes + j.b + x;
-  int32_t* o = planes + j.c + x;
+  const uint32_t x = j.x0 + blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= j.x1) return;
+  const uint32_t ah = j.h, pairs = j.y1 >> 1;
+  const size_t sa = j.sa, sb = j.sb, sc = j.sc;
+  const int32_t* a = planes + (j.a + x);
+  const int32_t* r = planes + (j.b + x);
+  int32_t* o = planes + (j.c + x);
   int64_t av = ah ? a[0] : 0, up = av;
-  for (uint32_t y = 0; y < rh; y++) {
-    const int64_t next_avg = y + 1 < ah ? a[size_t(y + 1) * w] : av;
-    const int64_t diff = int64_t(r[size_t(y) * w]) + smooth_tendency(up, av, next_avg);
+  for (uint32_t y = 0; y < pairs; y++) {
+    const int64_t next_avg = y + 1 < ah ? a[(y + 1) * sa] : av;
+    const int64_t diff = int64_t(r[y * sb]) + smooth_tendency(up, av, next_avg);
     const int64_t A = av + diff / 2;
-    o[size_t(2 * y) * w] = int32_t(A);
+    o[(2 * y) * sc] = int32_t(A);
     up = int32_t(A - diff);
-    o[size_t(2 * y + 1) * w] = int32_t(up);
+    o[(2 * y + 1) * sc] = int32_t(up);
     av = next_avg;
   }
-  if (oh & 1) o[size_t(oh - 1) * w] = a[size_t(ah - 1) * w];
+  if (j.y1 & 1) o[(j.y1 - 1) * sc] = a[(ah - 1) * sa];
 }
 
-// i32 planes -> interleaved RGB u8, clamped (convert.rs:675-680). job: a, b, c = R, G, B planes (w x h), op = orientation.
+// i32 planes -> interleaved RGB u8, clamped (convert.rs:675-680). job: a, b, c = R, G, B planes (w x h, the coded
+// frame), op = orientation; the coded window [x0, x1) x [y0, y1) goes to the output whose top-left pixel is display
+// pixel (out_x, out_y). Rows grid-strided over the CTAs, columns over the threads.
 __global__ void __launch_bounds__(256) k_modular_store(const MJobDev* jobs, const int32_t* planes) {
   const MJobDev j = jobs[blockIdx.y];
-  const size_t n = size_t(j.w) * j.h;
-  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
-    const uint32_t y = uint32_t(i / j.w), x = uint32_t(i - size_t(y) * j.w);
-    uint32_t dx = x, dy = y;
-    switch (j.op) {  // ImageMetadata.orientation (headers/image_metadata.rs:85-96 display_pixel); 1 = identity
-      case 2: dx = j.w - 1 - x; break;
-      case 3: dx = j.w - 1 - x; dy = j.h - 1 - y; break;
-      case 4: dy = j.h - 1 - y; break;
-      case 5: dx = y; dy = x; break;
-      case 6: dx = j.h - 1 - y; dy = x; break;
-      case 7: dx = j.h - 1 - y; dy = j.w - 1 - x; break;
-      case 8: dx = y; dy = j.w - 1 - x; break;
-      default: break;
+  for (uint32_t y = j.y0 + blockIdx.x; y < j.y1; y += gridDim.x) {
+    for (uint32_t x = j.x0 + threadIdx.x; x < j.x1; x += blockDim.x) {
+      uint32_t dx = x, dy = y;
+      switch (j.op) {  // ImageMetadata.orientation (headers/image_metadata.rs:85-96 display_pixel); 1 = identity
+        case 2: dx = j.w - 1 - x; break;
+        case 3: dx = j.w - 1 - x; dy = j.h - 1 - y; break;
+        case 4: dy = j.h - 1 - y; break;
+        case 5: dx = y; dy = x; break;
+        case 6: dx = j.h - 1 - y; dy = x; break;
+        case 7: dx = j.h - 1 - y; dy = j.w - 1 - x; break;
+        case 8: dx = y; dy = j.w - 1 - x; break;
+        default: break;
+      }
+      uint8_t* d = static_cast<uint8_t*>(j.out) + size_t(dy - j.out_y) * j.out_stride + size_t(dx - j.out_x) * 3;
+      d[0] = uint8_t(min(max(planes[j.a + int64_t(y) * j.sa + x], 0), 255));
+      d[1] = uint8_t(min(max(planes[j.b + int64_t(y) * j.sb + x], 0), 255));
+      d[2] = uint8_t(min(max(planes[j.c + int64_t(y) * j.sc + x], 0), 255));
     }
-    uint8_t* d = static_cast<uint8_t*>(j.out) + size_t(dy) * j.out_stride + size_t(dx) * 3;
-    d[0] = uint8_t(min(max(planes[j.a + i], 0), 255));
-    d[1] = uint8_t(min(max(planes[j.b + i], 0), 255));
-    d[2] = uint8_t(min(max(planes[j.c + i], 0), 255));
   }
 }
 
@@ -847,34 +858,33 @@ __device__ __forceinline__ int32_t palette_value8(const int32_t* pal, uint32_t p
   return pal[size_t(c) * pal_stride + idx];
 }
 
-// Inverse palette without delta entries (palette.rs:165-199): out[c][p] = palette_value(index[p], c). One job per colour
-// channel (blockIdx.y), grid-stride over the pixels.
+// Inverse palette without delta entries (palette.rs:165-199): out[c][p] = palette_value(index[p], c) over the job
+// rectangle. One job per colour channel (blockIdx.y); rows grid-strided over the CTAs, columns over the threads. The
+// palette plane b is held whole: row c = component c.
 __global__ void __launch_bounds__(256) k_modular_palette(const MJobDev* jobs, int32_t* planes) {
   const MJobDev j = jobs[blockIdx.y];
-  const size_t n = size_t(j.w) * j.h;
-  const int32_t* index = planes + j.a;
   const int32_t* pal = planes + j.b;
-  int32_t* out = planes + j.c;
-  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x)
-    out[i] = palette_value8(pal, uint32_t(j.out_stride), index[i], j.op, j.rw);
+  for (uint32_t y = j.y0 + blockIdx.x; y < j.y1; y += gridDim.x) {
+    const int32_t* index = planes + (j.a + int64_t(y) * j.sa);
+    int32_t* out = planes + (j.c + int64_t(y) * j.sc);
+    for (uint32_t x = j.x0 + threadIdx.x; x < j.x1; x += blockDim.x) out[x] = palette_value8(pal, j.sb, index[x], j.op, j.rw);
+  }
 }
 
 void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint32_t max_w, uint32_t max_h, int32_t* planes,
                          uint32_t sms, cudaStream_t stream) {
   if (!num_jobs) return;
+  const uint32_t rows = max(min(max_h, sms * 16), 1u);  // grid of the row-strided kernels
   if (kind == 0) {
-    const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sms) * 16));
-    k_modular_rct<<<dim3(max(gx, 1u), num_jobs), 256, 0, stream>>>(jobs, planes);
+    k_modular_rct<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes);
   } else if (kind == 1) {  // a level can hold only empty channels (a squeeze of a zero-height residual): one idle block
     k_unsqueeze_h<<<dim3(max((max_h + 127) / 128, 1u), num_jobs), 128, 0, stream>>>(jobs, planes);
   } else if (kind == 2) {
     k_unsqueeze_v<<<dim3(max((max_w + 127) / 128, 1u), num_jobs), 128, 0, stream>>>(jobs, planes);
   } else if (kind == 4) {
-    const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sms) * 16));
-    k_modular_palette<<<dim3(max(gx, 1u), num_jobs), 256, 0, stream>>>(jobs, planes);
+    k_modular_palette<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes);
   } else {
-    const uint32_t gx = uint32_t(min((size_t(max_w) * max_h + 255) / 256, size_t(sms) * 16));
-    k_modular_store<<<dim3(max(gx, 1u), num_jobs), 256, 0, stream>>>(jobs, planes);
+    k_modular_store<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes);
   }
 }
 

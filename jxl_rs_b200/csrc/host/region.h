@@ -30,6 +30,35 @@ struct RegionSlice {
   std::vector<int8_t> ytox_map, ytob_map;
 };
 
+// Coded pixel of display pixel (dx, dy) for a coded w x h frame: the inverse of display_pixel
+// (headers/image_metadata.rs:85-96, k_orient).
+inline void coded_pixel(uint32_t o, uint32_t w, uint32_t h, uint32_t dx, uint32_t dy, uint32_t& x, uint32_t& y) {
+  switch (o) {
+    case 2: x = w - 1 - dx; y = dy; break;
+    case 3: x = w - 1 - dx; y = h - 1 - dy; break;
+    case 4: x = dx; y = h - 1 - dy; break;
+    case 5: x = dy; y = dx; break;
+    case 6: x = dy; y = h - 1 - dx; break;
+    case 7: x = w - 1 - dy; y = h - 1 - dx; break;
+    case 8: x = w - 1 - dy; y = dx; break;
+    default: x = dx; y = dy; break;
+  }
+}
+
+// display_pixel itself.
+inline void display_pixel(uint32_t o, uint32_t w, uint32_t h, uint32_t x, uint32_t y, uint32_t& dx, uint32_t& dy) {
+  switch (o) {
+    case 2: dx = w - 1 - x; dy = y; break;
+    case 3: dx = w - 1 - x; dy = h - 1 - y; break;
+    case 4: dx = x; dy = h - 1 - y; break;
+    case 5: dx = y; dy = x; break;
+    case 6: dx = h - 1 - y; dy = x; break;
+    case 7: dx = h - 1 - y; dy = w - 1 - x; break;
+    case 8: dx = y; dy = w - 1 - x; break;
+    default: dx = x; dy = y; break;
+  }
+}
+
 // Geometry of the fused filter kernel the selection depends on: its 64x32 tile (kTW x kTH, launch.h kFusedTileW / H)
 // and its halo in pixels, Gaborish 1 + EPF 2 / +1 / +3 (FCfg<GAB, EPF>::H). kernels.cu checks both against the kernel's
 // own constants at compile time.

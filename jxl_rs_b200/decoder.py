@@ -538,6 +538,22 @@ class ModularParsedFrame:
     def height(self):
         return self.info.height
 
+    def region_plan(self, region):
+        """The dependency cone of a region (x, y, w, h in output coordinates; jxg_modular_parsed_region_plan), no device
+        needed: (groups, arena, need) with groups the whole-frame indices of the group streams decoded, and per buffer
+        of the inverse plan the rectangle the plane memory holds and the one the region needs, as (x0, y0, x1, y1)
+        half-open, (0, 0, 0, 0) when empty."""
+        reg = C.byref(_region(region))
+        ng, nb = C.c_uint32(), C.c_uint32()
+        abi.check(self._lib, self._lib.jxg_modular_parsed_region_plan(self._h, reg, None, 0, C.byref(ng), None, 0,
+                                                                      C.byref(nb)))
+        groups = (C.c_uint32 * max(ng.value, 1))()
+        rects = (C.c_uint32 * max(8 * nb.value, 1))()
+        abi.check(self._lib, self._lib.jxg_modular_parsed_region_plan(self._h, reg, groups, ng.value, C.byref(ng), rects,
+                                                                      nb.value, C.byref(nb)))
+        r = [tuple(rects[i * 8:i * 8 + 8]) for i in range(nb.value)]
+        return list(groups[:ng.value]), [t[:4] for t in r], [t[4:] for t in r]
+
     def __del__(self):
         if getattr(self, "_h", None) and self._h.value:
             self._lib.jxg_modular_parsed_free(self._h)
@@ -553,9 +569,15 @@ class ModularBatch(_BatchHandle):
         abi.check(self._lib, self._lib.jxg_modular_batch_set_lanes(self._h, lanes_per_warp))
         self.frames = []
 
-    def add(self, frame: ModularParsedFrame, out_ptr: int, row_stride: int, out_is_device: bool):
-        abi.check(self._lib, self._lib.jxg_modular_batch_add(self._h, frame._h, C.c_void_p(out_ptr), row_stride,
-                                                             1 if out_is_device else 0))
+    def add(self, frame: ModularParsedFrame, out_ptr: int, row_stride: int, out_is_device: bool, region=None):
+        """region: None for the whole frame, or (x, y, w, h) in output coordinates: only what that rectangle depends on
+        is decoded, and only it is stored, into a buffer of h rows of w pixels (jxg_modular_batch_add_region)."""
+        dev = 1 if out_is_device else 0
+        if region is None:
+            abi.check(self._lib, self._lib.jxg_modular_batch_add(self._h, frame._h, C.c_void_p(out_ptr), row_stride, dev))
+        else:
+            abi.check(self._lib, self._lib.jxg_modular_batch_add_region(self._h, frame._h, C.byref(_region(region)),
+                                                                        C.c_void_p(out_ptr), row_stride, dev))
         self.frames.append(frame)
 
     def wait(self):
