@@ -417,6 +417,38 @@ void jxg_modular_batch_end(void* batch);
 int jxg_modular_walk_table(const int32_t* nodes, uint32_t n_nodes, const uint8_t* context_map, uint32_t n_contexts,
                            uint32_t channel, uint32_t stream_id, uint32_t* lut, uint32_t* property);
 
+/* ---- Thumbnail decode (1:8) of VarDCT frames --------------------------------------------------------------------
+ * The LF image of a VarDCT frame (one sample per 8x8 block) is a 1:8 picture of it, coded in LfGlobal and the LfGroup
+ * sections ahead of HfGlobal and the HF groups. A thumbnail has ceil(width / 8) x ceil(height / 8) pixels (JxgImageInfo
+ * width and height, display orientation). Its pixel (bx, by) of the coded LF image is the reference's lf_image after
+ * finalize_lf (decode_vardct_lf, frame/modular/mod.rs:931-982; dequant_lf, mod.rs:837, with extra_precision and the LF
+ * chroma-from-luma; adaptive_lf_smoothing, frame/adaptive_lf_smoothing.rs:44, when the frame applies it): the planes
+ * JxgFrameDesc.lf carries. These go through the output stage of the full decode (XYB -> linear with the re-targeted
+ * opsin matrix, transfer function, sample format, orientation), with the u8 dither taken at the coded LF coordinate
+ * (bx, by). Gaborish and EPF are full-resolution filters and are not applied: a thumbnail is not a box-downscale of the
+ * full decode. The reference has no thumbnail API.
+ *
+ * jxg_lf_parse_file parses the headers, TOC and LfGlobal and, per LF group, the header of its LF-coefficient stream; it
+ * decodes no LF pixel, no HF metadata, no HfGlobal and no HF section, and reads no byte past the end of the last LF-group
+ * section, so a bare codestream cut anywhere after it parses (one cut inside an LF-group section:
+ * JXG_ERR_OUT_OF_BOUNDS). A container must be whole. A frame with one section (one group, one pass, at most 256x256)
+ * keeps LfGlobal, the LF group, HfGlobal and the HF group in one bit stream, and its HF byte count (JxgImageInfo.hf_bytes)
+ * is known only where HfGlobal ends: such a frame is parsed in full, as jxg_parse_file parses it, so its section must be
+ * whole and a one-section file whose HF metadata or HfGlobal is corrupt is refused. `info` is what jxg_parse_file returns for the same file, and the file checks are those of jxg_parse_file, with
+ * the same codes. */
+int jxg_lf_parse_file(const uint8_t* data, size_t size, void** parsed, JxgImageInfo* info);
+void jxg_lf_parsed_free(void* parsed);
+/* Adds a thumbnail of `parsed` (jxg_lf_parse_file; it must stay alive until jxg_modular_batch_end) as a frame of a
+ * Modular batch: its LF streams are decoded on the device with the batch's group streams (lanes, pools, status words
+ * and jxg_modular_batch_wait, which reports a failing LF stream by its LF-group index), then dequantised, smoothed and
+ * stored. All six output formats; XYB_F32_PLANAR holds the three LF planes after smoothing in the coded orientation,
+ * plane c from row c * height (the JxgFrameDesc.lf planes, bit for bit). Stride and alignment rules are those of
+ * jxg_batch_add_frame applied to the thumbnail's width (JXG_ERR_INVALID_OUTPUT). An LF stream with a local palette or
+ * Squeeze returns JXG_ERR_UNSUPPORTED (local RCT is decoded); an unknown format JXG_ERR_ARGUMENT. A refused thumbnail
+ * leaves the batch as it was. jxg_modular_batch_read_planes refuses a thumbnail frame (JXG_ERR_ARGUMENT). */
+int jxg_modular_batch_add_lf(void* batch, void* parsed, uint32_t output_format, void* out, size_t out_row_stride,
+                             int out_is_device);
+
 const char* jxg_last_error(void);
 
 #ifdef __cplusplus

@@ -82,6 +82,7 @@ EXPORTS = [
     "jxg_modular_batch_lz77_stats", "jxg_modular_batch_walk_stats", "jxg_batch_add_frame_region", "jxg_batch_add_parsed_region",
     "jxg_parsed_region_desc", "jxg_context_set_sm_budget", "jxg_batch_entropy_schedule", "jxg_batch_stream_status",
     "jxg_batch_read_transform_plan", "jxg_modular_batch_add_region", "jxg_modular_parsed_region_plan",
+    "jxg_lf_parse_file", "jxg_lf_parsed_free", "jxg_modular_batch_add_lf",
 ]
 
 ALL_FRAMES = 0xFFFFFFFF  # JXG_ALL_FRAMES
@@ -165,6 +166,10 @@ def load_library():
                                            C.POINTER(vp), u32p, u32p, u32p]
     lib.jxg_modular_batch_add_region.argtypes = [vp, vp, rp, vp, C.c_size_t, C.c_int]
     lib.jxg_modular_parsed_region_plan.argtypes = [vp, rp, u32p, C.c_uint32, u32p, u32p, C.c_uint32, u32p]
+    lib.jxg_lf_parse_file.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(vp), C.POINTER(JxgImageInfo)]
+    lib.jxg_lf_parsed_free.argtypes = [vp]
+    lib.jxg_lf_parsed_free.restype = None
+    lib.jxg_modular_batch_add_lf.argtypes = [vp, vp, C.c_uint32, vp, C.c_size_t, C.c_int]
     _LIB = lib
     return lib
 

@@ -371,10 +371,7 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   F.cxb = (F.xb + 7) / 8;
   const size_t nb = size_t(F.xb) * F.yb, ncm = size_t(F.cxb) * ((F.yb + 7) / 8);
   if (d->output_format > JXG_FORMAT_RGB_F16) return set_error(JXG_ERR_ARGUMENT, "unknown output format");
-  size_t bpp = d->output_format == JXG_FORMAT_RGB_U8 ? 3
-               : d->output_format == JXG_FORMAT_RGBA_U8 ? 4
-               : d->output_format == JXG_FORMAT_RGB_F32 ? 12
-               : (d->output_format == JXG_FORMAT_RGB_U16 || d->output_format == JXG_FORMAT_RGB_F16) ? 6 : 4;
+  const size_t bpp = format_bpp(d->output_format);
   if (d->orientation > 8) return set_error(JXG_ERR_ARGUMENT, "orientation must be 1..8");
   const uint32_t orientation = (d->orientation == 0 || d->output_format == JXG_FORMAT_XYB_F32_PLANAR) ? 1u : d->orientation;
   if (region && d->output_format == JXG_FORMAT_XYB_F32_PLANAR) return set_error(JXG_ERR_ARGUMENT, "XYB_F32_PLANAR has no region form");
@@ -384,14 +381,8 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   F.win_w = region ? region->coded_win[2] : F.width;
   F.win_h = region ? region->coded_win[3] : F.height;
   const uint32_t disp_w = orientation >= 5 ? F.win_h : F.win_w, disp_h = orientation >= 5 ? F.win_w : F.win_h;
-  if (out_row_stride < size_t(disp_w) * bpp) return set_error(JXG_ERR_INVALID_OUTPUT, "output row stride too small");
-  // The stores (and the orientation pass's word copies) write whole samples: rows, and a device buffer, must be
-  // aligned to the sample size (include/jxg.h).
-  const size_t sample_align = bpp == 3 ? 1 : (bpp == 6 ? 2 : 4);
-  if (out_row_stride % sample_align)
-    return set_error(JXG_ERR_INVALID_OUTPUT, "output row stride is not a multiple of the sample size");
-  if (out_is_device && reinterpret_cast<uintptr_t>(out) % sample_align)
-    return set_error(JXG_ERR_INVALID_OUTPUT, "device output is not aligned to the sample size");
+  // The stores and the orientation pass's word copies write whole samples.
+  if (int r = check_output(bpp, disp_w, out_row_stride, out, out_is_device != 0)) return r;
   if (!trusted)
     if (int r = validate_desc(d, sec_len, n_sections)) return r;
   F.num_histograms = d->num_histograms;
@@ -532,22 +523,7 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   F.epf_pass2_sigma_scale = d->epf_pass2_sigma_scale;
   F.epf_border_sad_mul = d->epf_border_sad_mul;
   F.quant_scale = 1.0f / F.inv_global_scale;
-  memcpy(F.opsin, d->opsin_inverse_matrix, sizeof(F.opsin));
-  F.intensity_scale = 255.0f / d->intensity_target;
-  for (int i = 0; i < 3; i++) {  // xyb.rs:147-160
-    F.bias_cbrt[i] = std::cbrt(d->opsin_biases[i]);
-    F.scaled_bias[i] = d->opsin_biases[i] * F.intensity_scale;
-  }
-  F.output_tf = d->output_tf;
-  F.output_format = d->output_format;
-  F.tf_gamma = d->output_gamma;
-  memcpy(F.tf_lum, d->output_luminances, sizeof(F.tf_lum));
-  {  // color/tf.rs:458-470 hlg_display_to_scene: exponent of the inverse OOTF; |exp| < 0.1 skips it (tf.rs:381-383)
-    const float system_gamma = 1.2f * std::pow(1.111f, std::log2(d->intensity_target / 1e3f));
-    const float e = (1.0f - system_gamma) / system_gamma;
-    F.tf_hlg_exp = std::fabs(e) < 0.1f ? 0.0f : e;
-  }
-  F.tf_pq_mul = d->intensity_target * (1.0f / 10000.0f);
+  set_output_colour(F, d);
   b->filter_cfg_mask |= 1u << ((d->gab ? 4 : 0) + std::min<uint32_t>(d->epf_iters, 3));
   // filter tiles that meet the window
   F.win_tx0 = F.win_x / kFusedTileW;
@@ -992,16 +968,9 @@ int jxg_parse_file_mt(const uint8_t* data, size_t size, int threads, void** pars
   try {
     std::unique_ptr<jxg::FrameState> fs = jxg::parse_vardct_file(data, size, threads);
     if (info) {
-      info->coded_width = fs->header.xsize();
-      info->coded_height = fs->header.ysize();
-      info->orientation = fs->file.orientation;
-      info->width = fs->file.orientation >= 5 ? info->coded_height : info->coded_width;
-      info->height = fs->file.orientation >= 5 ? info->coded_width : info->coded_height;
-      info->num_groups = fs->header.num_groups();
-      info->num_passes = fs->header.passes.num_passes;
-      info->encoding = 0;
-      info->hf_bytes = 0;
-      for (uint32_t l : fs->hf_len) info->hf_bytes += l;
+      uint64_t hf = 0;
+      for (uint32_t l : fs->hf_len) hf += l;
+      jxg::fill_image_info(fs->file, fs->header, hf, info);
     }
     *parsed = fs.release();
     return JXG_OK;

@@ -5,6 +5,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <cstring>
 #include <string>
 #include <thread>
@@ -225,6 +226,53 @@ int batch_first_failure(const BatchCore& b, const std::vector<Stream>& streams, 
       return set_error(b.status_host[i], what + std::to_string(streams[i].frame) + " group " + std::to_string(streams[i].group));
     }
   return 0;
+}
+
+// Bytes per output pixel of a sample format (XYB_F32_PLANAR: one f32 per plane row entry); 0 for an unknown format.
+inline size_t format_bpp(uint32_t format) {
+  switch (format) {
+    case JXG_FORMAT_RGB_U8: return 3;
+    case JXG_FORMAT_RGBA_U8: return 4;
+    case JXG_FORMAT_RGB_F32: return 12;
+    case JXG_FORMAT_XYB_F32_PLANAR: return 4;
+    case JXG_FORMAT_RGB_U16:
+    case JXG_FORMAT_RGB_F16: return 6;
+    default: return 0;
+  }
+}
+
+// The output rules of jxg_batch_add_frame for rows of `width` pixels: the stride holds a row, and the stores write whole
+// samples, so rows and a device buffer are aligned to the sample size (include/jxg.h). JXG_ERR_INVALID_OUTPUT otherwise.
+inline int check_output(size_t bpp, uint32_t width, size_t out_row_stride, const void* out, bool out_is_device) {
+  if (out_row_stride < size_t(width) * bpp) return set_error(JXG_ERR_INVALID_OUTPUT, "output row stride too small");
+  const size_t sample_align = bpp == 3 ? 1 : (bpp == 6 ? 2 : 4);
+  if (out_row_stride % sample_align)
+    return set_error(JXG_ERR_INVALID_OUTPUT, "output row stride is not a multiple of the sample size");
+  if (out_is_device && reinterpret_cast<uintptr_t>(out) % sample_align)
+    return set_error(JXG_ERR_INVALID_OUTPUT, "device output is not aligned to the sample size");
+  return 0;
+}
+
+// The colour fields of the output stage (cuda/output_stage.h) from a frame descriptor: opsin matrix and biases
+// (xyb.rs:147-160), transfer function and its constants, sample format. T: FrameDev or another block with those fields.
+template <typename T>
+void set_output_colour(T& F, const JxgFrameDesc* d) {
+  memcpy(F.opsin, d->opsin_inverse_matrix, sizeof(F.opsin));
+  F.intensity_scale = 255.0f / d->intensity_target;
+  for (int i = 0; i < 3; i++) {  // xyb.rs:147-160
+    F.bias_cbrt[i] = std::cbrt(d->opsin_biases[i]);
+    F.scaled_bias[i] = d->opsin_biases[i] * F.intensity_scale;
+  }
+  F.output_tf = d->output_tf;
+  F.output_format = d->output_format;
+  F.tf_gamma = d->output_gamma;
+  memcpy(F.tf_lum, d->output_luminances, sizeof(F.tf_lum));
+  {  // color/tf.rs:458-470 hlg_display_to_scene: exponent of the inverse OOTF; |exp| < 0.1 skips it (tf.rs:381-383)
+    const float system_gamma = 1.2f * std::pow(1.111f, std::log2(d->intensity_target / 1e3f));
+    const float e = (1.0f - system_gamma) / system_gamma;
+    F.tf_hlg_exp = std::fabs(e) < 0.1f ? 0.0f : e;
+  }
+  F.tf_pq_mul = d->intensity_target * (1.0f / 10000.0f);
 }
 
 // Appends a batch table to the pinned blob, so that it travels with the one H2D copy; `off`: its offset in the blob.

@@ -5,6 +5,7 @@
 
 #include <algorithm>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -13,6 +14,7 @@
 #include <vector>
 
 #include "../../../include/jxg.h"
+#include "../host/lf_frame.h"
 #include "../host/modular_frame.h"
 #include "../host/modular_region.h"
 #include "batch_common.h"
@@ -24,11 +26,14 @@ using namespace jxgpu::detail;
 namespace {
 
 struct MFrame {
-  jxg::ModularFrameState* ms;
+  jxg::ModularFrameState* ms = nullptr;
+  jxg::LfFrameState* lf = nullptr;  // a thumbnail of a VarDCT frame (jxg_modular_batch_add_lf); ms is null then
   void* out;
   size_t out_stride;
   bool out_is_device;
   bool region = false;             // a region of the frame (jxg_modular_batch_add_region)
+  size_t out_row_bytes = 0, out_rows = 0;  // the output's rows as the store writes them
+  size_t store_index = 0;          // its job in store_jobs, or in lf_store_jobs for a thumbnail
   jxg::ModularRegionPlan plan;     // the cone: per buffer the rectangle the arena holds, the streams decoded
   uint64_t arena_base = 0;         // element offset of this frame's planes
   std::vector<uint64_t> buf_off;   // per plan buffer, element offset in the arena of its arena rectangle's top-left
@@ -55,6 +60,7 @@ struct ModularBatch : BatchCore {
   std::vector<std::vector<MJobDev>> levels;  // jobs grouped by plan step index
   std::vector<jxg::ModularJobKind> level_kind;
   std::vector<MJobDev> store_jobs;
+  std::vector<MJobDev> lf_dequant_jobs, lf_smooth_jobs, lf_store_jobs;  // thumbnails: one job per LF stream / frame
   uint64_t arena_elems = 0, wp_bytes = 0, out_bytes = 0;
   uint64_t lz_window_elems = 0;             // symbol windows of the LZ77 streams, one per stream
   uint32_t lz77_streams = 0, rle_streams = 0;  // streams with LZ77; of those, streams whose copies all have distance 1
@@ -209,7 +215,8 @@ bool build_walk_table(const jxg::ModularTree& t, uint32_t root, uint32_t ci, uin
 
 // Everything add_frame appends to, so that a refused frame leaves the batch as it was (jxg_modular_batch_add).
 struct BatchMark {
-  size_t frames, streams, rct_streams, rects, codes, rcts, refs, levels, store_jobs, blob, blob_pending;
+  size_t frames, streams, rct_streams, rects, codes, rcts, refs, levels, store_jobs, lf_dequant_jobs, lf_smooth_jobs,
+      lf_store_jobs, blob, blob_pending;
   std::vector<size_t> level_jobs;
   uint64_t arena_elems, wp_bytes, out_bytes, lz_window_elems;
   uint32_t lz77_streams, rle_streams;
@@ -218,7 +225,8 @@ struct BatchMark {
   explicit BatchMark(const ModularBatch* b)
       : frames(b->frames.size()), streams(b->streams.size()), rct_streams(b->rct_streams.size()), rects(b->rects.size()),
         codes(b->codes.size()), rcts(b->rcts.size()), refs(b->refs.size()), levels(b->levels.size()),
-        store_jobs(b->store_jobs.size()), blob(b->ctx->blob.size), blob_pending(b->ctx->blob.pending.size()),
+        store_jobs(b->store_jobs.size()), lf_dequant_jobs(b->lf_dequant_jobs.size()),
+        lf_smooth_jobs(b->lf_smooth_jobs.size()), lf_store_jobs(b->lf_store_jobs.size()), blob(b->ctx->blob.size), blob_pending(b->ctx->blob.pending.size()),
         arena_elems(b->arena_elems), wp_bytes(b->wp_bytes), out_bytes(b->out_bytes), lz_window_elems(b->lz_window_elems),
         lz77_streams(b->lz77_streams), rle_streams(b->rle_streams), walks(b->walks) {
     for (const auto& l : b->levels) level_jobs.push_back(l.size());
@@ -235,6 +243,9 @@ struct BatchMark {
     b->level_kind.resize(levels);
     for (size_t l = 0; l < levels; l++) b->levels[l].resize(level_jobs[l]);
     b->store_jobs.resize(store_jobs);
+    b->lf_dequant_jobs.resize(lf_dequant_jobs);
+    b->lf_smooth_jobs.resize(lf_smooth_jobs);
+    b->lf_store_jobs.resize(lf_store_jobs);
     b->ctx->blob.size = blob;
     b->ctx->blob.pending.resize(blob_pending);
     b->arena_elems = arena_elems;
@@ -295,10 +306,10 @@ void check_tree(const jxg::ModularTree& t) {
   for (const jxg::TreeNode& n : t.nodes)
     if (n.property < 0 && n.ctx >= (1u << 27)) throw jxg::Error(JXG_ERR_UNSUPPORTED, "MA tree too large for the device encoding");
 }
-void check_streams(const jxg::ModularFrameState* ms) {
-  for (const jxg::ModularGroupStream& st : ms->hf) {
+void check_streams(const std::vector<jxg::ModularGroupStream>& hf, const jxg::ModularTree& global_tree) {
+  for (const jxg::ModularGroupStream& st : hf) {
     if (st.empty) continue;
-    check_tree(st.local_tree ? *st.local_tree : ms->global_tree);
+    check_tree(st.local_tree ? *st.local_tree : global_tree);
     for (const jxg::ModularTransform& t : st.header.transforms) {
       if (t.id != 0) throw jxg::Error(JXG_ERR_UNSUPPORTED, "only RCT is implemented as a group-local transform on the device path");
       if (t.begin_channel + 3 > st.rects.size()) throw jxg::Error(jxg::kErrBitstream, "RCT channel range");
@@ -308,19 +319,29 @@ void check_streams(const jxg::ModularFrameState* ms) {
   }
 }
 
-// Codes / trees, and per group stream the cone selects its MStreamDev, rects, reference channels, local RCTs and LZ77
-// window. The rects address the channels' arena rectangles; the stream keeps its whole-frame group index.
-void add_streams(ModularBatch* b, MFrame& f) {
-  const jxg::ModularFrameState* ms = f.ms;
+// The group streams of one frame of the batch: its section bytes, its channels (their shifts decide which rects are
+// reference channels), the global tree, the streams decoded (null: all) and where a rect lives in the plane arena.
+struct StreamSource {
+  const uint8_t* codestream;
+  const std::vector<jxg::ModularGroupStream>& hf;
+  const std::vector<jxg::ModularChannel>& coded;
+  const jxg::ModularTree& global_tree;
+  const std::vector<uint8_t>* selected;
+  std::function<void(const jxg::ModularRect&, uint32_t& stride, uint64_t& base)> addr;
+};
+
+// Codes / trees, and per selected group stream its MStreamDev, rects, reference channels, local RCTs and LZ77 window.
+// The stream keeps its index in src.hf (the whole-frame group index).
+void add_streams(ModularBatch* b, const StreamSource& src) {
   uint32_t global_code = 0;
   uint64_t global_tree = 0;
   bool have_global = false;
   std::map<WalkKey, WalkInfo> walk_cache;
   std::map<uint64_t, bool> inner_static;
-  for (size_t g = 0; g < ms->hf.size(); g++) {
-    const jxg::ModularGroupStream& st = ms->hf[g];
-    if (!f.plan.selected[g]) continue;
-    const jxg::ModularTree* tree = st.local_tree ? st.local_tree.get() : &ms->global_tree;
+  for (size_t g = 0; g < src.hf.size(); g++) {
+    const jxg::ModularGroupStream& st = src.hf[g];
+    if (src.selected && !(*src.selected)[g]) continue;
+    const jxg::ModularTree* tree = st.local_tree ? st.local_tree.get() : &src.global_tree;
     MStreamDev d;
     memset(&d, 0, sizeof(d));
     if (st.local_tree) {
@@ -337,7 +358,7 @@ void add_streams(ModularBatch* b, MFrame& f) {
     }
     d.frame = uint32_t(b->frames.size());
     d.group = st.group;
-    d.sec_off = blob_append(b, ms->codestream.data() + st.sec_off, st.sec_len, 8, 24);
+    d.sec_off = blob_append(b, src.codestream + st.sec_off, st.sec_len, 8, 24);
     d.sec_len = st.sec_len;
     d.data_bitpos = uint32_t(st.data_bitpos);
     d.stream_id = uint32_t(st.stream_id);
@@ -351,8 +372,7 @@ void add_streams(ModularBatch* b, MFrame& f) {
     for (size_t ri = 0; ri < st.rects.size(); ri++) {
       const jxg::ModularRect& r = st.rects[ri];
       MRectDev rd;
-      rd.stride = buf_stride(f, r.chan);
-      rd.base = buf_index(f, r.chan, r.x0, r.y0);
+      src.addr(r, rd.stride, rd.base);
       rd.w = r.w;
       rd.h = r.h;
       rd.walk = kWalkGeneric;
@@ -389,8 +409,8 @@ void add_streams(ModularBatch* b, MFrame& f) {
       if (tree->num_properties > 16)
         for (size_t k = ri; k-- > 0;) {
           const jxg::ModularRect& q = st.rects[k];
-          if (q.w == r.w && q.h == r.h && ms->coded[q.chan].hshift == ms->coded[r.chan].hshift &&
-              ms->coded[q.chan].vshift == ms->coded[r.chan].vshift)
+          if (q.w == r.w && q.h == r.h && src.coded[q.chan].hshift == src.coded[r.chan].hshift &&
+              src.coded[q.chan].vshift == src.coded[r.chan].vshift)
             b->refs.push_back(d.first_rect + uint32_t(k));
         }
       rd.ref_count = uint32_t(b->refs.size()) - rd.ref_first;
@@ -490,10 +510,13 @@ void add_store(ModularBatch* b, MFrame& f) {
   sj.op = ms->file.orientation;
   sj.out_x = f.plan.out_x;
   sj.out_y = f.plan.out_y;
+  f.out_row_bytes = size_t(f.plan.out_w) * 3;
+  f.out_rows = f.plan.out_h;
   if (!f.out_is_device) {
     f.dev_out_off = b->out_bytes;
-    b->out_bytes += (size_t(f.plan.out_w) * f.plan.out_h * 3 + 255) & ~size_t(255);
+    b->out_bytes += (f.out_row_bytes * f.out_rows + 255) & ~size_t(255);
   }
+  f.store_index = b->store_jobs.size();
   b->store_jobs.push_back(sj);
 }
 
@@ -505,7 +528,7 @@ void check_frame(const jxg::ModularFrameState* ms) {
     throw jxg::Error(JXG_ERR_UNSUPPORTED, "single-section Modular frames with a coded group are not on the device path");
 }
 void check_plan(const jxg::ModularFrameState* ms) {
-  check_streams(ms);
+  check_streams(ms->hf, ms->global_tree);
   for (const jxg::ModularStep& s : ms->steps)
     if (s.kind == jxg::kJobPalette && (ms->bufs[s.b].h < s.n || ms->bufs[s.b].w < s.num_colors))
       throw jxg::Error(jxg::kErrBitstream, "palette channel smaller than its header says");
@@ -533,9 +556,83 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, const JxgRegion* reg
   f.out_stride = stride;
   f.out_is_device = is_device;
   add_arena(b, f);
-  add_streams(b, f);
+  add_streams(b, StreamSource{ms->codestream.data(), ms->hf, ms->coded, ms->global_tree, &f.plan.selected,
+                              [&f](const jxg::ModularRect& r, uint32_t& stride, uint64_t& base) {
+                                stride = buf_stride(f, r.chan);
+                                base = buf_index(f, r.chan, r.x0, r.y0);
+                              }});
   add_plan(b, f);
   add_store(b, f);
+  b->frames.push_back(std::move(f));
+}
+
+// A thumbnail: the frame's LF streams decode into three i32 planes of xb x yb (Y, X, B); each stream's dequantisation
+// job writes its rectangle of the f32 planes X, Y, B; the smoothing (when the frame applies it) writes them to a second
+// f32 plane set; the store reads the last set.
+void add_lf(ModularBatch* b, jxg::LfFrameState* lp, uint32_t format, void* out, size_t stride, bool is_device) {
+  jxg::FrameState& fs = lp->fs;
+  const size_t bpp = format_bpp(format);
+  if (!bpp) throw jxg::Error(JXG_ERR_ARGUMENT, "unknown output format");
+  const uint32_t w = fs.xb, h = fs.yb;
+  const bool planar = format == JXG_FORMAT_XYB_F32_PLANAR;
+  const uint32_t orientation = planar || fs.file.orientation == 0 ? 1u : fs.file.orientation;
+  const uint32_t disp_w = orientation >= 5 ? h : w, disp_h = orientation >= 5 ? w : h;
+  if (int r = check_output(bpp, disp_w, stride, out, is_device)) throw jxg::Error(r, g_error);
+  check_streams(lp->streams, fs.global_tree);
+  MFrame f;
+  f.lf = lp;
+  f.out = out;
+  f.out_stride = stride;
+  f.out_is_device = is_device;
+  f.out_row_bytes = size_t(disp_w) * bpp;
+  f.out_rows = planar ? size_t(3) * h : disp_h;
+  const uint64_t plane = uint64_t(w) * h;
+  const bool smooth = fs.header.adaptive_lf_smoothing();
+  f.arena_base = b->arena_elems;
+  const uint64_t q = f.arena_base, dq = q + 3 * plane, sm = dq + 3 * plane;
+  b->arena_elems = (f.arena_base + (smooth ? 9 : 6) * plane + 63) & ~uint64_t(63);
+  add_streams(b, StreamSource{fs.codestream.data(), lp->streams, lp->coded, fs.global_tree, nullptr,
+                              [&](const jxg::ModularRect& r, uint32_t& s, uint64_t& base) {
+                                s = w;
+                                base = q + r.chan * plane + uint64_t(r.y0) * w + r.x0;
+                              }});
+  MJobDev j;
+  memset(&j, 0, sizeof(j));
+  j.sa = w;
+  j.w = w;
+  j.h = h;
+  j.a = int64_t(q);
+  j.c = int64_t(dq);
+  for (size_t k = 0; k < lp->streams.size(); k++) {
+    const jxg::LfDequantFactors lf = jxg::lf_dequant_factors(fs, lp->mul[k]);
+    const MLfDequantDev p{{lf.fac[0], lf.fac[1], lf.fac[2]}, lf.cfl_x, lf.cfl_b};
+    j.params = blob_append(b, &p, sizeof(p));
+    const jxg::ModularRect& r = lp->streams[k].rects[0];
+    set_rect(j, jxg::PlaneRect{r.x0, r.y0, r.x0 + r.w, r.y0 + r.h});
+    b->lf_dequant_jobs.push_back(j);
+  }
+  MLfFrameDev p;
+  memset(&p, 0, sizeof(p));
+  jxg::lf_smoothing_factors(fs, p.lf_factors);
+  JxgFrameDesc d;
+  fs.fill_desc(&d, format);
+  set_output_colour(p, &d);
+  j.params = blob_append(b, &p, sizeof(p));
+  set_rect(j, jxg::PlaneRect{0, 0, w, h});
+  if (smooth) {
+    j.a = int64_t(dq);
+    j.c = int64_t(sm);
+    b->lf_smooth_jobs.push_back(j);
+  }
+  j.a = int64_t(smooth ? sm : dq);
+  j.c = 0;
+  j.op = orientation;
+  if (!is_device) {
+    f.dev_out_off = b->out_bytes;
+    b->out_bytes += (f.out_row_bytes * f.out_rows + 255) & ~size_t(255);
+  }
+  f.store_index = b->lf_store_jobs.size();
+  b->lf_store_jobs.push_back(j);
   b->frames.push_back(std::move(f));
 }
 
@@ -572,19 +669,23 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
       mw = std::max(mw, j.x1 - j.x0);
       mh = std::max(mh, j.y1 - j.y0);
     }
-    launch_modular_jobs(kind, jobs, uint32_t(level.size()), mw, mh, B.planes, schedule_sms(cx), s);
+    launch_modular_jobs(kind, jobs, uint32_t(level.size()), mw, mh, B.planes, B.blob, schedule_sms(cx), s);
     jobs += level.size();
     b->launches++;
   };
   for (size_t l = 0; l < b->levels.size(); l++) launch_jobs(b->level_kind[l], b->levels[l]);
-  launch_jobs(jxg::kJobStore, b->store_jobs);
+  // the jobs of the Modular frames' stores, then the thumbnails' jobs in stage order (each kind waits for the one before)
+  const std::pair<jxg::ModularJobKind, const std::vector<MJobDev>*> tail[4] = {
+      {jxg::kJobStore, &b->store_jobs}, {jxg::kJobLfDequant, &b->lf_dequant_jobs},
+      {jxg::kJobLfSmooth, &b->lf_smooth_jobs}, {jxg::kJobLfStore, &b->lf_store_jobs}};
+  for (const auto& [kind, list] : tail)
+    if (!list->empty()) launch_jobs(kind, *list);
   if (copy_to_host) {
     for (const MFrame& f : b->frames)
       if (!f.out_is_device) {
-        const uint32_t W = f.plan.out_w, H = f.plan.out_h;  // display size of the frame or region
-        CUDA_TRY(cudaMemcpy2DAsync(f.out, f.out_stride, static_cast<uint8_t*>(cx->d_out.p) + f.dev_out_off, size_t(W) * 3,
-                                   size_t(W) * 3, H, cudaMemcpyDeviceToHost, s));
-        b->d2h += size_t(W) * 3 * H;
+        CUDA_TRY(cudaMemcpy2DAsync(f.out, f.out_stride, static_cast<uint8_t*>(cx->d_out.p) + f.dev_out_off, f.out_row_bytes,
+                                   f.out_row_bytes, f.out_rows, cudaMemcpyDeviceToHost, s));
+        b->d2h += f.out_row_bytes * f.out_rows;
       }
   }
   CUDA_TRY(cudaMemcpyAsync(b->status_host, cx->d_status.p, b->status_n * 4, cudaMemcpyDeviceToHost, s));
@@ -600,19 +701,10 @@ int jxg_modular_parse_file(const uint8_t* data, size_t size, void** parsed, JxgI
   if (!data || !parsed) return JXG_ERR_ARGUMENT;
   try {
     auto ms = jxg::parse_modular_file(data, size);
-    if (info) {
-      memset(info, 0, sizeof(*info));
-      info->coded_width = ms->header.xsize();
-      info->coded_height = ms->header.ysize();
-      info->orientation = ms->file.orientation;
-      info->width = ms->file.orientation >= 5 ? info->coded_height : info->coded_width;
-      info->height = ms->file.orientation >= 5 ? info->coded_width : info->coded_height;
-      info->num_groups = ms->header.num_groups();
-      info->num_passes = 1;
-      info->encoding = 1;
+    if (info) {  // the Modular path takes one-pass frames only (parse_modular_file)
       uint64_t hf = 0;
       for (const auto& st : ms->hf) hf += st.sec_len;
-      info->hf_bytes = hf;
+      jxg::fill_image_info(ms->file, ms->header, hf, info);
     }
     *parsed = ms.release();
     return JXG_OK;
@@ -659,6 +751,37 @@ int jxg_modular_batch_add_region(void* bp, void* parsed, const JxgRegion* region
     return set_error(e.code, e.what());
   }
 }
+
+int jxg_modular_batch_add_lf(void* bp, void* parsed, uint32_t output_format, void* out, size_t out_row_stride,
+                             int out_is_device) {
+  ModularBatch* b = static_cast<ModularBatch*>(bp);
+  if (!b || !parsed || !out) return JXG_ERR_ARGUMENT;
+  if (b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch already submitted");
+  const BatchMark mark(b);
+  try {
+    add_lf(b, static_cast<jxg::LfFrameState*>(parsed), output_format, out, out_row_stride, out_is_device != 0);
+    return JXG_OK;
+  } catch (jxg::Error& e) {
+    mark.restore(b);
+    return set_error(e.code, e.what());
+  }
+}
+
+int jxg_lf_parse_file(const uint8_t* data, size_t size, void** parsed, JxgImageInfo* info) {
+  if (!data || !parsed) return JXG_ERR_ARGUMENT;
+  try {
+    std::unique_ptr<jxg::LfFrameState> lp = jxg::parse_vardct_lf_file(data, size);
+    if (info) jxg::fill_image_info(lp->fs.file, lp->fs.header, lp->hf_bytes, info);
+    *parsed = lp.release();
+    return JXG_OK;
+  } catch (jxg::Error& e) {
+    return set_error(e.code, e.what());
+  } catch (std::exception& e) {
+    return set_error(JXG_ERR_BITSTREAM, e.what());
+  }
+}
+
+void jxg_lf_parsed_free(void* parsed) { delete static_cast<jxg::LfFrameState*>(parsed); }
 
 int jxg_modular_parsed_region_plan(void* parsed, const JxgRegion* region, uint32_t* groups, uint32_t max_groups,
                                    uint32_t* n_groups, uint32_t* rects, uint32_t max_buffers, uint32_t* n_buffers) {
@@ -720,15 +843,16 @@ int jxg_modular_batch_run(void* bp, void* cuda_stream) {
     return set_error(JXG_ERR_UNSUPPORTED, "no device memory for the LZ77 windows of the batch (" +
                                               std::to_string(b->lz_window_elems * 4) + " bytes)");
   }
-  for (size_t i = 0; i < b->frames.size(); i++) {
-    MFrame& f = b->frames[i];
-    b->store_jobs[i].out = f.out_is_device ? f.out : static_cast<uint8_t*>(cx->d_out.p) + f.dev_out_off;
-    b->store_jobs[i].out_stride = f.out_is_device ? f.out_stride : size_t(f.plan.out_w) * 3;
+  for (MFrame& f : b->frames) {
+    MJobDev& j = f.lf ? b->lf_store_jobs[f.store_index] : b->store_jobs[f.store_index];
+    j.out = f.out_is_device ? f.out : static_cast<uint8_t*>(cx->d_out.p) + f.dev_out_off;
+    j.out_stride = f.out_is_device ? f.out_stride : f.out_row_bytes;
   }
   if (int r = batch_status(*b, b->streams.size())) return r;
-  std::vector<MJobDev> all_jobs;
+  std::vector<MJobDev> all_jobs;  // the launch order of launch_all
   for (auto& l : b->levels) all_jobs.insert(all_jobs.end(), l.begin(), l.end());
-  all_jobs.insert(all_jobs.end(), b->store_jobs.begin(), b->store_jobs.end());
+  for (const auto* l : {&b->store_jobs, &b->lf_dequant_jobs, &b->lf_smooth_jobs, &b->lf_store_jobs})
+    all_jobs.insert(all_jobs.end(), l->begin(), l->end());
   PinnedArena& blob = cx->blob;
   if (!batch_table(blob, b->streams, b->tab.streams) || !batch_table(blob, b->order, b->tab.order) ||
       !batch_table(blob, b->rct_streams, b->tab.rct_streams) || !batch_table(blob, b->rects, b->tab.rects) ||
@@ -772,8 +896,9 @@ int jxg_modular_batch_read_planes(void* bp, uint32_t f, int32_t* out, size_t out
   ModularBatch* b = static_cast<ModularBatch*>(bp);
   if (!b || !b->uploaded || f >= b->frames.size() || !out) return JXG_ERR_ARGUMENT;
   if (b->frames[f].region) return set_error(JXG_ERR_ARGUMENT, "read_planes: a region frame holds no whole planes");
+  if (b->frames[f].lf) return set_error(JXG_ERR_ARGUMENT, "read_planes: a thumbnail holds no Modular colour planes");
   if (int r = batch_wait_last_run(*b)) return r;
-  const MJobDev& j = b->store_jobs[f];  // a whole frame: the planes are whole, rows of width w
+  const MJobDev& j = b->store_jobs[b->frames[f].store_index];  // a whole frame: the planes are whole, rows of width w
   const size_t n = size_t(j.w) * j.h;
   if (out_len < 3 * n) return set_error(JXG_ERR_ARGUMENT, "plane buffer too small");
   const int32_t* planes = static_cast<const int32_t*>(b->ctx->d_planes_a.p);

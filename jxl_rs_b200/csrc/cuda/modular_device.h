@@ -61,6 +61,19 @@ struct MJobDev {
   void* out;
   uint64_t out_stride;
   uint32_t out_x, out_y;  // store: display coordinates of the output's top-left pixel
+  uint64_t params;        // thumbnail jobs: blob offset of their MLfDequantDev / MLfFrameDev
+};
+
+// Thumbnail jobs (kJobLf*): the LF image is three planes of w x h samples with row stride sa; a plane set at element
+// index a holds X, Y, B (f32) or, as the dequantisation's input, Y, X, B (i32) at a, a + sa * h, a + 2 * sa * h.
+struct MLfDequantDev {  // one LF stream: dequant_lf_rect's factors for its extra_precision (frame.h lf_dequant_factors)
+  float fac[3], cfl_x, cfl_b;
+};
+struct MLfFrameDev {  // one thumbnail: the smoothing's divisors and the output stage (output_stage.h, set_output_colour)
+  float lf_factors[3];
+  float opsin[9], bias_cbrt[3], scaled_bias[3], intensity_scale;
+  uint32_t output_tf, output_format;
+  float tf_gamma, tf_lum[3], tf_hlg_exp, tf_pq_mul;
 };
 
 struct MBatchDev {
@@ -87,8 +100,9 @@ struct MBatchDev {
 int launch_modular_decode(const MBatchDev& B, uint32_t num_plain, uint32_t lanes_per_warp, uint32_t num_rct_streams,
                           uint32_t sms, cudaStream_t stream);
 // kind: a jxg::ModularJobKind (host/modular_frame.h): 0 RCT, 1 horizontal unsqueeze, 2 vertical unsqueeze, 3 store,
-// 4 palette look-up. max_w / max_h: the largest x1 - x0 / y1 - y0 of the jobs.
+// 4 palette look-up, 5-7 the thumbnail jobs. max_w / max_h: the largest x1 - x0 / y1 - y0 of the jobs. blob: the device
+// copy of the staging blob (the thumbnail jobs' parameters).
 void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint32_t max_w, uint32_t max_h, int32_t* planes,
-                         uint32_t sms, cudaStream_t stream);
+                         const uint8_t* blob, uint32_t sms, cudaStream_t stream);
 
 }  // namespace jxgpu

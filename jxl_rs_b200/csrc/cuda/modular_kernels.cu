@@ -16,6 +16,7 @@
 #include "../../../include/jxg.h"
 #include "launch.h"
 #include "modular_device.h"
+#include "output_stage.h"
 
 namespace jxgpu {
 
@@ -751,6 +752,24 @@ __global__ void __launch_bounds__(128) k_unsqueeze_v(const MJobDev* jobs, int32_
   if (j.y1 & 1) o[(j.y1 - 1) * sc] = a[(ah - 1) * sa];
 }
 
+// ImageMetadata.orientation (headers/image_metadata.rs:85-96 display_pixel): coded pixel (x, y) of a w x h image -> its
+// display position; 1 = identity.
+__device__ __forceinline__ void display_pixel(uint32_t orientation, uint32_t w, uint32_t h, uint32_t x, uint32_t y,
+                                              uint32_t& dx, uint32_t& dy) {
+  dx = x;
+  dy = y;
+  switch (orientation) {
+    case 2: dx = w - 1 - x; break;
+    case 3: dx = w - 1 - x; dy = h - 1 - y; break;
+    case 4: dy = h - 1 - y; break;
+    case 5: dx = y; dy = x; break;
+    case 6: dx = h - 1 - y; dy = x; break;
+    case 7: dx = h - 1 - y; dy = w - 1 - x; break;
+    case 8: dx = y; dy = w - 1 - x; break;
+    default: break;
+  }
+}
+
 // i32 planes -> interleaved RGB u8, clamped (convert.rs:675-680). job: a, b, c = R, G, B planes (w x h, the coded
 // frame), op = orientation; the coded window [x0, x1) x [y0, y1) goes to the output whose top-left pixel is display
 // pixel (out_x, out_y). Rows grid-strided over the CTAs, columns over the threads.
@@ -758,17 +777,8 @@ __global__ void __launch_bounds__(256) k_modular_store(const MJobDev* jobs, cons
   const MJobDev j = jobs[blockIdx.y];
   for (uint32_t y = j.y0 + blockIdx.x; y < j.y1; y += gridDim.x) {
     for (uint32_t x = j.x0 + threadIdx.x; x < j.x1; x += blockDim.x) {
-      uint32_t dx = x, dy = y;
-      switch (j.op) {  // ImageMetadata.orientation (headers/image_metadata.rs:85-96 display_pixel); 1 = identity
-        case 2: dx = j.w - 1 - x; break;
-        case 3: dx = j.w - 1 - x; dy = j.h - 1 - y; break;
-        case 4: dy = j.h - 1 - y; break;
-        case 5: dx = y; dy = x; break;
-        case 6: dx = j.h - 1 - y; dy = x; break;
-        case 7: dx = j.h - 1 - y; dy = j.w - 1 - x; break;
-        case 8: dx = y; dy = j.w - 1 - x; break;
-        default: break;
-      }
+      uint32_t dx, dy;
+      display_pixel(j.op, j.w, j.h, x, y, dx, dy);
       uint8_t* d = static_cast<uint8_t*>(j.out) + size_t(dy - j.out_y) * j.out_stride + size_t(dx - j.out_x) * 3;
       d[0] = uint8_t(min(max(planes[j.a + int64_t(y) * j.sa + x], 0), 255));
       d[1] = uint8_t(min(max(planes[j.b + int64_t(y) * j.sb + x], 0), 255));
@@ -871,8 +881,112 @@ __global__ void __launch_bounds__(256) k_modular_palette(const MJobDev* jobs, in
   }
 }
 
+// ---------------------------------------------------------------------------
+// Thumbnail jobs: the LF image of a VarDCT frame (modular/mod.rs:837-982, adaptive_lf_smoothing.rs:44-125) and its
+// store. The host computes the same values with scalar float code compiled without contraction: every operation here
+// is the correctly rounded one of the host, in the host's order.
+// ---------------------------------------------------------------------------
+
+// dequant_lf_rect (frame.cc) on one LF group's rectangle: quantised Y, X, B at a -> X, Y, B at c.
+__global__ void __launch_bounds__(256) k_lf_dequant(const MJobDev* jobs, int32_t* planes, const uint8_t* blob) {
+  const MJobDev j = jobs[blockIdx.y];
+  const MLfDequantDev p = *reinterpret_cast<const MLfDequantDev*>(blob + j.params);
+  const size_t plane = size_t(j.sa) * j.h;
+  const int32_t* qy = planes + j.a;
+  const int32_t* qx = qy + plane;
+  const int32_t* qb = qx + plane;
+  float* out = reinterpret_cast<float*>(planes + j.c);
+  for (uint32_t y = j.y0 + blockIdx.x; y < j.y1; y += gridDim.x) {
+    for (uint32_t x = j.x0 + threadIdx.x; x < j.x1; x += blockDim.x) {
+      const size_t i = size_t(y) * j.sa + x;
+      const float in_x = __fmul_rn(float(qx[i]), p.fac[0]), in_y = __fmul_rn(float(qy[i]), p.fac[1]),
+                  in_b = __fmul_rn(float(qb[i]), p.fac[2]);
+      out[i] = __fadd_rn(__fmul_rn(in_y, p.cfl_x), in_x);
+      out[plane + i] = in_y;
+      out[2 * plane + i] = __fadd_rn(__fmul_rn(in_y, p.cfl_b), in_b);
+    }
+  }
+}
+
+// adaptive_lf_smoothing (frame.cc smooth_band's scalar loop) of the whole LF image, X, Y, B at a -> c; border samples
+// and images of at most two rows or columns are copied.
+__global__ void __launch_bounds__(256) k_lf_smooth(const MJobDev* jobs, int32_t* planes, const uint8_t* blob) {
+  const MJobDev j = jobs[blockIdx.y];
+  const MLfFrameDev& p = *reinterpret_cast<const MLfFrameDev*>(blob + j.params);
+  const size_t plane = size_t(j.sa) * j.h;
+  const float* in = reinterpret_cast<const float*>(planes + j.a);
+  float* out = reinterpret_cast<float*>(planes + j.c);
+  const float kSide = 0.20345139757231578f, kCorner = 0.0334829185968739f;
+  const float kCenter = __fsub_rn(1.0f, __fmul_rn(4.0f, __fadd_rn(kSide, kCorner)));
+  const bool smooth = j.w > 2 && j.h > 2;
+  for (uint32_t y = blockIdx.x; y < j.h; y += gridDim.x) {
+    for (uint32_t x = threadIdx.x; x < j.w; x += blockDim.x) {
+      const size_t i = size_t(y) * j.sa + x;
+      if (!smooth || x == 0 || y == 0 || x + 1 == j.w || y + 1 == j.h) {
+        for (int c = 0; c < 3; c++) out[c * plane + i] = in[c * plane + i];
+        continue;
+      }
+      float gap = 0.5f, mc[3], sm[3];
+      for (int c = 0; c < 3; c++) {
+        const float* m = in + c * plane + i;
+        const float* t = m - j.sa;
+        const float* b = m + j.sa;
+        const float corner = __fadd_rn(__fadd_rn(__fadd_rn(t[-1], t[1]), b[-1]), b[1]);
+        const float side = __fadd_rn(__fadd_rn(__fadd_rn(m[-1], m[1]), t[0]), b[0]);
+        mc[c] = m[0];
+        sm[c] = __fadd_rn(__fadd_rn(__fmul_rn(corner, kCorner), __fmul_rn(side, kSide)), __fmul_rn(mc[c], kCenter));
+        const float d = fabsf(__fdiv_rn(__fsub_rn(mc[c], sm[c]), p.lf_factors[c]));
+        gap = gap < d ? d : gap;  // std::max(gap, d)
+      }
+      const float f = __fsub_rn(3.0f, __fmul_rn(4.0f, gap));
+      const float factor = f < 0.0f ? 0.0f : f;  // std::max(f, 0.0f)
+      for (int c = 0; c < 3; c++) out[c * plane + i] = __fadd_rn(__fmul_rn(__fsub_rn(sm[c], mc[c]), factor), mc[c]);
+    }
+  }
+}
+
+// LF image X, Y, B at a -> the thumbnail: the output stage of the full decode's store (output_stage.h), the u8 dither at
+// the coded LF coordinate, then the orientation (op); XYB_F32_PLANAR writes the planes in the coded orientation,
+// plane c from row c * h. Rows grid-strided over the CTAs, columns over the threads.
+__global__ void __launch_bounds__(256) k_lf_store(const MJobDev* jobs, int32_t* planes, const uint8_t* blob) {
+  const MJobDev j = jobs[blockIdx.y];
+  const MLfFrameDev& p = *reinterpret_cast<const MLfFrameDev*>(blob + j.params);
+  const size_t plane = size_t(j.sa) * j.h;
+  const float* in = reinterpret_cast<const float*>(planes + j.a);
+  uint8_t* const out = static_cast<uint8_t*>(j.out);
+  for (uint32_t y = blockIdx.x; y < j.h; y += gridDim.x) {
+    for (uint32_t x = threadIdx.x; x < j.w; x += blockDim.x) {
+      const size_t i = size_t(y) * j.sa + x;
+      if (p.output_format == JXG_FORMAT_XYB_F32_PLANAR) {
+        for (int c = 0; c < 3; c++) reinterpret_cast<float*>(out + (size_t(c) * j.h + y) * j.out_stride)[x] = in[c * plane + i];
+        continue;
+      }
+      float v[3];
+      xyb_to_output(p, in[i], in[plane + i], in[2 * plane + i], v);
+      uint32_t dx, dy;
+      display_pixel(j.op, j.w, j.h, x, y, dx, dy);
+      uint8_t* const row = out + size_t(dy) * j.out_stride;
+      switch (p.output_format) {
+        case JXG_FORMAT_RGB_F32:
+          for (int c = 0; c < 3; c++) reinterpret_cast<float*>(row)[size_t(dx) * 3 + c] = v[c];
+          break;
+        case JXG_FORMAT_RGB_U16:
+        case JXG_FORMAT_RGB_F16:
+          for (int c = 0; c < 3; c++) reinterpret_cast<uint16_t*>(row)[size_t(dx) * 3 + c] = sample16(p, v[c]);
+          break;
+        default: {  // RGB_U8, RGBA_U8
+          const uint32_t bpp = p.output_format == JXG_FORMAT_RGBA_U8 ? 4 : 3;
+          uint8_t* d = row + size_t(dx) * bpp;
+          for (int c = 0; c < 3; c++) d[c] = sample8(v[c], int(x), int(y), c);
+          if (bpp == 4) d[3] = 255;
+        }
+      }
+    }
+  }
+}
+
 void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint32_t max_w, uint32_t max_h, int32_t* planes,
-                         uint32_t sms, cudaStream_t stream) {
+                         const uint8_t* blob, uint32_t sms, cudaStream_t stream) {
   if (!num_jobs) return;
   const uint32_t rows = max(min(max_h, sms * 16), 1u);  // grid of the row-strided kernels
   if (kind == 0) {
@@ -883,6 +997,12 @@ void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint3
     k_unsqueeze_v<<<dim3(max((max_w + 127) / 128, 1u), num_jobs), 128, 0, stream>>>(jobs, planes);
   } else if (kind == 4) {
     k_modular_palette<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes);
+  } else if (kind == 5) {
+    k_lf_dequant<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes, blob);
+  } else if (kind == 6) {
+    k_lf_smooth<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes, blob);
+  } else if (kind == 7) {
+    k_lf_store<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes, blob);
   } else {
     k_modular_store<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes);
   }

@@ -105,6 +105,8 @@ void skip_extra_channels_lf_group(FrameState& fs, uint32_t g, BitReader& br) {
   decode_modular_subbitstream(ch, 1 + size_t(h.num_lf_groups()) + g, fs.has_global_tree ? &fs.global_tree : nullptr, br);
 }
 
+}  // namespace
+
 // frame/decode.rs:307-427
 void decode_lf_global(FrameState& fs, BitReader& br) {
   const FrameHeader& h = fs.header;
@@ -198,18 +200,22 @@ void decode_lf_global(FrameState& fs, BitReader& br) {
   br.check();
 }
 
+LfDequantFactors lf_dequant_factors(const FrameState& fs, float mul) {
+  const float inv_quant_lf = 65536.0f / (float(fs.global_scale) * float(fs.quant_lf));
+  LfDequantFactors f;
+  for (int c = 0; c < 3; c++) f.fac[c] = fs.lf_quant[c] * inv_quant_lf * mul;
+  f.cfl_x = fs.base_correlation_x + float(fs.ytox_lf) / float(fs.color_factor);
+  f.cfl_b = fs.base_correlation_b + float(fs.ytob_lf) / float(fs.color_factor);
+  return f;
+}
+
 // modular/mod.rs:837-929 dequant_lf for a 4:4:4 frame: quantised LF integers of a w x h rect (row stride qstride) ->
 // dequantised X / Y / B LF samples with the LF chroma-from-luma, and the LF context bucket of every block, written at
 // element offset `o0` (row stride fs.xb) of fs.lf[] / fs.quant_lf_map.
-}  // namespace
 void dequant_lf_rect(FrameState& fs, const int32_t* qy_p, const int32_t* qx_p, const int32_t* qb_p, size_t qstride, uint32_t w,
                      uint32_t hh, float mul, size_t o0) {
-  float inv_quant_lf = 65536.0f / (float(fs.global_scale) * float(fs.quant_lf));
-  float fac_x = fs.lf_quant[0] * inv_quant_lf * mul;
-  float fac_y = fs.lf_quant[1] * inv_quant_lf * mul;
-  float fac_b = fs.lf_quant[2] * inv_quant_lf * mul;
-  float cfl_x = fs.base_correlation_x + float(fs.ytox_lf) / float(fs.color_factor);
-  float cfl_b = fs.base_correlation_b + float(fs.ytob_lf) / float(fs.color_factor);
+  const LfDequantFactors f = lf_dequant_factors(fs, mul);
+  const float fac_x = f.fac[0], fac_y = f.fac[1], fac_b = f.fac[2], cfl_x = f.cfl_x, cfl_b = f.cfl_b;
   for (uint32_t y = 0; y < hh; y++) {
     const int32_t *qy = qy_p + size_t(y) * qstride, *qx = qx_p + size_t(y) * qstride, *qb = qb_p + size_t(y) * qstride;
     size_t o = o0 + size_t(y) * fs.xb;
@@ -452,14 +458,18 @@ void decode_hf_global(FrameState& fs, BitReader& br) {
 // order as compute_pixel_channel (:20-41): results are bit-identical to the scalar definition.
 #pragma GCC push_options
 #pragma GCC optimize("fp-contract=off")
+void lf_smoothing_factors(const FrameState& fs, float out[3]) {
+  const float inv_quant_lf = (65536.0f / float(fs.global_scale)) / float(fs.quant_lf);
+  for (int c = 0; c < 3; c++) out[c] = inv_quant_lf * fs.lf_quant[c];
+}
+
 // Rows [y_begin, y_end) of the smoothing, in place. `top0[c]` is the original row y_begin - 1 and `bot_last[c]` the
 // original row y_end (both saved by the caller before any band runs, because neighbouring bands overwrite them).
 static void smooth_band(FrameState& fs, size_t y_begin, size_t y_end, const float* const top0[3],
                         const float* const bot_last[3]) {
   const size_t xs = fs.xb;
-  const float inv_quant_lf = (65536.0f / float(fs.global_scale)) / float(fs.quant_lf);
-  const float lf_factors[3] = {inv_quant_lf * fs.lf_quant[0], inv_quant_lf * fs.lf_quant[1],
-                               inv_quant_lf * fs.lf_quant[2]};
+  float lf_factors[3];
+  lf_smoothing_factors(fs, lf_factors);
   const float kSide = 0.20345139757231578f, kCorner = 0.0334829185968739f;
   const float kCenter = 1.0f - 4.0f * (kSide + kCorner);
   // In place: row y of the output only needs the original rows y-1, y, y+1, so two saved original rows per channel
@@ -607,10 +617,20 @@ void recycle_frame_state(FrameState* fs) {
   }  // else: b is freed on return
 }
 
-std::unique_ptr<FrameState> parse_vardct_file(const uint8_t* data, size_t size, int threads) {
-  auto fsp = std::make_unique<FrameState>();
-  FrameState& fs = *fsp;
-  take_buffers(fs);
+void fill_image_info(const FileHeader& file, const FrameHeader& h, uint64_t hf_bytes, JxgImageInfo* info) {
+  memset(info, 0, sizeof(*info));
+  info->coded_width = h.xsize();
+  info->coded_height = h.ysize();
+  info->orientation = file.orientation;
+  info->width = file.orientation >= 5 ? info->coded_height : info->coded_width;
+  info->height = file.orientation >= 5 ? info->coded_width : info->coded_height;
+  info->num_groups = h.num_groups();
+  info->num_passes = h.passes.num_passes;
+  info->encoding = h.encoding;
+  info->hf_bytes = hf_bytes;
+}
+
+void read_vardct_headers(FrameState& fs, const uint8_t* data, size_t size, bool lf_sections_only) {
   extract_codestream(data, size, fs.codestream);
   BitReader br(fs.codestream.data(), fs.codestream.size());
   fs.file = read_file_header(br);
@@ -627,13 +647,21 @@ std::unique_ptr<FrameState> parse_vardct_file(const uint8_t* data, size_t size, 
   resolve_output_colour(fs.file);  // refuses the colour encodings this path cannot reproduce
   fs.toc = read_toc(br, h.num_toc_entries());
   fs.sections_base = br.byte_pos();
-  const uint8_t* base = fs.codestream.data() + fs.sections_base;
-  size_t avail = fs.codestream.size() - fs.sections_base;
-  for (size_t i = 0; i < fs.toc.offsets.size(); i++)
+  const size_t avail = fs.codestream.size() - fs.sections_base;
+  const size_t n = fs.toc.offsets.size(), whole = lf_sections_only && n > 1 ? 1 + size_t(h.num_lf_groups()) : n;
+  for (size_t i = 0; i < whole; i++)
     if (fs.toc.offsets[i] + fs.toc.lengths[i] > avail) fail("truncated file: section beyond end", kErrOutOfBounds);
-
   fs.xb = h.xsize_blocks();
   fs.yb = h.ysize_blocks();
+}
+
+std::unique_ptr<FrameState> parse_vardct_file(const uint8_t* data, size_t size, int threads) {
+  auto fsp = std::make_unique<FrameState>();
+  FrameState& fs = *fsp;
+  take_buffers(fs);
+  read_vardct_headers(fs, data, size, false);
+  const FrameHeader& h = fs.header;
+  const uint8_t* base = fs.codestream.data() + fs.sections_base;
   size_t nb = size_t(fs.xb) * fs.yb;
   // LF samples, raw quant and EPF sharpness of every block are written by its LF group (a stream that leaves a block
   // uncovered is rejected below), so pooled buffers are only resized; the transform map is the coverage marker.

@@ -105,8 +105,30 @@ void place_varblocks(uint32_t w, uint32_t hh, size_t stride, uint32_t count, con
 void dequant_lf_rect(FrameState& fs, const int32_t* qy, const int32_t* qx, const int32_t* qb, size_t qstride, uint32_t w, uint32_t h,
                      float mul, size_t o0);
 
+// The scalars of dequant_lf_rect for LF multiplier `mul` (1 / 2^extra_precision): per X / Y / B the factor of the
+// quantised sample, and the LF chroma-from-luma of X and B.
+struct LfDequantFactors {
+  float fac[3], cfl_x, cfl_b;
+};
+LfDequantFactors lf_dequant_factors(const FrameState& fs, float mul);
+// The per-channel divisors of the adaptive LF smoothing's gap (adaptive_lf_smoothing.rs:57-60).
+void lf_smoothing_factors(const FrameState& fs, float out[3]);
+
 // frame/adaptive_lf_smoothing.rs:44 on fs.lf (uses xb, yb, global_scale, quant_lf, lf_quant). Exposed for the tests.
 void adaptive_lf_smoothing(FrameState& fs, int threads = 1);
+
+// JxgImageInfo of a parsed frame (jxg_parse_file, jxg_lf_parse_file, jxg_modular_parse_file): sizes, orientation,
+// groups, passes, encoding and the HF section bytes `hf_bytes`.
+void fill_image_info(const FileHeader& file, const FrameHeader& h, uint64_t hf_bytes, JxgImageInfo* info);
+
+// Container, headers, scope checks (everything outside this path's scope is refused with kErrUnsupported), the output
+// colour check and the TOC: fills fs.codestream, file, header, toc, sections_base, xb and yb. A section that does not fit
+// in the file is refused with kErrOutOfBounds: every section, or with `lf_sections_only` LfGlobal and the LF groups
+// (the single section of a one-section frame).
+void read_vardct_headers(FrameState& fs, const uint8_t* data, size_t size, bool lf_sections_only);
+// frame/decode.rs:307-427: LfGlobal of a VarDCT frame (quantiser, block context map, colour correlation, global tree,
+// extra-channel data).
+void decode_lf_global(FrameState& fs, BitReader& br);
 
 // Parses a complete file up to (not including) the HF groups of its first
 // displayed VarDCT frame. Throws jxg::Error.

@@ -126,32 +126,8 @@ void decode_lf_group_modular(ModularFrameState& ms, uint32_t g, BitReader& br) {
   br.check();
 }
 
-// Reads what precedes the pixel symbols of one ModularHF section (bitstream.rs:134-190).
 void parse_hf_stream_header(ModularFrameState& ms, ModularGroupStream& st, BitReader& br) {
-  if (st.empty) return;
-  st.header_bitpos = br.total_bits_read();
-  st.header = GroupHeader::read(br);
-  std::vector<ModularChannel> shapes;
-  for (const ModularRect& r : st.rects) {
-    ModularChannel c;
-    c.w = r.w;
-    c.h = r.h;
-    c.hshift = ms.coded[r.chan].hshift;
-    c.vshift = ms.coded[r.chan].vshift;
-    shapes.push_back(c);
-  }
-  uint32_t nb_meta = 0;
-  meta_apply_transforms(shapes, nb_meta, st.header, /*allocate=*/false);
-  if (!st.header.use_global_tree) {
-    size_t samples = 0;
-    for (auto& c : shapes) samples += size_t(c.w) * c.h;
-    st.local_tree = std::make_shared<ModularTree>(ModularTree::read(br, std::min<size_t>(1024 + samples, size_t(1) << 20)));
-  } else if (!ms.has_global_tree) {
-    fail("no global MA tree");
-  }
-  st.data_bitpos = br.total_bits_read();
-  for (const ModularChannel& c : shapes) st.dist_multiplier = std::max(st.dist_multiplier, c.w);
-  br.check();
+  read_group_stream_header(st, ms.coded, ms.has_global_tree, br);
 }
 
 // Symbolic undo_transforms (modular.cc) over buffer ids.
@@ -224,6 +200,34 @@ void build_inverse_plan(ModularFrameState& ms) {
 }
 
 }  // namespace
+
+void read_group_stream_header(ModularGroupStream& st, const std::vector<ModularChannel>& coded, bool has_global_tree,
+                              BitReader& br) {
+  if (st.empty) return;
+  st.header_bitpos = br.total_bits_read();
+  st.header = GroupHeader::read(br);
+  std::vector<ModularChannel> shapes;
+  for (const ModularRect& r : st.rects) {
+    ModularChannel c;
+    c.w = r.w;
+    c.h = r.h;
+    c.hshift = coded[r.chan].hshift;
+    c.vshift = coded[r.chan].vshift;
+    shapes.push_back(c);
+  }
+  uint32_t nb_meta = 0;
+  meta_apply_transforms(shapes, nb_meta, st.header, /*allocate=*/false);
+  if (!st.header.use_global_tree) {
+    size_t samples = 0;
+    for (auto& c : shapes) samples += size_t(c.w) * c.h;
+    st.local_tree = std::make_shared<ModularTree>(ModularTree::read(br, std::min<size_t>(1024 + samples, size_t(1) << 20)));
+  } else if (!has_global_tree) {
+    fail("no global MA tree");
+  }
+  st.data_bitpos = br.total_bits_read();
+  for (const ModularChannel& c : shapes) st.dist_multiplier = std::max(st.dist_multiplier, c.w);
+  br.check();
+}
 
 std::unique_ptr<ModularFrameState> parse_modular_file(const uint8_t* data, size_t size) {
   auto msp = std::make_unique<ModularFrameState>();

@@ -47,6 +47,10 @@ enum ModularJobKind : uint32_t {
   kJobVSqueeze = 2,  // vertical unsqueeze
   kJobStore = 3,     // final colour planes -> u8 output (device job only, no plan step)
   kJobPalette = 4,   // palette without delta entries: a index channel, b palette, c .. c + n - 1 the colour channels
+  // Thumbnail jobs (device only), over a VarDCT LF image of three xb x yb planes at a, a + plane, a + 2 * plane:
+  kJobLfDequant = 5,  // quantised Y, X, B (i32) of one LF group's rectangle -> dequantised X, Y, B (f32)
+  kJobLfSmooth = 6,   // adaptive LF smoothing, X, Y, B at a -> c (out of place)
+  kJobLfStore = 7,    // X, Y, B planes -> the thumbnail output
 };
 struct ModularStep {
   ModularJobKind kind = kJobRct;
@@ -75,6 +79,12 @@ struct ModularFrameState {
   std::vector<ModularStep> steps;
   uint32_t out_buf[3] = {0, 0, 0};  // buffers holding the final colour channels
 };
+
+// Reads what precedes the pixel symbols of one group stream (bitstream.rs:134-190): its GroupHeader and local tree, the
+// bit position of its first entropy-coded bit and its LZ77 distance multiplier. `coded` gives the shifts of the channels
+// the stream's rects index. Nothing is read for an empty stream.
+void read_group_stream_header(ModularGroupStream& st, const std::vector<ModularChannel>& coded, bool has_global_tree,
+                              BitReader& br);
 
 // Parses a complete file holding one Modular frame. Throws jxg::Error (kErrUnsupported for features outside the
 // scope of the device path).

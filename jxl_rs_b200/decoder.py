@@ -560,6 +560,40 @@ class ModularParsedFrame:
             self._h = C.c_void_p()
 
 
+class LfParsedFrame:
+    """A VarDCT .jxl file parsed for its 1:8 thumbnail (jxg_lf_parse_file): headers, TOC, LfGlobal and the headers of
+    the LF-group streams, nothing of HfGlobal or the HF sections. `info` is what ParsedFrame gives for the same file;
+    width / height are the thumbnail's (display orientation)."""
+
+    def __init__(self, data: bytes):
+        self._lib = abi.load_library()
+        self._h = C.c_void_p()
+        self.info = abi.JxgImageInfo()
+        abi.check(self._lib, self._lib.jxg_lf_parse_file(data, len(data), C.byref(self._h), C.byref(self.info)))
+
+    @property
+    def coded_width(self):
+        """Thumbnail width in the coded orientation (the LF image's blocks across)."""
+        return (self.info.coded_width + 7) // 8
+
+    @property
+    def coded_height(self):
+        return (self.info.coded_height + 7) // 8
+
+    @property
+    def width(self):
+        return (self.info.width + 7) // 8
+
+    @property
+    def height(self):
+        return (self.info.height + 7) // 8
+
+    def __del__(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self._lib.jxg_lf_parsed_free(self._h)
+            self._h = C.c_void_p()
+
+
 class ModularBatch(_BatchHandle):
     """jxg_modular_batch_*: Modular frames whose group streams are decoded together on the GPU."""
     _PREFIX = "jxg_modular_batch_"
@@ -580,9 +614,19 @@ class ModularBatch(_BatchHandle):
                                                                         C.c_void_p(out_ptr), row_stride, dev))
         self.frames.append(frame)
 
+    def add_lf(self, frame: LfParsedFrame, out_ptr: int, row_stride: int, fmt: int, out_is_device: bool):
+        """Adds the 1:8 thumbnail of a VarDCT frame (jxg_modular_batch_add_lf) in output format `fmt`."""
+        abi.check(self._lib, self._lib.jxg_modular_batch_add_lf(self._h, frame._h, fmt, C.c_void_p(out_ptr), row_stride,
+                                                                1 if out_is_device else 0))
+        self.frames.append(frame)
+
     def wait(self):
+        """Raises the first failing stream's error; `last_failure` holds its (frame, group), the group being the LF-group
+        index for a thumbnail."""
         bf, bg = C.c_uint32(), C.c_uint32()
-        abi.check(self._lib, self._lib.jxg_modular_batch_wait(self._h, C.byref(bf), C.byref(bg)))
+        r = self._lib.jxg_modular_batch_wait(self._h, C.byref(bf), C.byref(bg))
+        self.last_failure = (bf.value, bg.value) if r != abi.JXG_OK else None
+        abi.check(self._lib, r)
 
     def stats(self):
         h2d, d2h, launches = C.c_uint64(), C.c_uint64(), C.c_uint64()
@@ -632,6 +676,32 @@ def decode_modular_files(ctx: JxgContext, files, to_host: bool = True, lanes_per
                 t = torch.empty((fr.height, fr.width, 3), dtype=torch.uint8, device=f"cuda:{ctx.device}")
             outs.append(t)
             batch.add(fr, t.data_ptr(), fr.width * 3, not to_host)
+        batch.run()
+        batch.wait()
+    finally:
+        batch.close()
+    return outs
+
+
+def decode_thumbnails(ctx: JxgContext, files, pixel_format: JxlPixelFormat = JxlPixelFormat(), to_host: bool = True):
+    """1:8 thumbnails of VarDCT .jxl files (the LF image through the output stage, see jxg_modular_batch_add_lf):
+    H x W x C torch tensors, H = ceil(height / 8), W = ceil(width / 8) of the display-oriented image. Only the headers,
+    LfGlobal and the LF-group sections are parsed; the LF streams are decoded on the GPU."""
+    import torch
+    fmt = pixel_format.abi_format()
+    frames = [LfParsedFrame(f) for f in files]
+    ch = 4 if fmt == abi.FORMAT_RGBA_U8 else 3
+    dt = {abi.FORMAT_RGB_F32: torch.float32, abi.FORMAT_RGB_U16: torch.uint16, abi.FORMAT_RGB_F16: torch.float16}.get(fmt, torch.uint8)
+    batch = ModularBatch(ctx)
+    outs = []
+    try:
+        for fr in frames:
+            if to_host:
+                t = torch.empty((fr.height, fr.width, ch), dtype=dt).pin_memory()
+            else:
+                t = torch.empty((fr.height, fr.width, ch), dtype=dt, device=f"cuda:{ctx.device}")
+            outs.append(t)
+            batch.add_lf(fr, t.data_ptr(), fr.width * ch * t.element_size(), fmt, not to_host)
         batch.run()
         batch.wait()
     finally:

@@ -45,7 +45,8 @@ def _lib():
 
 
 def encode_synthetic(width, height, seed, distance=1.0, epf_iters=2, gab=1, profile=1, lf_tree=0, entropy=0, orientation=1,
-                     colour=0, dequant=None, x_qm_scale=3, b_qm_scale=2, header=None) -> bytes:
+                     colour=0, dequant=None, x_qm_scale=3, b_qm_scale=2, header=None, lf_extra_precision=0,
+                     skip_lf_smoothing=False, lf_entropy=0) -> bytes:
     """One synthetic VarDCT frame. profile 0: DCT8x8 only; 1: mixed transforms up to 32x32;
     2: also 64x64 / 64x32 / 32x64; 3: also the 128 / 256 families (DCT128X128 ... DCT256X256, transform types 21..26);
     4: profile 3 plus IDENTITY, DCT2X2 and AFV0-3 among the 8x8 blocks, so that every dequantisation table is used.
@@ -64,9 +65,14 @@ def encode_synthetic(width, height, seed, distance=1.0, epf_iters=2, gab=1, prof
     is converted with the opsin matrix and biases written, and quantised with the colour correlation (factor, bases,
     LF factors, tile maps clamped to i8) the decoder derives, so the round trip holds as for default headers; a
     non-finite f16 falls back to the default value there (the decoder refuses such a frame). Gaborish and EPF are not
-    inverted by the writer, as with the default weights."""
+    inverted by the writer, as with the default weights.
+    lf_extra_precision: 0..3, written in every LF group with the quantised LF samples unchanged (the decoded LF image is
+    scaled by 2^-lf_extra_precision, a valid frame of a different picture). skip_lf_smoothing: sets the frame flag that
+    turns the adaptive LF smoothing off. lf_entropy: code of the LF image's pixel symbols, as `entropy` (0 ANS, 1 prefix
+    codes, 2 / 3 the same with LZ77 copies at plain distances)."""
     profile = ((profile & 0xff) | ((lf_tree & 1) << 8) | ((entropy & 3) << 9) | (((orientation - 1) & 7) << 12)
-               | ((colour & 15) << 16))
+               | ((colour & 15) << 16) | ((lf_extra_precision & 3) << 20) | ((1 if skip_lf_smoothing else 0) << 22)
+               | ((lf_entropy & 3) << 23))
     lib = _lib()
     words = _dequant_words(dequant)
     arr = (C.c_uint32 * max(1, len(words)))(*[w & 0xFFFFFFFF for w in words])

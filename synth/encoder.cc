@@ -53,6 +53,10 @@ struct Params {
   // 7 DCI transfer function with the E white point
   uint32_t colour = 0;
   uint32_t x_qm_scale = 3, b_qm_scale = 2;  // FrameHeader, 0..7 (group.rs:395-396)
+  // LF image: extra_precision 0..3 of every LF group (mod.rs:938; the quantised LF samples are written as they are, so
+  // the decoded LF is scaled by 2^-extra_precision) and the frame flag that skips the adaptive LF smoothing
+  uint32_t lf_extra_precision = 0, skip_lf_smoothing = 0;
+  uint32_t lf_entropy = 0;  // code of the LF image's pixel symbols: as `entropy` (0 ANS, 1 prefix, 2 / 3 with LZ77)
   // Custom dequantisation matrices, one entry per table index (see jxs_encode_synthetic_ex); all mode 0 = all_default
   struct DequantSpec {
     uint32_t mode = 0;                                   // quant_weights.rs:128 (0 library, 1..7)
@@ -507,7 +511,10 @@ static std::vector<TNode> flatten_tree(const std::vector<TDesc>& d, int root) {
 
 // lf_tree: false = one leaf (`predictor`) per channel; true = libjxl-like: the same channel prefix, then per channel
 // a subtree that splits on the weighted-predictor property (15) and predicts with the weighted predictor (6).
-static void write_modular(BitWriter& bw, const std::vector<Chan>& ch, uint32_t predictor, bool wp_tree = false) {
+// entropy: code of the pixel symbols, 0 ANS, 1 prefix codes, 2 / 3 the same with LZ77 copies (plain distances behind
+// the stream's distance multiplier).
+static void write_modular(BitWriter& bw, const std::vector<Chan>& ch, uint32_t predictor, bool wp_tree = false,
+                          uint32_t entropy = 0) {
   bool empty = true;
   for (auto& c : ch)
     if (c.w && c.h) empty = false;
@@ -593,7 +600,20 @@ static void write_modular(BitWriter& bw, const std::vector<Chan>& ch, uint32_t p
   uint32_t nc;
   HybridCfg cfg;
   std::vector<uint8_t> map = cluster_contexts(num_leaves, {&dt}, 8, nc, cfg);
-  AnsCode code = build_code(num_leaves, map, nc, {&dt});
+  const bool use_prefix = (entropy & 1) != 0;
+  if (entropy >= 2) {
+    Lz77 lz;
+    lz.enabled = true;
+    const HybridCfg len_cfg{0, 0, 0};
+    const std::vector<Sym> syms = lz77_symbols(dt, cfg, lz, len_cfg, uint32_t(num_leaves), 120);
+    map.push_back(uint8_t(nc));  // the distance context gets a cluster of its own
+    AnsCode code = build_code_lz77(num_leaves + 1, map, nc + 1, {&syms}, lz, use_prefix);
+    code.lz_len_cfg = len_cfg;
+    write_code(bw, code);
+    write_symbols(bw, code, syms);
+    return;
+  }
+  AnsCode code = build_code(num_leaves, map, nc, {&dt}, 5, use_prefix);
   write_code(bw, code);
   write_tokens(bw, code, dt);
 }
@@ -947,7 +967,7 @@ std::vector<uint8_t> encode(const Params& p) {
     BitWriter& bw = lf_groups[g];
     uint32_t x0 = (g % f.xlfg) * 256, y0 = (g / f.xlfg) * 256;
     uint32_t w = std::min(256u, f.xb - x0), h = std::min(256u, f.yb - y0);
-    bw.write(0, 2);  // extra_precision
+    bw.write(f.p.lf_extra_precision, 2);  // extra_precision
     std::vector<Chan> ch(3);
     const int order[3] = {1, 0, 2};  // stored Y, X, B
     for (int i = 0; i < 3; i++) {
@@ -957,7 +977,7 @@ std::vector<uint8_t> encode(const Params& p) {
       for (uint32_t y = 0; y < h; y++)
         for (uint32_t x = 0; x < w; x++) ch[i].d[size_t(y) * w + x] = f.lfq[order[i]][size_t(y0 + y) * f.xb + x0 + x];
     }
-    write_modular(bw, ch, 5, f.p.lf_tree != 0);
+    write_modular(bw, ch, 5, f.p.lf_tree != 0, f.p.lf_entropy);
     // HF metadata (modular/mod.rs:984-1080)
     std::vector<int32_t> types, quants;
     for (uint32_t y = 0; y < h; y++)
@@ -1122,14 +1142,15 @@ std::vector<uint8_t> encode(const Params& p) {
   out.zero_pad_to_byte();
   // FrameHeader (frame_header.rs:267-444)
   const bool custom_rf = hd.gab_custom || hd.sharp_custom || hd.weight_custom || hd.sigma_custom;
-  const bool default_header = p.epf_iters == 2 && p.gab == 1 && p.x_qm_scale == 3 && p.b_qm_scale == 2 && !custom_rf;
+  const bool default_header =
+      p.epf_iters == 2 && p.gab == 1 && p.x_qm_scale == 3 && p.b_qm_scale == 2 && !custom_rf && !p.skip_lf_smoothing;
   if (default_header) {
     out.write(1, 1);
   } else {
     out.write(0, 1);       // all_default
     out.write(0, 2);       // RegularFrame
     out.write(0, 1);       // VarDCT
-    out.write_u64(0);      // flags
+    out.write_u64(p.skip_lf_smoothing ? 0x80 : 0);  // flags: SKIP_ADAPTIVE_LF_SMOOTHING
     out.write(0, 2);       // upsampling = 1
     out.write(p.x_qm_scale, 3);
     out.write(p.b_qm_scale, 3);
@@ -1586,10 +1607,14 @@ void jxs_set_threads(int n) { jxs::g_threads.store(n < 1 ? 1 : n); }
 int64_t jxs_encode_synthetic(uint32_t width, uint32_t height, uint64_t seed, float distance, uint32_t epf_iters,
                              uint32_t gab, uint32_t profile, uint8_t* out, size_t cap) {
   try {
-    // profile: bits 0..7 transform mix, bit 8: libjxl-like LF tree (weighted predictor), bits 9..10: AC entropy coder
+    // profile: bits 0..7 transform mix, bit 8: libjxl-like LF tree (weighted predictor), bits 9..10: AC entropy coder,
+    // bits 20..21: LF extra_precision, bit 22: skip the adaptive LF smoothing, bits 23..24: LF entropy coder
     // bits 12..15: orientation - 1, bits 16..19: colour encoding variant
     jxs::Params p{width, height, seed, distance, epf_iters, gab, profile & 0xff, (profile >> 8) & 1, (profile >> 9) & 3,
                   ((profile >> 12) & 7) + 1, (profile >> 16) & 15};
+    p.lf_extra_precision = (profile >> 20) & 3;
+    p.skip_lf_smoothing = (profile >> 22) & 1;
+    p.lf_entropy = (profile >> 23) & 3;
     std::vector<uint8_t> b = jxs::encode(p);
     if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
     return int64_t(b.size());
@@ -1613,6 +1638,9 @@ int64_t jxs_encode_synthetic_ex(uint32_t width, uint32_t height, uint64_t seed, 
   try {
     jxs::Params p{width, height, seed, distance, epf_iters, gab, profile & 0xff, (profile >> 8) & 1, (profile >> 9) & 3,
                   ((profile >> 12) & 7) + 1, (profile >> 16) & 15};
+    p.lf_extra_precision = (profile >> 20) & 3;
+    p.skip_lf_smoothing = (profile >> 22) & 1;
+    p.lf_entropy = (profile >> 23) & 3;
     if (x_qm_scale > 7 || b_qm_scale > 7) throw std::runtime_error("x_qm_scale / b_qm_scale must be 0..7");
     p.x_qm_scale = x_qm_scale;
     p.b_qm_scale = b_qm_scale;

@@ -397,7 +397,7 @@ static std::vector<Sym> plain_symbols(const std::vector<Token>& tokens, const st
 }
 
 std::vector<Sym> lz77_symbols(const std::vector<Token>& tokens, const HybridCfg& cfg, const Lz77& lz, const HybridCfg& len_cfg,
-                              uint32_t dist_ctx) {
+                              uint32_t dist_ctx, uint32_t dist_base) {
   std::vector<Sym> out;
   out.reserve(tokens.size());
   static const uint32_t kDist[6] = {1, 2, 3, 4, 8, 64};
@@ -415,7 +415,7 @@ std::vector<Sym> lz77_symbols(const std::vector<Token>& tokens, const HybridCfg&
       len.tok += lz.min_symbol;
       out.push_back(len);
       Sym dist{dist_ctx, 0, 0, 0};
-      cfg.encode(uint32_t(best_dist - 1), dist.tok, dist.nbits, dist.bits);
+      cfg.encode(uint32_t(dist_base + best_dist - 1), dist.tok, dist.nbits, dist.bits);
       out.push_back(dist);
       i += best_len;
     } else {

@@ -158,9 +158,11 @@ void write_code(BitWriter& bw, const AnsCode& code);
 void write_tokens(BitWriter& bw, const AnsCode& code, const std::vector<Token>& tokens);
 
 // LZ77 variant: tokens -> coded symbols with greedy copies (runs and short-distance repeats), then a code built from
-// the symbols of all streams (num_contexts counts the distance context), and the symbol writer.
+// the symbols of all streams (num_contexts counts the distance context), and the symbol writer. A copy's distance is
+// coded as dist_base + distance - 1: dist_base 0 for a stream without a distance multiplier, 120 for one with a
+// multiplier (Modular streams), whose plain distances start at symbol 120 (decode.rs:87-124).
 std::vector<Sym> lz77_symbols(const std::vector<Token>& tokens, const HybridCfg& cfg, const Lz77& lz, const HybridCfg& len_cfg,
-                              uint32_t dist_ctx);
+                              uint32_t dist_ctx, uint32_t dist_base = 0);
 AnsCode build_code_lz77(size_t num_contexts, const std::vector<uint8_t>& cluster_of_ctx, uint32_t num_clusters,
                         const std::vector<const std::vector<Sym>*>& streams, const Lz77& lz, bool use_prefix);
 void write_symbols(BitWriter& bw, const AnsCode& code, const std::vector<Sym>& syms);
