@@ -449,6 +449,33 @@ void jxg_lf_parsed_free(void* parsed);
 int jxg_modular_batch_add_lf(void* batch, void* parsed, uint32_t output_format, void* out, size_t out_row_stride,
                              int out_is_device);
 
+/* ---- Prefix decode of VarDCT frames (a partly received file) ---------------------------------------------------
+ * The full-resolution picture of a file of which only a prefix has arrived, as the reference renders it when asked to
+ * flush (api/inner/process.rs:169 flush_pixels, frame_info.rs:601 do_flush). A section counts when its whole byte range
+ * (TOC offset + length, after any TOC permutation) lies in the prefix (frame_info.rs:302-328). HF group g is decoded with
+ * passes 0 .. k_g - 1, k_g the longest run of arrived passes from pass 0 (frame_info.rs:548-565): a later pass that has
+ * arrived is not used while an earlier one is missing, and the coefficients of the missing passes are zero. A group with
+ * k_g = 0 is the frame's LF image (JxgFrameDesc.lf, after smoothing) upsampled 8x by the reference's Upsample8x
+ * (frame/decode.rs:51-150 upsample_lf_group; render/stages/upsample.rs): per output pixel a 5x5 convolution whose weights
+ * are the file's CustomTransformData.weights8 (default or custom), clamped to the window's min / max, with LF rows
+ * mirrored at the image edges and LF columns taken from the group's row buffer as the reference fills it: where that
+ * buffer is never written (the right margin of a frame one group wide; the group left of a last group column one LF
+ * sample wide) the window reads 0.0. Both kinds of group then go through the full decode's Gaborish, EPF, colour
+ * conversion, store and orientation.
+ *
+ * jxg_parse_file_prefix takes a bare codestream cut anywhere after HfGlobal; LfGlobal, every LF group and HfGlobal must be
+ * whole (JXG_ERR_OUT_OF_BOUNDS otherwise: a shorter prefix has only the thumbnail, jxg_lf_parse_file). A container must
+ * be whole, and so must the section of a one-section frame (one group, one pass). The handle is an ordinary parsed frame
+ * for jxg_batch_add_parsed, jxg_batch_read_coeffs, jxg_batch_read_xyb and jxg_parsed_free; info.hf_bytes counts the bytes
+ * of the HF sections the decode uses. A complete prefix decodes exactly as jxg_parse_file + jxg_batch_add_parsed, with
+ * the same kernels. jxg_parsed_desc (the descriptor has no per-group pass counts), jxg_batch_add_parsed_region and
+ * jxg_parsed_region_desc refuse a prefix frame with JXG_ERR_ARGUMENT. A decode error in a section it uses is reported
+ * by jxg_batch_wait as for a whole frame. */
+int jxg_parse_file_prefix(const uint8_t* data, size_t size, void** parsed, JxgImageInfo* info);
+/* k_g of each HF group of a frame of jxg_parse_file_prefix, out[0 .. num_groups). JXG_ERR_ARGUMENT for another frame or
+ * when n < the frame's group count. */
+int jxg_parsed_group_passes(void* parsed, uint8_t* out, uint32_t n);
+
 const char* jxg_last_error(void);
 
 #ifdef __cplusplus

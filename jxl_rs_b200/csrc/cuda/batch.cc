@@ -63,7 +63,7 @@ struct Batch : BatchCore {
       : blob(c->blob), d_blob(c->d_blob), d_coeffs(c->d_coeffs), d_planes_a(c->d_planes_a), d_status(c->d_status), d_out(c->d_out) {}
   std::vector<FrameDev> frames;
   std::vector<SectionDev> sections;
-  std::vector<StreamDev> streams, streams_lean, streams_fast, streams_slow;
+  std::vector<StreamDev> streams, streams_lean, streams_fast, streams_slow, streams_lf8;
   bool lean_all_420 = true;
   bool lean_ctx_smem = true;  // every lean frame's context map (+64 spill) fits k_entropy_lean's 16 KB staging area
   uint32_t lean_S = 1, lean_ctas = 0;  // k_entropy_lean schedule (see schedule_lean)
@@ -87,7 +87,7 @@ struct Batch : BatchCore {
   // other batches in flight)
   struct {
     uint64_t frames = 0, sections = 0, streams = 0, lean_cta = 0, lean_warp = 0, streams_lean = 0, streams_fast = 0, streams_slow = 0,
-             ftiles = 0;
+             streams_lf8 = 0, ftiles = 0;
   } tab;
   bool profile = false;
   cudaEvent_t stage_ev[kNumStages + 1] = {nullptr};
@@ -347,9 +347,12 @@ int jxg_batch_set_debug_stop(void* bp, int stage) {
 // `trusted`: the descriptor comes from the in-tree front-end, which guarantees every invariant validate_desc checks by
 // construction (the scan costs ~0.45 ms per 4K frame, 30 ms per 64-frame batch on the dispatcher's critical path).
 // `region`: d is the sub-frame of a region (jxg::slice_region) and only its window is stored; nullptr: the whole frame.
+// `group_passes` (a prefix frame, jxg_parse_file_prefix): the passes each group decodes, and `up8` the expanded Upsample8x
+// kernel for the groups without one; nullptr: every group decodes all passes.
 static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_bytes, const uint64_t* sec_off,
                           const uint32_t* sec_len, uint32_t n_sections, void* out, size_t out_row_stride,
-                          int out_is_device, bool trusted, const jxg::RegionSlice* region = nullptr) {
+                          int out_is_device, bool trusted, const jxg::RegionSlice* region = nullptr,
+                          const uint8_t* group_passes = nullptr, const float* up8 = nullptr) {
   Batch* b = static_cast<Batch*>(bp);
   if (!b || !d || !hf_bytes || !sec_off || !sec_len || !out) return JXG_ERR_ARGUMENT;
   if (d->abi_version != JXG_ABI_VERSION) return set_error(JXG_ERR_ARGUMENT, "ABI version mismatch");
@@ -449,6 +452,11 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   APPEND(F.quant_lf_off, d->quant_lf, nb, 16);
   APPEND(F.ytox_off, d->ytox_map, ncm, 16);
   APPEND(F.ytob_off, d->ytob_map, ncm, 16);
+  if (group_passes) {
+    F.has_prefix = 1;
+    APPEND(F.group_passes_off, group_passes, F.num_groups, 16);
+    APPEND(F.up8_off, up8, 64 * 25 * 4, 16);
+  }
   F.section_base = uint32_t(b->sections.size());
   for (uint32_t s = 0; s < n_sections; s++) {
     SectionDev sd;
@@ -477,6 +485,10 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
   F.first_stream = uint32_t(b->streams.size());
   for (uint32_t g = 0; g < F.num_groups; g++) {
     b->streams.push_back(StreamDev{uint32_t(b->frames.size()), g});
+    if (group_passes && group_passes[g] == 0) {
+      b->streams_lf8.push_back(StreamDev{uint32_t(b->frames.size()), g});
+      continue;
+    }
     ((F.num_passes != 1 || F.has_lz) ? b->streams_slow : ((F.passes[0].code.use_prefix || F.passes[0].shift != 0) ? b->streams_fast : b->streams_lean)).push_back(StreamDev{uint32_t(b->frames.size()), g});
   }
   F.coeff_group_base = b->total_groups;
@@ -659,6 +671,8 @@ static BatchDev make_batch_dev(Batch* b) {
   B.streams_slow = reinterpret_cast<const StreamDev*>(tab(b->tab.streams_slow));
   B.num_fast = uint32_t(b->streams_fast.size());
   B.num_slow = uint32_t(b->streams_slow.size());
+  B.streams_lf8 = reinterpret_cast<const StreamDev*>(tab(b->tab.streams_lf8));
+  B.num_lf8 = uint32_t(b->streams_lf8.size());
   B.nzlist = static_cast<uint32_t*>(b->d_coeffs.p);  // the pool that held the dense coefficients now holds the lists
   B.lzwin = static_cast<uint32_t*>(b->ctx->d_lzwin.p);
   B.planes_a = static_cast<float*>(b->d_planes_a.p);
@@ -776,7 +790,7 @@ int jxg_batch_run(void* bp, void* cuda_stream) {
       !batch_table(b->blob, b->streams, b->tab.streams) || !batch_table(b->blob, b->lean_cta_first, b->tab.lean_cta) ||
       !batch_table(b->blob, b->lean_warps, b->tab.lean_warp) || !batch_table(b->blob, b->streams_lean, b->tab.streams_lean) ||
       !batch_table(b->blob, b->streams_fast, b->tab.streams_fast) || !batch_table(b->blob, b->streams_slow, b->tab.streams_slow) ||
-      !batch_table(b->blob, b->fused_prefix, b->tab.ftiles))
+      !batch_table(b->blob, b->streams_lf8, b->tab.streams_lf8) || !batch_table(b->blob, b->fused_prefix, b->tab.ftiles))
     return set_error(JXG_ERR_CUDA, "pinned staging allocation failed");
   if (int r = b->d_blob.ensure(b->blob.size + 64)) return r;
   trace.mark("alloc");
@@ -981,12 +995,39 @@ int jxg_parse_file_mt(const uint8_t* data, size_t size, int threads, void** pars
   }
 }
 
+int jxg_parse_file_prefix(const uint8_t* data, size_t size, void** parsed, JxgImageInfo* info) {
+  if (!data || !parsed) return JXG_ERR_ARGUMENT;
+  try {
+    std::unique_ptr<jxg::FrameState> fs = jxg::parse_vardct_file(data, size, 1, /*prefix=*/true);
+    if (info) {
+      uint64_t hf = 0;
+      for (uint32_t l : fs->hf_len) hf += l;
+      jxg::fill_image_info(fs->file, fs->header, hf, info);
+    }
+    *parsed = fs.release();
+    return JXG_OK;
+  } catch (jxg::Error& e) {
+    return set_error(e.code, e.what());
+  } catch (std::exception& e) {
+    return set_error(JXG_ERR_BITSTREAM, e.what());
+  }
+}
+
+int jxg_parsed_group_passes(void* parsed, uint8_t* out, uint32_t n) {
+  jxg::FrameState* fs = static_cast<jxg::FrameState*>(parsed);
+  if (!fs || !out || !fs->prefix) return set_error(JXG_ERR_ARGUMENT, "group passes: a frame of jxg_parse_file_prefix");
+  if (n < fs->group_passes.size()) return set_error(JXG_ERR_ARGUMENT, "group passes: n < the frame's group count");
+  memcpy(out, fs->group_passes.data(), fs->group_passes.size());
+  return JXG_OK;
+}
+
 void jxg_parsed_free(void* parsed) { jxg::recycle_frame_state(static_cast<jxg::FrameState*>(parsed)); }
 
 int jxg_parsed_desc(void* parsed, uint32_t output_format, JxgFrameDesc* desc, const uint8_t** hf_bytes,
                     const uint64_t** sec_off, const uint32_t** sec_len, uint32_t* n_sections) {
   jxg::FrameState* fs = static_cast<jxg::FrameState*>(parsed);
   if (!fs || !desc) return JXG_ERR_ARGUMENT;
+  if (fs->prefix) return set_error(JXG_ERR_ARGUMENT, "a prefix frame has no JxgFrameDesc form (no per-group pass counts)");
   fs->fill_desc(desc, output_format);
   if (hf_bytes) *hf_bytes = fs->codestream.data();
   if (sec_off) *sec_off = fs->hf_off.data();
@@ -1001,14 +1042,21 @@ int jxg_batch_add_parsed(void* batch, void* parsed, uint32_t output_format, void
   if (!fs) return JXG_ERR_ARGUMENT;
   JxgFrameDesc d;
   fs->fill_desc(&d, output_format);
+  // A prefix frame whose groups all have every pass is added as a whole frame: the same kernels and launches.
+  const bool short_group = fs->prefix && std::any_of(fs->group_passes.begin(), fs->group_passes.end(),
+                                                     [&](uint8_t k) { return k < d.num_passes; });
+  float up8[64 * 25];
+  if (short_group) jxg::upsample8_kernel(fs->file.weights8, up8);
   return add_frame_impl(batch, &d, fs->codestream.data(), fs->hf_off.data(), fs->hf_len.data(), uint32_t(fs->hf_off.size()), out,
-                        out_row_stride, out_is_device, /*trusted=*/true);
+                        out_row_stride, out_is_device, /*trusted=*/true, nullptr, short_group ? fs->group_passes.data() : nullptr,
+                        short_group ? up8 : nullptr);
 }
 
 int jxg_batch_add_parsed_region(void* batch, void* parsed, uint32_t output_format, const JxgRegion* region, void* out,
                                 size_t out_row_stride, int out_is_device) {
   jxg::FrameState* fs = static_cast<jxg::FrameState*>(parsed);
   if (!fs) return JXG_ERR_ARGUMENT;
+  if (fs->prefix) return set_error(JXG_ERR_ARGUMENT, "a prefix frame has no region form");
   JxgFrameDesc d;
   fs->fill_desc(&d, output_format);
   return add_region_impl(batch, &d, fs->codestream.data(), fs->hf_off.data(), fs->hf_len.data(), uint32_t(fs->hf_off.size()),
@@ -1020,6 +1068,7 @@ int jxg_parsed_region_desc(void* parsed, uint32_t output_format, const JxgRegion
                            uint32_t* n_sections, uint32_t origin[2], uint32_t window[2]) {
   jxg::FrameState* fs = static_cast<jxg::FrameState*>(parsed);
   if (!fs || !desc || !region) return JXG_ERR_ARGUMENT;
+  if (fs->prefix) return set_error(JXG_ERR_ARGUMENT, "a prefix frame has no region form");
   JxgFrameDesc d;
   fs->fill_desc(&d, output_format);
   auto s = std::make_unique<jxg::RegionSlice>();

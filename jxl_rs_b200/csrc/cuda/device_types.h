@@ -94,6 +94,11 @@ struct FrameDev {
   // LZ77 inside the HF streams (entropy_coding/decode.rs:286-330): such frames take the one-lane-per-warp kernel and own
   // one window of decoded symbols per section in BatchDev::lzwin
   uint32_t has_lz, lz_win_base;
+  // A frame decoded from a prefix of its file with a group short of passes (has_prefix = 1): u8[num_groups] passes per
+  // group at group_passes_off (k_entropy and the transforms stop there), and the Upsample8x kernel f32[64 * 25] at up8_off
+  // for the groups with none (k_upsample_lf8). has_prefix = 0: every group decodes num_passes passes.
+  uint32_t has_prefix;
+  uint64_t group_passes_off, up8_off;
   // device-only buffers (element offsets)
   uint64_t coeff_group_base;  // group index base into coeffs
   uint64_t plane_base;        // float index base into plane sets (per channel: + c * plane_size)
@@ -136,7 +141,8 @@ struct BatchDev {
   const StreamDev* streams_lean;  // single-pass ANS frames: k_entropy_lean
   const StreamDev* streams_fast;  // single-pass prefix-coded or shifted frames: k_entropy_fast
   const StreamDev* streams_slow;  // multi-pass and LZ77 frames: k_entropy
-  uint32_t num_frames, num_streams, num_lean, num_fast, num_slow;
+  const StreamDev* streams_lf8;  // groups of prefix frames without a pass: k_upsample_lf8, in no entropy list
+  uint32_t num_frames, num_streams, num_lean, num_fast, num_slow, num_lf8;
   uint32_t* nzlist;     // [sections][kListStride]: list of section (pass * num_groups + group) of a frame, see above
   uint32_t* lzwin;      // [lz sections][kLzWindow] LZ77 windows (decode.rs:86-146), frames with has_lz only
   float* planes_a;

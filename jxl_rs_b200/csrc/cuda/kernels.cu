@@ -206,6 +206,10 @@ __device__ __forceinline__ int32_t unpack_signed(uint32_t u) { return int32_t((u
 
 // One coefficient list (device_types.h): base of the entries, offset words behind them.
 __device__ __forceinline__ uint32_t* list_base(const BatchDev& B, uint32_t section) { return B.nzlist + size_t(section) * kListStride; }
+// The passes group g of frame F decodes: all of them, or for a prefix frame the ones that have arrived (FrameDev).
+__device__ __forceinline__ uint32_t group_passes(const BatchDev& B, const FrameDev& F, uint32_t g) {
+  return F.has_prefix ? uint32_t(B.blob[F.group_passes_off + g]) : F.num_passes;
+}
 // Writer side: the entry of coefficient value v at position pos of a varblock with 2^lnc coefficients per channel is
 // stored at the cursor whatever v is; the cursor only moves for v != 0 (branch-free; a zero is overwritten by the next
 // entry or stays behind the end of the channel). `ovf` collects values that do not fit the entry.
@@ -363,7 +367,7 @@ __global__ void __launch_bounds__(kEntropyWarps * 32) k_entropy(const BatchDev B
     return;
   }
   const uint4* desc = B.desc + size_t(stream) * 1024;
-  const uint32_t np = F.num_passes;
+  const uint32_t np = group_passes(B, F, g);
   int err = 0;
   // one coefficient list per pass (section = pass * num_groups + group); the transform kernels add the passes up
   PassState st[kMaxPasses];
@@ -571,6 +575,14 @@ __global__ void __launch_bounds__(128) k_block_plan(const BatchDev B) {
   const int32_t* rq = reinterpret_cast<const int32_t*>(B.blob + F.raw_quant_off) + goff;
   const uint8_t* qlf = B.blob + F.quant_lf_off + goff;
   const uint8_t* bcm = B.blob + F.block_ctx_map_off;
+  if (group_passes(B, F, g) == 0) {  // a prefix frame's group without a pass: k_upsample_lf8 writes its planes
+    if (lane < kClassWords) B.cls_n[size_t(sidx) * kClassWords + lane] = 0;
+    if (lane == 0) {
+      B.nblk[sidx] = 0;
+      B.status[sidx] = 0;  // no entropy kernel takes the stream
+    }
+    return;
+  }
   uint4* desc = B.desc + size_t(sidx) * 1024;
   uint32_t seq = 0, coeffs_offset = 0;
   bool bad = false;
@@ -1170,7 +1182,8 @@ __device__ __forceinline__ void gather_dequant_tile(const BatchDev& B, const Fra
     return;
   }
   int32_t* it = reinterpret_cast<int32_t*>(tile);
-  for (uint32_t p = 0; p < F.num_passes; p++) {
+  const uint32_t np = group_passes(B, F, g);
+  for (uint32_t p = 0; p < np; p++) {
     const uint32_t* base = list_base(B, F.section_base + p * F.num_groups + g);
     const uint32_t* ow = base + kOffBase + seq * 3;
     if (valid) {
@@ -1627,7 +1640,8 @@ __global__ void __launch_bounds__(kIdctWarps * 32) k_dequant_idct(const BatchDev
       __syncthreads();
     } else {
       int32_t* ip[3] = {reinterpret_cast<int32_t*>(planes[0]), reinterpret_cast<int32_t*>(planes[1]), reinterpret_cast<int32_t*>(planes[2])};
-      for (uint32_t p = 0; p < F.num_passes; p++) {
+      const uint32_t np = group_passes(B, F, g);
+      for (uint32_t p = 0; p < np; p++) {
         const uint32_t* base = list_base(B, F.section_base + p * F.num_groups + g);
         const uint32_t* ow = base + kOffBase + seq * 3;
         const uint32_t o0 = __ldg(ow), o1 = __ldg(ow + 1), o2 = __ldg(ow + 2), o3 = min(__ldg(ow + 3), kListCap);
@@ -2004,6 +2018,90 @@ __global__ void __launch_bounds__(kSmallThreads, KIND == 0 ? 3 : 2) k_idct_small
 __device__ __forceinline__ int mirror(int v, int s) {  // util/mirror.rs:8
   while (v < 0 || v >= s) v = v < 0 ? -v - 1 : 2 * s - v - 1;
   return v;
+}
+
+// ===========================================================================
+// Groups of a prefix frame without an HF pass (frame/decode.rs:51-150 upsample_lf_group): the smoothed LF image
+// upsampled 8x (Upsample8x, render/stages/upsample.rs). One CTA per group and channel. Output pixel (ox, oy) of LF
+// sample (x, y) is the 5x5 window around the sample convolved with kernel (ox, oy), in the reference's accumulation order
+// (kernel_conv!: three accumulators, term t into t % 3, the first three products plain, the rest fused), then clamped to
+// the window's min / max.
+// ===========================================================================
+
+constexpr int kUpWin = 40;  // window row length: 32 samples + 2 on each side (36), padded
+
+__global__ void __launch_bounds__(256) k_upsample_lf8(const BatchDev B) {
+  __shared__ float s_k[64 * 25];       // [oy][tap][ox]: the 8 lanes of one LF sample read 8 consecutive words
+  __shared__ float s_win[36][kUpWin];  // window row j = LF row mirror(ly0 - 2 + j); column i = LF column lx0 - 2 + i
+  __shared__ float s_min[32][33], s_max[32][33];
+  const StreamDev sd = B.streams_lf8[blockIdx.x];
+  const FrameDev& F = B.frames[sd.frame];
+  const uint32_t c = blockIdx.y, g = sd.group, tid = threadIdx.x;
+  const int lw = int(F.xb), lh = int(F.yb);
+  const int lx0 = int(g % F.xg) * 32, ly0 = int(g / F.xg) * 32;
+  const int lx1 = min(lx0 + 32, lw), xs = lx1 - lx0, ys = min(32, lh - ly0);
+  // upsample_lf_group's row buffer (decode.rs:80-111): the columns start_x .. end_x - 1 copied to position save_start
+  const int start_x = max(lx0 - 2, 0), end_x = min(lx1 + 2, lw), cw = end_x - start_x;
+  const int save_start = start_x == lx0 ? 2 : 0, save_end = save_start + cw;
+  const float* lf = reinterpret_cast<const float*>(B.blob + F.lf_off[c]);
+  const float* kern = reinterpret_cast<const float*>(B.blob + F.up8_off);
+  for (uint32_t i = tid; i < 64 * 25; i += blockDim.x) {
+    const uint32_t o = i / 25, t = i % 25;  // o = oy * 8 + ox
+    s_k[((o >> 3) * 25 + t) * 8 + (o & 7)] = kern[i];
+  }
+  for (uint32_t i = tid; i < 36 * kUpWin; i += blockDim.x) {
+    const int j = int(i) / kUpWin, col = int(i) % kUpWin;
+    float v = 0.0f;  // the reference's buffer starts zeroed; slots past a short copy are never written
+    if (j < ys + 4 && col >= save_start && col < save_end) v = lf[size_t(mirror(ly0 - 2 + j, lh)) * lw + start_x + col - save_start];
+    s_win[j][col] = v;
+  }
+  __syncthreads();
+  if (tid < 36) {  // the margin fills, in the reference's order: a fill may read a slot that still holds 0.0
+    float* r = s_win[tid];
+    if (start_x == lx0) {
+      r[0] = r[2 + mirror(-2, cw)];
+      r[1] = r[2 + mirror(-1, cw)];
+    }
+    if (end_x == lx1) {
+      r[save_end] = r[save_start + mirror(save_end, save_end)];
+      r[save_end + 1] = r[save_start + mirror(save_end + 1, save_end)];
+    }
+  }
+  __syncthreads();
+  for (uint32_t i = tid; i < 32 * 32; i += blockDim.x) {  // the clamp range: once per LF sample, shared by its 64 outputs
+    const int y = int(i) >> 5, x = int(i) & 31;
+    if (y >= ys || x >= xs) continue;
+    float mn = s_win[y][x], mx = mn;
+#pragma unroll
+    for (int ky = 0; ky < 5; ky++)
+#pragma unroll
+      for (int kx = 0; kx < 5; kx++) {
+        mn = fminf(mn, s_win[y + ky][x + kx]);
+        mx = fmaxf(mx, s_win[y + ky][x + kx]);
+      }
+    s_min[y][x] = mn;
+    s_max[y][x] = mx;
+  }
+  __syncthreads();
+  const int x = int(tid >> 3), ox = int(tid & 7);
+  if (x >= xs) return;
+  float* plane = B.planes_a + F.plane_base + size_t(c) * F.plane_size;
+  const size_t col = size_t(lx0 + x) * 8 + ox;
+  for (int y = 0; y < ys; y++) {
+    const float mn = s_min[y][x], mx = s_max[y][x];
+    for (int oy = 0; oy < 8; oy++) {
+      const float* k = s_k + oy * 25 * 8 + ox;
+      float a[3];
+#pragma unroll
+      for (int t = 0; t < 25; t++) {
+        const float v = s_win[y + t / 5][x + t % 5], w = k[t * 8];
+        if (t < 3) a[t] = __fmul_rn(v, w);
+        else a[t % 3] = fmaf(v, w, a[t % 3]);
+      }
+      const float v = __fadd_rn(__fadd_rn(a[0], a[1]), a[2]);
+      plane[size_t((ly0 + y) * 8 + oy) * F.plane_stride + col] = fminf(fmaxf(v, mn), mx);
+    }
+  }
 }
 
 // ===========================================================================
@@ -2864,6 +2962,10 @@ int launch_pipeline(const BatchDev& B, cudaStream_t stream, int debug_stop, cuda
   launches += 2;
   k_dequant_idct<<<B.num_streams, kIdctWarps * 32, kLargeSmemBytes, stream>>>(B);
   launches++;
+  if (B.num_lf8) {  // only batches with a prefix frame that has a group without a pass
+    k_upsample_lf8<<<dim3(B.num_lf8, 3), 256, 0, stream>>>(B);
+    launches++;
+  }
   mark(3);
   return launches;  // the fused filter + colour + store kernel is launched per frame range by the caller
 }
@@ -2877,7 +2979,8 @@ __global__ void __launch_bounds__(256) k_expand_coeffs(const BatchDev B, uint32_
   if (nblk == 0xffffffffu) return;
   const uint4* desc = B.desc + size_t(gsid) * 1024;
   int32_t* out = dense + size_t(g) * 3 * kGroupCoeffs;
-  for (uint32_t p = 0; p < F.num_passes; p++) {
+  const uint32_t np = group_passes(B, F, g);
+  for (uint32_t p = 0; p < np; p++) {
     const uint32_t section = F.section_base + p * F.num_groups + g;
     const uint32_t* base = list_base(B, section);
     const uint32_t* ow = base + kOffBase;

@@ -630,7 +630,7 @@ void fill_image_info(const FileHeader& file, const FrameHeader& h, uint64_t hf_b
   info->hf_bytes = hf_bytes;
 }
 
-void read_vardct_headers(FrameState& fs, const uint8_t* data, size_t size, bool lf_sections_only) {
+void read_vardct_headers(FrameState& fs, const uint8_t* data, size_t size, WholeSections whole_sections) {
   extract_codestream(data, size, fs.codestream);
   BitReader br(fs.codestream.data(), fs.codestream.size());
   fs.file = read_file_header(br);
@@ -648,18 +648,26 @@ void read_vardct_headers(FrameState& fs, const uint8_t* data, size_t size, bool 
   fs.toc = read_toc(br, h.num_toc_entries());
   fs.sections_base = br.byte_pos();
   const size_t avail = fs.codestream.size() - fs.sections_base;
-  const size_t n = fs.toc.offsets.size(), whole = lf_sections_only && n > 1 ? 1 + size_t(h.num_lf_groups()) : n;
+  const size_t n = fs.toc.offsets.size();
+  const size_t whole = n == 1 || whole_sections == WholeSections::kAll ? n
+                       : 1 + size_t(h.num_lf_groups()) + (whole_sections == WholeSections::kLfAndHfGlobal ? 1 : 0);
   for (size_t i = 0; i < whole; i++)
-    if (fs.toc.offsets[i] + fs.toc.lengths[i] > avail) fail("truncated file: section beyond end", kErrOutOfBounds);
+    if (fs.toc.offsets[i] + fs.toc.lengths[i] > avail)
+      fail(whole_sections == WholeSections::kLfAndHfGlobal
+               ? "truncated file: a prefix decode needs LfGlobal, every LF group and HfGlobal whole (a shorter prefix has "
+                 "only the thumbnail, jxg_lf_parse_file)"
+               : "truncated file: section beyond end",
+           kErrOutOfBounds);
   fs.xb = h.xsize_blocks();
   fs.yb = h.ysize_blocks();
 }
 
-std::unique_ptr<FrameState> parse_vardct_file(const uint8_t* data, size_t size, int threads) {
+std::unique_ptr<FrameState> parse_vardct_file(const uint8_t* data, size_t size, int threads, bool prefix) {
   auto fsp = std::make_unique<FrameState>();
   FrameState& fs = *fsp;
   take_buffers(fs);
-  read_vardct_headers(fs, data, size, false);
+  read_vardct_headers(fs, data, size, prefix ? WholeSections::kLfAndHfGlobal : WholeSections::kAll);
+  fs.prefix = prefix;
   const FrameHeader& h = fs.header;
   const uint8_t* base = fs.codestream.data() + fs.sections_base;
   size_t nb = size_t(fs.xb) * fs.yb;
@@ -757,17 +765,52 @@ std::unique_ptr<FrameState> parse_vardct_file(const uint8_t* data, size_t size, 
       BitReader sbr(base + fs.toc.offsets[s], fs.toc.lengths[s]);
       decode_hf_global(fs, sbr);
     }
-    for (uint32_t p = 0; p < num_passes; p++)
-      for (uint32_t g = 0; g < num_groups; g++) {
-        size_t s = 2 + h.num_lf_groups() + size_t(num_groups) * p + g;
+    // A prefix uses a section only when all of it has arrived, and a group only with its first passes up to the first
+    // one missing (frame_info.rs:302-328 dequeue_ready_sections, 548-565 check_group).
+    const size_t avail = fs.codestream.size() - fs.sections_base;
+    if (prefix) fs.group_passes.assign(num_groups, 0);
+    for (uint32_t g = 0; g < num_groups; g++) {
+      bool used = true;
+      for (uint32_t p = 0; p < num_passes; p++) {
+        const size_t s = 2 + h.num_lf_groups() + size_t(num_groups) * p + g;
+        used = used && fs.toc.offsets[s] + fs.toc.lengths[s] <= avail;
+        if (!used) break;
         fs.hf_off[size_t(p) * num_groups + g] = fs.sections_base + fs.toc.offsets[s];
         fs.hf_len[size_t(p) * num_groups + g] = fs.toc.lengths[s];
+        if (prefix) fs.group_passes[g] = uint8_t(p + 1);
       }
+    }
   }
+  if (prefix && fs.group_passes.empty()) fs.group_passes.assign(num_groups, uint8_t(num_passes));  // one-section frame
+  // modular/mod.rs:326-331, 477 + frame/decode.rs:266-272: a palette of several channels or with a predictor in the global
+  // Modular header (extra channels) rules out rendering before the last pass
+  if (prefix)
+    for (const ModularTransform& t : fs.ec.header.transforms)
+      if (t.id == 1 && (t.num_channels > 1 || t.predictor_id != 0))
+        for (uint8_t k : fs.group_passes)
+          if (k < num_passes) fail("this frame's extra channels rule out a partial render (a global palette over several channels or with a predictor)", kErrUnsupported);
   for (uint8_t t : fs.transform_map)
     if (t == 27) fail("VarDCT transform map has uncovered blocks");
   if (h.adaptive_lf_smoothing()) adaptive_lf_smoothing(fs, threads);
   return fsp;
+}
+
+void upsample8_kernel(const std::array<float, 210>& weights, float out[64 * 25]) {
+  // kernel[oy][ox][ky][kx], filled from the top-left quarter (N / 2 = 4 outputs, 5 * 4 = 20 taps per axis) by mirroring
+  float k[8][8][5][5];
+  for (int i = 0; i < 20; i++)
+    for (int j = 0; j < 20; j++) {
+      const int y = std::min(i, j), x = std::max(i, j);
+      const float w = weights[size_t(20 * y - y * (y - 1) / 2 + x - y)];
+      k[j / 5][i / 5][j % 5][i % 5] = w;
+      k[7 - j / 5][i / 5][4 - j % 5][i % 5] = w;
+      k[j / 5][7 - i / 5][j % 5][4 - i % 5] = w;
+      k[7 - j / 5][7 - i / 5][4 - j % 5][4 - i % 5] = w;
+    }
+  for (int oy = 0; oy < 8; oy++)
+    for (int ox = 0; ox < 8; ox++)
+      for (int ky = 0; ky < 5; ky++)
+        for (int kx = 0; kx < 5; kx++) out[(oy * 8 + ox) * 25 + ky * 5 + kx] = k[oy][ox][ky][kx];
 }
 
 void FrameState::fill_desc(JxgFrameDesc* d, uint32_t output_format) {

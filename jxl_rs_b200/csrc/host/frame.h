@@ -91,6 +91,12 @@ struct FrameState {
   std::vector<uint64_t> hf_off;
   std::vector<uint32_t> hf_len;
 
+  // A frame parsed from a prefix of its file (parse_vardct_file with `prefix`): group_passes[g] is the number of HF
+  // passes group g decodes with, the longest run of whole sections from pass 0 (frame_info.rs:548-565 check_group);
+  // hf_len is 0 for the sections past it. Empty group_passes: a frame parsed from a whole file.
+  bool prefix = false;
+  std::vector<uint8_t> group_passes;
+
   // the sub-frame jxg_parsed_region_desc handed out last (its pointers stay valid until the next call)
   std::unique_ptr<RegionSlice> region_tap;
 
@@ -121,11 +127,14 @@ void adaptive_lf_smoothing(FrameState& fs, int threads = 1);
 // groups, passes, encoding and the HF section bytes `hf_bytes`.
 void fill_image_info(const FileHeader& file, const FrameHeader& h, uint64_t hf_bytes, JxgImageInfo* info);
 
+// Which sections read_vardct_headers requires whole: every section, LfGlobal and the LF groups (a thumbnail), or those
+// and HfGlobal (a prefix decode). A one-section frame always needs its section whole.
+enum class WholeSections { kAll, kLf, kLfAndHfGlobal };
+
 // Container, headers, scope checks (everything outside this path's scope is refused with kErrUnsupported), the output
-// colour check and the TOC: fills fs.codestream, file, header, toc, sections_base, xb and yb. A section that does not fit
-// in the file is refused with kErrOutOfBounds: every section, or with `lf_sections_only` LfGlobal and the LF groups
-// (the single section of a one-section frame).
-void read_vardct_headers(FrameState& fs, const uint8_t* data, size_t size, bool lf_sections_only);
+// colour check and the TOC: fills fs.codestream, file, header, toc, sections_base, xb and yb. A required section that
+// does not fit in the file is refused with kErrOutOfBounds.
+void read_vardct_headers(FrameState& fs, const uint8_t* data, size_t size, WholeSections whole);
 // frame/decode.rs:307-427: LfGlobal of a VarDCT frame (quantiser, block context map, colour correlation, global tree,
 // extra-channel data).
 void decode_lf_global(FrameState& fs, BitReader& br);
@@ -136,7 +145,14 @@ void decode_lf_global(FrameState& fs, BitReader& br);
 // frame/decode.rs:429) on that many host threads: the latency path for one large image (a 16384x16384 frame has 64
 // LF groups and ~45 M Modular symbols); batches of many frames keep 1 and parallelise over frames instead. The
 // parsed state does not depend on `threads`.
-std::unique_ptr<FrameState> parse_vardct_file(const uint8_t* data, size_t size, int threads = 1);
+// `prefix`: `data` may end anywhere after HfGlobal (a bare codestream; a container must be whole). Sections are used
+// only when their whole byte range is inside `data` (frame_info.rs:302-328), and group g only with its passes
+// 0 .. group_passes[g] - 1 (see FrameState::group_passes).
+std::unique_ptr<FrameState> parse_vardct_file(const uint8_t* data, size_t size, int threads = 1, bool prefix = false);
+
+// Upsample8x::new (render/stages/upsample.rs:21-69): the 210 weights8 expanded by symmetry into the 64 5x5 kernels,
+// out[(oy * 8 + ox) * 25 + ky * 5 + kx] for output pixel (ox, oy) of an LF sample and input (x + kx - 2, y + ky - 2).
+void upsample8_kernel(const std::array<float, 210>& weights, float out[64 * 25]);
 
 // Test hook: decode the LF groups of serial parses one at a time instead of in lockstep pairs.
 void set_pair_lf_groups(bool on);

@@ -280,7 +280,7 @@ FileHeader read_file_header(BitReader& br) {
     if (h.custom_upsampling_mask & 2)
       for (int i = 0; i < 55; i++) read_f16(br);
     if (h.custom_upsampling_mask & 4)
-      for (int i = 0; i < 210; i++) read_f16(br);
+      for (float& v : h.weights8) v = read_f16(br);
   }
   if (h.color_encoding.want_icc) skip_icc(br);
   br.check();
@@ -296,6 +296,12 @@ static BlendingInfo read_blending(BitReader& br, uint32_t num_ec, bool full_fram
   if (uses_alpha || b.mode == 4) b.clamp = br.read_bool();
   if (!(full_frame && b.mode == 0)) b.source = u2s(br, V(0), V(1), V(2), V(3));
   return b;
+}
+
+std::array<float, 210> FileHeader::default_weights8() {
+  return {
+#include "upsample8_weights.inc"
+  };
 }
 
 FrameHeader read_frame_header(BitReader& br, const FileHeader& fh) {

@@ -69,6 +69,9 @@ struct FileHeader {
   float intensity_target = 255.0f;
   OpsinInverseMatrix opsin;
   uint32_t custom_upsampling_mask = 0;
+  // CustomTransformData.weights8 (transform_data.rs:343): the 8x upsampling weights, default or custom (mask bit 4)
+  std::array<float, 210> weights8 = default_weights8();
+  static std::array<float, 210> default_weights8();
 };
 
 struct Passes {

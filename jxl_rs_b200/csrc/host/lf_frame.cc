@@ -8,7 +8,7 @@ namespace jxg {
 std::unique_ptr<LfFrameState> parse_vardct_lf_file(const uint8_t* data, size_t size) {
   auto lp = std::make_unique<LfFrameState>();
   FrameState& fs = lp->fs;
-  read_vardct_headers(fs, data, size, /*lf_sections_only=*/true);
+  read_vardct_headers(fs, data, size, WholeSections::kLf);
   const FrameHeader& h = fs.header;
   const uint8_t* base = fs.codestream.data() + fs.sections_base;
   for (int c = 0; c < 3; c++) {

@@ -76,6 +76,25 @@ class ParsedFrame:
             self._h = C.c_void_p()
 
 
+class PrefixParsedFrame(ParsedFrame):
+    """A prefix of a VarDCT .jxl file (jxg_parse_file_prefix): a bare codestream cut anywhere after HfGlobal. Usable
+    with Batch.add (whole frame only): each HF group is decoded from the passes of it that have arrived, and a group
+    with none shows the LF image upsampled 8x. A complete prefix decodes as ParsedFrame does."""
+
+    def __init__(self, data: bytes):
+        self._lib = abi.load_library()
+        self._h = C.c_void_p()
+        self.info = abi.JxgImageInfo()
+        abi.check(self._lib, self._lib.jxg_parse_file_prefix(data, len(data), C.byref(self._h), C.byref(self.info)))
+
+    @property
+    def passes(self):
+        """k_g of each HF group (jxg_parsed_group_passes): the passes it is decoded with, 0 = LF upsampled 8x."""
+        out = np.zeros(self.info.num_groups, np.uint8)
+        abi.check(self._lib, self._lib.jxg_parsed_group_passes(self._h, out.ctypes.data, out.size))
+        return out
+
+
 def _region(region):
     x, y, w, h = (int(v) for v in region)
     return abi.JxgRegion(x, y, w, h)
@@ -702,6 +721,31 @@ def decode_thumbnails(ctx: JxgContext, files, pixel_format: JxlPixelFormat = Jxl
                 t = torch.empty((fr.height, fr.width, ch), dtype=dt, device=f"cuda:{ctx.device}")
             outs.append(t)
             batch.add_lf(fr, t.data_ptr(), fr.width * ch * t.element_size(), fmt, not to_host)
+        batch.run()
+        batch.wait()
+    finally:
+        batch.close()
+    return outs
+
+
+def decode_prefixes(ctx: JxgContext, files, pixel_format: JxlPixelFormat = JxlPixelFormat(), to_host: bool = True):
+    """Full-resolution pictures of partly received VarDCT files (PrefixParsedFrame: bare codestreams cut anywhere after
+    HfGlobal): H x W x C torch tensors of the display-oriented image, decoded in one batch."""
+    import torch
+    fmt = pixel_format.abi_format()
+    frames = [PrefixParsedFrame(f) for f in files]
+    ch = 4 if fmt == abi.FORMAT_RGBA_U8 else 3
+    dt = {abi.FORMAT_RGB_F32: torch.float32, abi.FORMAT_RGB_U16: torch.uint16, abi.FORMAT_RGB_F16: torch.float16}.get(fmt, torch.uint8)
+    batch = Batch(ctx, len(frames))
+    outs = []
+    try:
+        for fr in frames:
+            if to_host:
+                t = torch.empty((fr.height, fr.width, ch), dtype=dt).pin_memory()
+            else:
+                t = torch.empty((fr.height, fr.width, ch), dtype=dt, device=f"cuda:{ctx.device}")
+            outs.append(t)
+            batch.add(fr, t.data_ptr(), fr.width * ch * t.element_size(), fmt, not to_host)
         batch.run()
         batch.wait()
     finally:

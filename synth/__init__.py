@@ -140,7 +140,9 @@ def _header_words(header):
       color: {"factor": (selector 0..3, bits: 84 / 256 / bits + 2 (8 bits) / bits + 258 (16 bits)), "base_x",
       "base_b", "ytox_lf", "ytob_lf" (integers -128..127)};
       opsin: {"matrix": 9, "biases": 3, "quant_biases": 4};
-      cfl: (ytox, ytob), each one integer per 64x64 tile in raster order, any i32 (the decoder clamps to i8)."""
+      cfl: (ytox, ytob), each one integer per 64x64 tile in raster order, any i32 (the decoder clamps to i8);
+      weights8: the 210 CustomTransformData.weights8 (custom_weight_mask bit 4), the 8x upsampling weights a prefix
+      decode applies to groups without an HF pass."""
     if not header:
         return []
     words = []
@@ -168,6 +170,10 @@ def _header_words(header):
         ytox, ytob = (list(_flat(m)) for m in cfl)
         assert len(ytox) == len(ytob)
         words += [len(ytox)] + [int(v) for v in ytox] + [int(v) for v in ytob]
+    w8 = header.get("weights8")
+    if w8 is not None:  # a trailing group: arrays without it (and their files) stay as they were
+        assert len(w8) == 210
+        words += [1] + [int(x) & 0xFFFF for x in w8]
     return words
 
 

@@ -81,6 +81,8 @@ struct Params {
     uint32_t ytox_lf = 128, ytob_lf = 128;  // the 8-bit fields: value + 128
     bool ct_custom = false;         // CustomTransformData's OpsinInverseMatrix (transform_data.rs:18-32)
     uint16_t opsin[9] = {}, bias[3] = {}, qbias[4] = {};
+    bool w8_custom = false;         // CustomTransformData.weights8 (custom_weight_mask bit 4, transform_data.rs:343)
+    uint16_t weights8[210] = {};
     std::vector<int32_t> cfl_x, cfl_b;  // CfL tile maps, one value per 64x64 tile; empty: random small values
   } hdr = {};
 };
@@ -659,13 +661,17 @@ static void write_color_correlation(BitWriter& bw, const Params::HeaderSpec& hd)
 }
 
 static void write_custom_transform_data(BitWriter& out, const Params::HeaderSpec& hd) {  // transform_data.rs:325-345
-  out.write(hd.ct_custom ? 0 : 1, 1);
-  if (!hd.ct_custom) return;
-  out.write(0, 1);  // OpsinInverseMatrix all_default (xyb_encoded is always set)
-  for (uint16_t v : hd.opsin) out.write(v, 16);
-  for (uint16_t v : hd.bias) out.write(v, 16);
-  for (uint16_t v : hd.qbias) out.write(v, 16);
-  out.write(0, 3);  // custom_weight_mask: default upsampling weights
+  out.write(hd.ct_custom || hd.w8_custom ? 0 : 1, 1);
+  if (!hd.ct_custom && !hd.w8_custom) return;
+  out.write(hd.ct_custom ? 0 : 1, 1);  // OpsinInverseMatrix all_default (xyb_encoded is always set)
+  if (hd.ct_custom) {
+    for (uint16_t v : hd.opsin) out.write(v, 16);
+    for (uint16_t v : hd.bias) out.write(v, 16);
+    for (uint16_t v : hd.qbias) out.write(v, 16);
+  }
+  out.write(hd.w8_custom ? 4 : 0, 3);  // custom_weight_mask: only the 8x weights can be custom here
+  if (hd.w8_custom)
+    for (uint16_t v : hd.weights8) out.write(v, 16);
 }
 
 // RestorationFilter after its all_default bit (frame_header.rs:146-234), extensions included
@@ -1215,6 +1221,7 @@ static void read_header_words(const uint32_t* w, size_t n, Params::HeaderSpec& h
   const uint32_t tiles = next();
   for (uint32_t i = 0; i < tiles; i++) h.cfl_x.push_back(int32_t(next()));
   for (uint32_t i = 0; i < tiles; i++) h.cfl_b.push_back(int32_t(next()));
+  if (pos < n) group(h.w8_custom, h.weights8, 210);  // optional trailing group
   if (pos != n) throw std::runtime_error("header array too long");
 }
 
