@@ -466,15 +466,31 @@ int jxg_modular_batch_add_lf(void* batch, void* parsed, uint32_t output_format, 
  * jxg_parse_file_prefix takes a bare codestream cut anywhere after HfGlobal; LfGlobal, every LF group and HfGlobal must be
  * whole (JXG_ERR_OUT_OF_BOUNDS otherwise: a shorter prefix has only the thumbnail, jxg_lf_parse_file). A container must
  * be whole, and so must the section of a one-section frame (one group, one pass). The handle is an ordinary parsed frame
- * for jxg_batch_add_parsed, jxg_batch_read_coeffs, jxg_batch_read_xyb and jxg_parsed_free; info.hf_bytes counts the bytes
- * of the HF sections the decode uses. A complete prefix decodes exactly as jxg_parse_file + jxg_batch_add_parsed, with
- * the same kernels. jxg_parsed_desc (the descriptor has no per-group pass counts), jxg_batch_add_parsed_region and
- * jxg_parsed_region_desc refuse a prefix frame with JXG_ERR_ARGUMENT. A decode error in a section it uses is reported
- * by jxg_batch_wait as for a whole frame. */
+ * for jxg_batch_add_parsed, jxg_batch_add_parsed_region, jxg_batch_read_coeffs, jxg_batch_read_xyb and jxg_parsed_free;
+ * info.hf_bytes counts the bytes of the HF sections the decode uses. A complete prefix decodes exactly as
+ * jxg_parse_file + jxg_batch_add_parsed, with the same kernels. jxg_parsed_desc and jxg_parsed_region_desc refuse a prefix frame with JXG_ERR_ARGUMENT (a descriptor
+ * has no per-group pass counts). A decode error in a section it uses is reported by jxg_batch_wait as for a whole frame.
+ *
+ * A region of a prefix frame (jxg_batch_add_parsed_region): its pixels are the whole prefix decode's pixels
+ * (jxg_batch_add_parsed of the same handle) on that rectangle, byte-identical under the alignment rule of region
+ * decode above. The region takes the groups a region of the whole file takes, each with its k_g; only its groups with
+ * k_g > 0 are entropy-decoded, and its groups with k_g = 0 are upsampled in the coordinates of the whole frame, from the
+ * region's LF blocks and 2 LF samples around them (clipped to the image): rows mirror at the frame's LF edges and the
+ * two 0.0 margins above fall where they fall in the whole frame. When every group of the region has all passes, the
+ * region is decoded exactly as a region of the whole file, with the same kernels. jxg_batch_wait reports the group
+ * index of the whole frame. Region checks and codes are those of region decode. */
 int jxg_parse_file_prefix(const uint8_t* data, size_t size, void** parsed, JxgImageInfo* info);
 /* k_g of each HF group of a frame of jxg_parse_file_prefix, out[0 .. num_groups). JXG_ERR_ARGUMENT for another frame or
  * when n < the frame's group count. */
 int jxg_parsed_group_passes(void* parsed, uint8_t* out, uint32_t n);
+/* Parity tap, no device needed: the groups a region of a frame of jxg_parse_file_prefix decodes, as
+ * jxg_batch_add_parsed_region computes them. groups: their whole-frame indices in sub-frame order (row by row of the
+ * rectangle of groups); passes: their k_g; lf_window: the rectangle of the frame's LF image (x0, y0, x1, y1 in LF
+ * samples, half-open) uploaded for the upsampling, all zero when no group of the region has k_g = 0. *n_groups is always
+ * written; groups and passes may be NULL (only the count), otherwise max_groups must be at least *n_groups, and
+ * lf_window may be NULL. JXG_ERR_ARGUMENT for another frame and for a region a whole-file region refuses. */
+int jxg_parsed_prefix_region_plan(void* parsed, const JxgRegion* region, uint32_t* groups, uint8_t* passes,
+                                  uint32_t max_groups, uint32_t* n_groups, uint32_t lf_window[4]);
 
 const char* jxg_last_error(void);
 

@@ -456,6 +456,24 @@ static int add_frame_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_byt
     F.has_prefix = 1;
     APPEND(F.group_passes_off, group_passes, F.num_groups, 16);
     APPEND(F.up8_off, up8, 64 * 25 * 4, 16);
+    // the geometry of k_upsample_lf8: the frame's own, or that of the region's frame with its LF window
+    F.lf_w = F.xb;
+    F.lf_h = F.yb;
+    F.lfw_stride = F.xb;
+    for (int c = 0; c < 3; c++) F.lfw_off[c] = F.lf_off[c];
+    if (region) {
+      F.lf_w = region->lf_size[0];
+      F.lf_h = region->lf_size[1];
+      F.cone_gx0 = region->origin[0] / 256;
+      F.cone_gy0 = region->origin[1] / 256;
+      if (region->lf_window[2] > region->lf_window[0]) {  // a group without a pass: upload the window it reads
+        F.lfw_x0 = region->lf_window[0];
+        F.lfw_y0 = region->lf_window[1];
+        F.lfw_stride = region->lf_window[2] - region->lf_window[0];
+        const size_t n = size_t(F.lfw_stride) * (region->lf_window[3] - region->lf_window[1]);
+        for (int c = 0; c < 3; c++) APPEND(F.lfw_off[c], region->lf_win[c].data(), n * 4, 16);
+      }
+    }
   }
   F.section_base = uint32_t(b->sections.size());
   for (uint32_t s = 0; s < n_sections; s++) {
@@ -555,10 +573,12 @@ int jxg_batch_add_frame(void* bp, const JxgFrameDesc* d, const uint8_t* hf_bytes
 }
 
 // A region of a frame: the full descriptor is checked as jxg_batch_add_frame checks it, sliced to the sub-frame of the
-// region, and the sub-frame is added as an ordinary frame that stores only the region.
+// region, and the sub-frame is added as an ordinary frame that stores only the region. `group_passes` and `up8`: a
+// prefix frame, as for add_frame_impl; a region whose groups all have every pass is added as a region of a whole file.
 static int add_region_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_bytes, const uint64_t* sec_off,
                            const uint32_t* sec_len, uint32_t n_sections, const JxgRegion* region, void* out,
-                           size_t out_row_stride, int out_is_device, bool trusted) {
+                           size_t out_row_stride, int out_is_device, bool trusted, const uint8_t* group_passes = nullptr,
+                           const float* up8 = nullptr) {
   Batch* b = static_cast<Batch*>(bp);
   if (!b || !d || !hf_bytes || !sec_off || !sec_len || !out || !region) return JXG_ERR_ARGUMENT;
   if (d->abi_version != JXG_ABI_VERSION) return set_error(JXG_ERR_ARGUMENT, "ABI version mismatch");
@@ -567,9 +587,11 @@ static int add_region_impl(void* bp, const JxgFrameDesc* d, const uint8_t* hf_by
     if (int r = validate_desc(d, sec_len, n_sections)) return r;
   auto s = std::make_unique<jxg::RegionSlice>();
   const char* why = "";
-  if (int r = jxg::slice_region(*d, sec_off, sec_len, n_sections, *region, s.get(), &why)) return set_error(r, why);
+  if (int r = jxg::slice_region(*d, sec_off, sec_len, n_sections, *region, s.get(), &why, group_passes)) return set_error(r, why);
+  const bool short_group = std::any_of(s->group_passes.begin(), s->group_passes.end(), [&](uint8_t k) { return k < d->num_passes; });
   const int r = add_frame_impl(bp, &s->desc, hf_bytes, s->sec_off.data(), s->sec_len.data(), uint32_t(s->sec_off.size()), out,
-                               out_row_stride, out_is_device, /*trusted=*/true, s.get());
+                               out_row_stride, out_is_device, /*trusted=*/true, s.get(), short_group ? s->group_passes.data() : nullptr,
+                               short_group ? up8 : nullptr);
   if (r == JXG_OK) b->regions.push_back(std::move(s));
   return r;
 }
@@ -1056,11 +1078,34 @@ int jxg_batch_add_parsed_region(void* batch, void* parsed, uint32_t output_forma
                                 size_t out_row_stride, int out_is_device) {
   jxg::FrameState* fs = static_cast<jxg::FrameState*>(parsed);
   if (!fs) return JXG_ERR_ARGUMENT;
-  if (fs->prefix) return set_error(JXG_ERR_ARGUMENT, "a prefix frame has no region form");
   JxgFrameDesc d;
   fs->fill_desc(&d, output_format);
+  float up8[64 * 25];
+  if (fs->prefix) jxg::upsample8_kernel(fs->file.weights8, up8);
   return add_region_impl(batch, &d, fs->codestream.data(), fs->hf_off.data(), fs->hf_len.data(), uint32_t(fs->hf_off.size()),
-                         region, out, out_row_stride, out_is_device, /*trusted=*/true);
+                         region, out, out_row_stride, out_is_device, /*trusted=*/true,
+                         fs->prefix ? fs->group_passes.data() : nullptr, fs->prefix ? up8 : nullptr);
+}
+
+int jxg_parsed_prefix_region_plan(void* parsed, const JxgRegion* region, uint32_t* groups, uint8_t* passes,
+                                  uint32_t max_groups, uint32_t* n_groups, uint32_t lf_window[4]) {
+  jxg::FrameState* fs = static_cast<jxg::FrameState*>(parsed);
+  if (!fs || !region || !n_groups) return JXG_ERR_ARGUMENT;
+  if (!fs->prefix) return set_error(JXG_ERR_ARGUMENT, "prefix region plan: a frame of jxg_parse_file_prefix");
+  JxgFrameDesc d;
+  fs->fill_desc(&d, JXG_FORMAT_RGB_U8);
+  jxg::RegionSlice s;
+  const char* why = "";
+  if (int r = jxg::slice_region(d, fs->hf_off.data(), fs->hf_len.data(), uint32_t(fs->hf_off.size()), *region, &s, &why,
+                                fs->group_passes.data()))
+    return set_error(r, why);
+  const uint32_t n = uint32_t(s.real_group.size());
+  *n_groups = n;
+  if (lf_window) memcpy(lf_window, s.lf_window, sizeof(s.lf_window));
+  if ((groups || passes) && max_groups < n) return set_error(JXG_ERR_ARGUMENT, "prefix region plan: max_groups < the cone's groups");
+  if (groups) memcpy(groups, s.real_group.data(), size_t(n) * 4);
+  if (passes) memcpy(passes, s.group_passes.data(), n);
+  return JXG_OK;
 }
 
 int jxg_parsed_region_desc(void* parsed, uint32_t output_format, const JxgRegion* region, JxgFrameDesc* desc,

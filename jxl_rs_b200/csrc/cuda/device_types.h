@@ -99,6 +99,12 @@ struct FrameDev {
   // for the groups with none (k_upsample_lf8). has_prefix = 0: every group decodes num_passes passes.
   uint32_t has_prefix;
   uint64_t group_passes_off, up8_off;
+  // k_upsample_lf8 works in the coordinates of the whole frame, also when this frame is the sub-frame of a region: the
+  // frame's LF size (lf_w x lf_h blocks), the sub-frame's first group column and row in the frame (cone_gx0, cone_gy0),
+  // and the LF window it reads: channel c at lfw_off[c], its top-left (lfw_x0, lfw_y0) in the frame's LF image, rows of
+  // lfw_stride samples. A whole frame reads its own LF planes (lf_off, origin 0, stride xb).
+  uint32_t lf_w, lf_h, cone_gx0, cone_gy0, lfw_x0, lfw_y0, lfw_stride;
+  uint64_t lfw_off[3];
   // device-only buffers (element offsets)
   uint64_t coeff_group_base;  // group index base into coeffs
   uint64_t plane_base;        // float index base into plane sets (per channel: + c * plane_size)

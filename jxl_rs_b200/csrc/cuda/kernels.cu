@@ -2037,13 +2037,17 @@ __global__ void __launch_bounds__(256) k_upsample_lf8(const BatchDev B) {
   const StreamDev sd = B.streams_lf8[blockIdx.x];
   const FrameDev& F = B.frames[sd.frame];
   const uint32_t c = blockIdx.y, g = sd.group, tid = threadIdx.x;
-  const int lw = int(F.xb), lh = int(F.yb);
-  const int lx0 = int(g % F.xg) * 32, ly0 = int(g / F.xg) * 32;
+  // frame coordinates (FrameDev::lf_w): a region's sub-frame mirrors and fills margins where the whole frame does
+  const int lw = int(F.lf_w), lh = int(F.lf_h);
+  const int sx0 = int(F.cone_gx0) * 32, sy0 = int(F.cone_gy0) * 32;  // the sub-frame's LF origin
+  const int lx0 = sx0 + int(g % F.xg) * 32, ly0 = sy0 + int(g / F.xg) * 32;
   const int lx1 = min(lx0 + 32, lw), xs = lx1 - lx0, ys = min(32, lh - ly0);
   // upsample_lf_group's row buffer (decode.rs:80-111): the columns start_x .. end_x - 1 copied to position save_start
   const int start_x = max(lx0 - 2, 0), end_x = min(lx1 + 2, lw), cw = end_x - start_x;
   const int save_start = start_x == lx0 ? 2 : 0, save_end = save_start + cw;
-  const float* lf = reinterpret_cast<const float*>(B.blob + F.lf_off[c]);
+  // LF sample (x, y) of the frame is lf[(y - lfw_y0) * lfw_stride + x - lfw_x0]
+  const float* lf = reinterpret_cast<const float*>(B.blob + F.lfw_off[c]);
+  const int wx0 = int(F.lfw_x0), wy0 = int(F.lfw_y0);
   const float* kern = reinterpret_cast<const float*>(B.blob + F.up8_off);
   for (uint32_t i = tid; i < 64 * 25; i += blockDim.x) {
     const uint32_t o = i / 25, t = i % 25;  // o = oy * 8 + ox
@@ -2052,7 +2056,8 @@ __global__ void __launch_bounds__(256) k_upsample_lf8(const BatchDev B) {
   for (uint32_t i = tid; i < 36 * kUpWin; i += blockDim.x) {
     const int j = int(i) / kUpWin, col = int(i) % kUpWin;
     float v = 0.0f;  // the reference's buffer starts zeroed; slots past a short copy are never written
-    if (j < ys + 4 && col >= save_start && col < save_end) v = lf[size_t(mirror(ly0 - 2 + j, lh)) * lw + start_x + col - save_start];
+    if (j < ys + 4 && col >= save_start && col < save_end)
+      v = lf[size_t(mirror(ly0 - 2 + j, lh) - wy0) * F.lfw_stride + start_x + col - save_start - wx0];
     s_win[j][col] = v;
   }
   __syncthreads();
@@ -2086,7 +2091,7 @@ __global__ void __launch_bounds__(256) k_upsample_lf8(const BatchDev B) {
   const int x = int(tid >> 3), ox = int(tid & 7);
   if (x >= xs) return;
   float* plane = B.planes_a + F.plane_base + size_t(c) * F.plane_size;
-  const size_t col = size_t(lx0 + x) * 8 + ox;
+  const size_t col = size_t(lx0 - sx0 + x) * 8 + ox;
   for (int y = 0; y < ys; y++) {
     const float mn = s_min[y][x], mx = s_max[y][x];
     for (int oy = 0; oy < 8; oy++) {
@@ -2099,7 +2104,7 @@ __global__ void __launch_bounds__(256) k_upsample_lf8(const BatchDev B) {
         else a[t % 3] = fmaf(v, w, a[t % 3]);
       }
       const float v = __fadd_rn(__fadd_rn(a[0], a[1]), a[2]);
-      plane[size_t((ly0 + y) * 8 + oy) * F.plane_stride + col] = fminf(fmaxf(v, mn), mx);
+      plane[size_t((ly0 - sy0 + y) * 8 + oy) * F.plane_stride + col] = fminf(fmaxf(v, mn), mx);
     }
   }
 }

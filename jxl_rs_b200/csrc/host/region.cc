@@ -18,7 +18,7 @@ void slice_plane(const T* src, size_t src_stride, uint32_t x0, uint32_t y0, uint
 }  // namespace
 
 int slice_region(const JxgFrameDesc& full, const uint64_t* sec_off, const uint32_t* sec_len, uint32_t n_sections,
-                 const JxgRegion& r, RegionSlice* out, const char** why) {
+                 const JxgRegion& r, RegionSlice* out, const char** why, const uint8_t* group_passes) {
   auto bad = [&](const char* w) {
     *why = w;
     return int(JXG_ERR_ARGUMENT);
@@ -83,6 +83,26 @@ int slice_region(const JxgFrameDesc& full, const uint64_t* sec_off, const uint32
   slice_plane(full.quant_lf, xb, bx0, by0, sxb, syb, s.quant_lf);
   slice_plane(full.ytox_map, cxb, bx0 / 8, by0 / 8, scxb, scyb, s.ytox_map);
   slice_plane(full.ytob_map, cxb, bx0 / 8, by0 / 8, scxb, scyb, s.ytob_map);
+  // a prefix frame: the sub-frame's pass counts and, for its groups without a pass, the LF window of the upsampling
+  const uint32_t yb = (Hh + 7) / 8;
+  s.group_passes.clear();
+  for (int c = 0; c < 3; c++) s.lf_win[c].clear();
+  std::fill(s.lf_size, s.lf_size + 2, 0u);
+  std::fill(s.lf_window, s.lf_window + 4, 0u);
+  if (group_passes) {
+    for (uint32_t g : s.real_group) s.group_passes.push_back(group_passes[g]);
+    s.lf_size[0] = xb;
+    s.lf_size[1] = yb;
+    if (std::find(s.group_passes.begin(), s.group_passes.end(), uint8_t(0)) != s.group_passes.end()) {
+      const uint32_t wx0 = bx0 > 2 ? bx0 - 2 : 0, wy0 = by0 > 2 ? by0 - 2 : 0;
+      const uint32_t wx1 = std::min(xb, bx0 + sxb + 2), wy1 = std::min(yb, by0 + syb + 2);
+      s.lf_window[0] = wx0;
+      s.lf_window[1] = wy0;
+      s.lf_window[2] = wx1;
+      s.lf_window[3] = wy1;
+      for (int c = 0; c < 3; c++) slice_plane(full.lf[c], xb, wx0, wy0, wx1 - wx0, wy1 - wy0, s.lf_win[c]);
+    }
+  }
   s.desc = full;
   s.desc.width = sw;
   s.desc.height = sh;

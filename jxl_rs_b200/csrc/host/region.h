@@ -8,6 +8,11 @@
 // * with Gaborish + EPF 2 (the only configuration with a vector filter path) the halo is taken around the filter tiles
 //   that meet the region, so that each of them is interior in the sub-frame exactly when it is interior in the frame and
 //   takes the same path.
+// A region of a prefix frame (jxg_parse_file_prefix) takes the same groups. A group there without an HF pass (k_g = 0)
+// is the LF image upsampled 8x (k_upsample_lf8), whose window reads LF samples up to 2 columns and rows outside the
+// group, mirrors rows at the frame's LF height and takes its column margins from the frame's LF width. Those are LF
+// samples, not neighbouring HF groups, so the selection does not grow; instead the sub-frame carries the frame's LF
+// geometry and an LF window (its LF blocks grown by 2, clipped to the frame), and the kernel works in frame coordinates.
 #pragma once
 #include <cstdint>
 #include <vector>
@@ -28,6 +33,13 @@ struct RegionSlice {
   std::vector<uint8_t> transform_map, epf_map, quant_lf;
   std::vector<int32_t> raw_quant_map;
   std::vector<int8_t> ytox_map, ytob_map;
+  // A region of a prefix frame: the passes of each sub-frame group (group_passes[real_group[i]]), the frame's LF size
+  // (blocks across and down) and, when one of those pass counts is 0, the LF window the upsampling reads: x0, y0, x1, y1
+  // (half-open) of the frame's LF image and its three planes. All zero and empty otherwise.
+  std::vector<uint8_t> group_passes;
+  uint32_t lf_size[2] = {0, 0};
+  uint32_t lf_window[4] = {0, 0, 0, 0};
+  std::vector<float> lf_win[3];
 };
 
 // Coded pixel of display pixel (dx, dy) for a coded w x h frame: the inverse of display_pixel
@@ -69,8 +81,9 @@ constexpr uint32_t filter_halo(bool gab, uint32_t epf_iters) {
 
 // Slices `full` (and its n_sections sections) to the region r, given in display coordinates (the frame's orientation
 // applied; XYB output has none). Returns 0, or JXG_ERR_ARGUMENT with *why set when the region is empty or leaves the
-// image, or the output format is XYB_F32_PLANAR.
+// image, or the output format is XYB_F32_PLANAR. `group_passes` (a prefix frame: the passes of each group of the frame,
+// nullptr otherwise) fills the prefix fields of the slice.
 int slice_region(const JxgFrameDesc& full, const uint64_t* sec_off, const uint32_t* sec_len, uint32_t n_sections,
-                 const JxgRegion& r, RegionSlice* out, const char** why);
+                 const JxgRegion& r, RegionSlice* out, const char** why, const uint8_t* group_passes = nullptr);
 
 }  // namespace jxg

@@ -78,8 +78,8 @@ class ParsedFrame:
 
 class PrefixParsedFrame(ParsedFrame):
     """A prefix of a VarDCT .jxl file (jxg_parse_file_prefix): a bare codestream cut anywhere after HfGlobal. Usable
-    with Batch.add (whole frame only): each HF group is decoded from the passes of it that have arrived, and a group
-    with none shows the LF image upsampled 8x. A complete prefix decodes as ParsedFrame does."""
+    with Batch.add, whole or with a region: each HF group is decoded from the passes of it that have arrived, and a
+    group with none shows the LF image upsampled 8x. A complete prefix decodes as ParsedFrame does."""
 
     def __init__(self, data: bytes):
         self._lib = abi.load_library()
@@ -93,6 +93,19 @@ class PrefixParsedFrame(ParsedFrame):
         out = np.zeros(self.info.num_groups, np.uint8)
         abi.check(self._lib, self._lib.jxg_parsed_group_passes(self._h, out.ctypes.data, out.size))
         return out
+
+    def region_plan(self, region):
+        """The groups a region (x, y, w, h in output coordinates) decodes (jxg_parsed_prefix_region_plan), no device
+        needed: (groups, passes, lf_window) with groups their whole-frame indices in sub-frame order, passes their k_g,
+        and lf_window the LF rectangle (x0, y0, x1, y1) uploaded for the upsampling, (0, 0, 0, 0) when none is."""
+        reg = C.byref(_region(region))
+        n = C.c_uint32()
+        abi.check(self._lib, self._lib.jxg_parsed_prefix_region_plan(self._h, reg, None, None, 0, C.byref(n), None))
+        groups, passes = np.zeros(n.value, np.uint32), np.zeros(n.value, np.uint8)
+        win = (C.c_uint32 * 4)()
+        abi.check(self._lib, self._lib.jxg_parsed_prefix_region_plan(self._h, reg, groups.ctypes.data, passes.ctypes.data,
+                                                                     n.value, C.byref(n), win))
+        return groups, passes, tuple(win)
 
 
 def _region(region):
@@ -728,24 +741,32 @@ def decode_thumbnails(ctx: JxgContext, files, pixel_format: JxlPixelFormat = Jxl
     return outs
 
 
-def decode_prefixes(ctx: JxgContext, files, pixel_format: JxlPixelFormat = JxlPixelFormat(), to_host: bool = True):
+def decode_prefixes(ctx: JxgContext, files, pixel_format: JxlPixelFormat = JxlPixelFormat(), to_host: bool = True,
+                    regions=None):
     """Full-resolution pictures of partly received VarDCT files (PrefixParsedFrame: bare codestreams cut anywhere after
-    HfGlobal): H x W x C torch tensors of the display-oriented image, decoded in one batch."""
+    HfGlobal): H x W x C torch tensors of the display-oriented image, decoded in one batch.
+    regions: None, or one entry per file: None (the whole image) or (x, y, w, h) in output coordinates, which decodes
+    only that rectangle into an h x w x C tensor."""
     import torch
     fmt = pixel_format.abi_format()
+    if regions is None:
+        regions = [None] * len(files)
+    if len(regions) != len(files):
+        raise ValueError("regions: one entry per file")
     frames = [PrefixParsedFrame(f) for f in files]
     ch = 4 if fmt == abi.FORMAT_RGBA_U8 else 3
     dt = {abi.FORMAT_RGB_F32: torch.float32, abi.FORMAT_RGB_U16: torch.uint16, abi.FORMAT_RGB_F16: torch.float16}.get(fmt, torch.uint8)
     batch = Batch(ctx, len(frames))
     outs = []
     try:
-        for fr in frames:
+        for fr, reg in zip(frames, regions):
+            h, w = _out_size(fr, reg)
             if to_host:
-                t = torch.empty((fr.height, fr.width, ch), dtype=dt).pin_memory()
+                t = torch.empty((h, w, ch), dtype=dt).pin_memory()
             else:
-                t = torch.empty((fr.height, fr.width, ch), dtype=dt, device=f"cuda:{ctx.device}")
+                t = torch.empty((h, w, ch), dtype=dt, device=f"cuda:{ctx.device}")
             outs.append(t)
-            batch.add(fr, t.data_ptr(), fr.width * ch * t.element_size(), fmt, not to_host)
+            batch.add(fr, t.data_ptr(), w * ch * t.element_size(), fmt, not to_host, reg)
         batch.run()
         batch.wait()
     finally:

@@ -4,7 +4,9 @@ each cut at the end of HfGlobal (every group the LF image upsampled 8x), half wa
 Reports, as one JSON line, per cut: the bytes of the files kept, and the device time of one batch of all frames
 (RGB_U8, device outputs; median of CUDA events around `--reps` reruns after `--warmup`), also as a share of the
 whole-file batch; with the card's name and power limit read in the same run.
-Usage: python tools/bench_prefix.py [--frames 64] [--reps 20] [--warmup 5] [--distance 0.5]"""
+--region: per cut, a centred 512x512 region and a centred 1920x1080 quarter of every frame
+(jxg_batch_add_parsed_region) against the whole prefix decode at the same cut: device ms and H2D bytes per batch.
+Usage: python tools/bench_prefix.py [--frames 64] [--reps 20] [--warmup 5] [--distance 0.5] [--region]"""
 import argparse
 import json
 import os
@@ -22,15 +24,19 @@ def card():
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
 
 
-def batch_ms(ctx, frames, outs, reps, warmup):
+def batch_ms(ctx, frames, outs, reps, warmup, region=None, stats=None):
+    """Median device ms of one batch of `frames` (each whole, or the region (x, y, w, h)); `stats` receives the
+    batch's stats() of its first run."""
     import torch
     import jxl_rs_b200 as j
     b = j.Batch(ctx, len(frames))
     try:
         for fr, t in zip(frames, outs):
-            b.add(fr, t.data_ptr(), fr.width * 3, 0, True)
+            b.add(fr, t.data_ptr(), (fr.width if region is None else region[2]) * 3, 0, True, region)
         b.run()
         b.wait()
+        if stats is not None:
+            stats.update(b.stats())
         st = torch.cuda.Stream()
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         times = []
@@ -54,6 +60,7 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--distance", type=float, default=0.5, help="synth.encode_synthetic distance (bench.py's 0.5)")
+    ap.add_argument("--region", action="store_true", help="regions of each prefix against the whole prefix")
     a = ap.parse_args()
     import torch
     import jxl_rs_b200 as j
@@ -68,6 +75,17 @@ def main():
     ctx = j.JxgContext(0)
     try:
         outs = [torch.empty((2160, 3840, 3), dtype=torch.uint8, device="cuda:0") for _ in files]
+        if a.region:
+            regions = {"whole": None, "512x512": (1664, 824, 512, 512), "1920x1080": (960, 540, 1920, 1080)}
+            for name, cut in cuts.items():
+                frames = [j.PrefixParsedFrame(f[:c]) for f, c in zip(files, cut)]
+                res[name] = {}
+                for rname, reg in regions.items():
+                    st = {}
+                    t = batch_ms(ctx, frames, outs, a.reps, a.warmup, reg, st)
+                    res[name][rname] = {"device_ms_per_batch": t, "h2d_bytes_per_batch": st["h2d_bytes"]}
+            print(json.dumps(res))
+            return
         ms = {}
         for name, cut in cuts.items():
             frames = [j.PrefixParsedFrame(f[:c]) for f, c in zip(files, cut)]
