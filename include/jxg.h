@@ -344,27 +344,51 @@ int jxg_parsed_region_desc(void* parsed, uint32_t output_format, const JxgRegion
  * ConvertI32ToU8 (render/stages/convert.rs:642). The host front end (headers, LfGlobal incl. the global MA tree,
  * section 0, ModularLF streams, group headers / local trees) is jxg_modular_parse_file; a Rust host would hand over
  * the same state from Frame::decode_lf_global / decode_lf_group (frame/decode.rs:307-497).
- * Device scope: 8-bit RGB / grey, one pass, global transforms RCT and Squeeze, group-local RCT, ANS or prefix codes,
+ * Device scope: lossless 8-bit RGB / grey and lossy (XYB-encoded) frames, one pass, global transforms RCT and Squeeze,
+ * group-local RCT, ANS or prefix codes,
  * all 14 predictors incl. the weighted one, all properties incl. those of reference channels, the global palette
  * transform without delta entries (transforms/palette.rs:165-199), LZ77 in group streams (decode.rs:286-330, the window
  * in device memory: min(2^20, pixels) x 4 bytes per LZ77 stream). Delta palettes return JXG_ERR_UNSUPPORTED (no CPU
  * fallback). A group stream that fails (ANS checksum, over-read, an LZ77 copy before any symbol or a copy length
- * overflow: JXG_ERR_LZ77) is reported by jxg_modular_batch_wait; the other streams still decode. Output: interleaved
- * RGB u8 (grey replicated). Frames of one batch must agree on the kind of each inverse-transform step they share: one
+ * overflow: JXG_ERR_LZ77) is reported by jxg_modular_batch_wait; the other streams still decode. Output of a lossless
+ * frame: interleaved RGB u8 (grey replicated), ConvertI32ToU8. An XYB frame (ImageMetadata.xyb_encoded, what lossy
+ * Modular encoders write) codes three channels Y, X, B whatever its colour encoding (frame/decode.rs:167-170); they are
+ * converted as ConvertModularXYBToF32Stage does (render/stages/convert.rs:278-343: X = x s_x, Y = y s_y,
+ * B = (b + y) s_b with the frame's LfQuantFactors) and stored through the output stage of a VarDCT frame (XYB to the
+ * output colour, transfer curve, sample conversion with the u8 dither at frame coordinates, orientation), in any
+ * JXG_FORMAT_* (jxg_modular_batch_add_output). An XYB frame with Gaborish or EPF enabled is refused with
+ * JXG_ERR_UNSUPPORTED at the parse: those filters are not applied to Modular frames here. Frames of one batch must agree on the kind of each inverse-transform step they share: one
  * frame's step list may be a prefix of another's, in either order of adding. A frame jxg_modular_batch_add refuses
  * leaves the batch as it was (no stream of it decodes, no statistic counts it); a group-local Squeeze is refused with
  * JXG_ERR_UNSUPPORTED. A rectangle of a frame can be decoded alone (jxg_modular_batch_add_region). */
 int jxg_modular_parse_file(const uint8_t* data, size_t size, void** parsed, JxgImageInfo* info);
 void jxg_modular_parsed_free(void* parsed);
 int jxg_modular_batch_begin(void* ctx, void** batch);
-/* `parsed` must stay alive until jxg_modular_batch_end. */
+/* `parsed` must stay alive until jxg_modular_batch_end. Output RGB_U8 (an XYB frame too); the same as
+ * jxg_modular_batch_add_output with JXG_FORMAT_RGB_U8 and no region. */
 int jxg_modular_batch_add(void* batch, void* parsed, void* out, size_t out_row_stride, int out_is_device);
+/* Adds a frame, or the region `region` of it (NULL: the whole frame; see jxg_modular_batch_add_region), in output
+ * format `output_format`. An XYB frame takes every format, with the stride and alignment rules of jxg_batch_add_frame
+ * applied to the frame's or region's width; XYB_F32_PLANAR writes the X, Y, B planes of the whole frame in the coded
+ * orientation (3 x coded height rows of coded width f32) and has no region form (JXG_ERR_ARGUMENT). A lossless frame
+ * takes RGB_U8 only, and is then exactly jxg_modular_batch_add / _add_region; any other format returns
+ * JXG_ERR_UNSUPPORTED. An unknown format returns JXG_ERR_ARGUMENT. A refused frame leaves the batch as it was. */
+int jxg_modular_batch_add_output(void* batch, void* parsed, uint32_t output_format, const JxgRegion* region, void* out,
+                                 size_t out_row_stride, int out_is_device);
+/* The colour side of a parsed Modular frame, no device needed: *xyb_encoded (1: an XYB frame), the coded colour
+ * channels (3 for every XYB frame), and for an XYB frame its LfQuantFactors (lf_quant[3], X, Y, B) and in `desc` the
+ * output stage a batch applies for output_format: width, height, orientation, output_format, opsin_biases,
+ * intensity_target, output_tf, output_gamma, output_luminances, opsin_inverse_matrix (every other field zero). Any
+ * pointer may be NULL; lf_quant and desc are not written for a lossless frame. An unknown format: JXG_ERR_ARGUMENT. */
+int jxg_modular_parsed_colour(void* parsed, uint32_t output_format, int* xyb_encoded, uint32_t* colour_channels,
+                              float* lf_quant, JxgFrameDesc* desc);
 
 /* ---- Region decode of Modular frames ----------------------------------------------------------------------------
  * A region is a JxgRegion rectangle of the OUTPUT image (display orientation, the JxgImageInfo width x height of
  * jxg_modular_parse_file). Its pixels are defined as the pixels of the whole-frame decode on that rectangle, and they
  * are byte-identical to them for every orientation, host and device outputs and any valid stride: everything up to the
- * u8 store is integer arithmetic. The output holds region.height rows of region.width RGB u8 pixels; the stride rule
+ * u8 store is integer arithmetic, and an XYB frame's conversion and output stage are per pixel, with the u8 dither at
+ * whole-frame coordinates. The output holds region.height rows of region.width RGB u8 pixels; the stride rule
  * is that of jxg_modular_batch_add applied to the region's width (JXG_ERR_INVALID_OUTPUT). An empty region or one
  * outside the image returns JXG_ERR_ARGUMENT; a frame jxg_modular_batch_add refuses is refused with the same code, and
  * a refused region leaves the batch as it was. Only the group streams the region depends on are uploaded and decoded,
@@ -391,7 +415,8 @@ int jxg_modular_batch_run(void* batch, void* cuda_stream);
 int jxg_modular_batch_wait(void* batch, uint32_t* first_bad_frame, uint32_t* first_bad_group);
 /* Ordered after the batch's own last run, whichever stream that ran on. */
 int jxg_modular_batch_rerun_device(void* batch, void* cuda_stream);
-/* Parity tap: final colour planes of frame f (3 x H x W i32, before the u8 conversion), after waiting for the
+/* Parity tap: final colour planes of frame f (3 x H x W i32, before the u8 conversion; Y, X, B of an XYB frame before
+ * its conversion to XYB floats), after waiting for the
  * batch's own last run on whichever stream it ran. JXG_ERR_ARGUMENT for a region frame. */
 int jxg_modular_batch_read_planes(void* batch, uint32_t f, int32_t* out, size_t out_len);
 /* ms[0]: whole batch on the device, ms[1]: group-stream decode kernel (+ local RCT). */

@@ -83,7 +83,7 @@ EXPORTS = [
     "jxg_parsed_region_desc", "jxg_context_set_sm_budget", "jxg_batch_entropy_schedule", "jxg_batch_stream_status",
     "jxg_batch_read_transform_plan", "jxg_modular_batch_add_region", "jxg_modular_parsed_region_plan",
     "jxg_lf_parse_file", "jxg_lf_parsed_free", "jxg_modular_batch_add_lf", "jxg_parse_file_prefix", "jxg_parsed_group_passes",
-    "jxg_parsed_prefix_region_plan",
+    "jxg_parsed_prefix_region_plan", "jxg_modular_batch_add_output", "jxg_modular_parsed_colour",
 ]
 
 ALL_FRAMES = 0xFFFFFFFF  # JXG_ALL_FRAMES
@@ -174,6 +174,9 @@ def load_library():
     lib.jxg_parse_file_prefix.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(vp), C.POINTER(JxgImageInfo)]
     lib.jxg_parsed_group_passes.argtypes = [vp, vp, C.c_uint32]
     lib.jxg_parsed_prefix_region_plan.argtypes = [vp, rp, vp, vp, C.c_uint32, u32p, vp]
+    lib.jxg_modular_batch_add_output.argtypes = [vp, vp, C.c_uint32, rp, vp, C.c_size_t, C.c_int]
+    lib.jxg_modular_parsed_colour.argtypes = [vp, C.c_uint32, C.POINTER(C.c_int), u32p, C.POINTER(C.c_float),
+                                              C.POINTER(JxgFrameDesc)]
     _LIB = lib
     return lib
 

@@ -33,7 +33,7 @@ struct MFrame {
   bool out_is_device;
   bool region = false;             // a region of the frame (jxg_modular_batch_add_region)
   size_t out_row_bytes = 0, out_rows = 0;  // the output's rows as the store writes them
-  size_t store_index = 0;          // its job in store_jobs, or in lf_store_jobs for a thumbnail
+  size_t store_index = 0;          // its job in store_jobs, xyb_store_jobs (ms->xyb) or lf_store_jobs (a thumbnail)
   jxg::ModularRegionPlan plan;     // the cone: per buffer the rectangle the arena holds, the streams decoded
   uint64_t arena_base = 0;         // element offset of this frame's planes
   std::vector<uint64_t> buf_off;   // per plan buffer, element offset in the arena of its arena rectangle's top-left
@@ -60,6 +60,7 @@ struct ModularBatch : BatchCore {
   std::vector<std::vector<MJobDev>> levels;  // jobs grouped by plan step index
   std::vector<jxg::ModularJobKind> level_kind;
   std::vector<MJobDev> store_jobs;
+  std::vector<MJobDev> xyb_store_jobs;  // the stores of XYB frames
   std::vector<MJobDev> lf_dequant_jobs, lf_smooth_jobs, lf_store_jobs;  // thumbnails: one job per LF stream / frame
   uint64_t arena_elems = 0, wp_bytes = 0, out_bytes = 0;
   uint64_t lz_window_elems = 0;             // symbol windows of the LZ77 streams, one per stream
@@ -215,8 +216,8 @@ bool build_walk_table(const jxg::ModularTree& t, uint32_t root, uint32_t ci, uin
 
 // Everything add_frame appends to, so that a refused frame leaves the batch as it was (jxg_modular_batch_add).
 struct BatchMark {
-  size_t frames, streams, rct_streams, rects, codes, rcts, refs, levels, store_jobs, lf_dequant_jobs, lf_smooth_jobs,
-      lf_store_jobs, blob, blob_pending;
+  size_t frames, streams, rct_streams, rects, codes, rcts, refs, levels, store_jobs, xyb_store_jobs, lf_dequant_jobs,
+      lf_smooth_jobs, lf_store_jobs, blob, blob_pending;
   std::vector<size_t> level_jobs;
   uint64_t arena_elems, wp_bytes, out_bytes, lz_window_elems;
   uint32_t lz77_streams, rle_streams;
@@ -225,7 +226,7 @@ struct BatchMark {
   explicit BatchMark(const ModularBatch* b)
       : frames(b->frames.size()), streams(b->streams.size()), rct_streams(b->rct_streams.size()), rects(b->rects.size()),
         codes(b->codes.size()), rcts(b->rcts.size()), refs(b->refs.size()), levels(b->levels.size()),
-        store_jobs(b->store_jobs.size()), lf_dequant_jobs(b->lf_dequant_jobs.size()),
+        store_jobs(b->store_jobs.size()), xyb_store_jobs(b->xyb_store_jobs.size()), lf_dequant_jobs(b->lf_dequant_jobs.size()),
         lf_smooth_jobs(b->lf_smooth_jobs.size()), lf_store_jobs(b->lf_store_jobs.size()), blob(b->ctx->blob.size), blob_pending(b->ctx->blob.pending.size()),
         arena_elems(b->arena_elems), wp_bytes(b->wp_bytes), out_bytes(b->out_bytes), lz_window_elems(b->lz_window_elems),
         lz77_streams(b->lz77_streams), rle_streams(b->rle_streams), walks(b->walks) {
@@ -243,6 +244,7 @@ struct BatchMark {
     b->level_kind.resize(levels);
     for (size_t l = 0; l < levels; l++) b->levels[l].resize(level_jobs[l]);
     b->store_jobs.resize(store_jobs);
+    b->xyb_store_jobs.resize(xyb_store_jobs);
     b->lf_dequant_jobs.resize(lf_dequant_jobs);
     b->lf_smooth_jobs.resize(lf_smooth_jobs);
     b->lf_store_jobs.resize(lf_store_jobs);
@@ -490,8 +492,10 @@ void add_plan(ModularBatch* b, const MFrame& f) {
   }
 }
 
-// Store job: the coded window of the final colour planes -> the u8 output, in the file's orientation (render/save.rs).
-void add_store(ModularBatch* b, MFrame& f) {
+// Store job: the coded window of the final colour planes -> the output, in the file's orientation (render/save.rs).
+// A lossless frame: k_modular_store's u8 clamp. An XYB frame: k_xyb_store's conversion and output stage in `format`,
+// its parameters in the blob; XYB_F32_PLANAR keeps the coded orientation (whole frames only, see add_frame).
+void add_store(ModularBatch* b, MFrame& f, uint32_t format) {
   const jxg::ModularFrameState* ms = f.ms;
   const uint32_t W = ms->header.xsize(), H = ms->header.ysize();
   MJobDev sj;
@@ -512,12 +516,32 @@ void add_store(ModularBatch* b, MFrame& f) {
   sj.out_y = f.plan.out_y;
   f.out_row_bytes = size_t(f.plan.out_w) * 3;
   f.out_rows = f.plan.out_h;
+  if (ms->xyb) {
+    const bool planar = format == JXG_FORMAT_XYB_F32_PLANAR;
+    MLfFrameDev p;
+    memset(&p, 0, sizeof(p));
+    memcpy(p.lf_factors, ms->lf_quant, sizeof(p.lf_factors));
+    JxgFrameDesc d;
+    memset(&d, 0, sizeof(d));
+    jxg::fill_output_colour(ms->file, format, &d);
+    set_output_colour(p, &d);
+    sj.params = blob_append(b, &p, sizeof(p));
+    if (planar) sj.op = 1;
+    f.out_row_bytes = (planar ? size_t(W) : size_t(f.plan.out_w)) * format_bpp(format);
+    f.out_rows = planar ? size_t(3) * H : f.plan.out_h;
+  }
   if (!f.out_is_device) {
     f.dev_out_off = b->out_bytes;
     b->out_bytes += (f.out_row_bytes * f.out_rows + 255) & ~size_t(255);
   }
-  f.store_index = b->store_jobs.size();
-  b->store_jobs.push_back(sj);
+  std::vector<MJobDev>& list = ms->xyb ? b->xyb_store_jobs : b->store_jobs;
+  f.store_index = list.size();
+  list.push_back(sj);
+}
+
+MJobDev& store_job(ModularBatch* b, const MFrame& f) {
+  if (f.lf) return b->lf_store_jobs[f.store_index];
+  return (f.ms->xyb ? b->xyb_store_jobs : b->store_jobs)[f.store_index];
 }
 
 // The frame checks of jxg_modular_batch_add, for the whole frame and for any region of it alike.
@@ -545,10 +569,18 @@ void plan_frame(const jxg::ModularFrameState* ms, const JxgRegion* region, jxg::
   check_frame(ms);
 }
 
-void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, const JxgRegion* region, void* out, size_t stride, bool is_device) {
+// A whole frame or a region in output format `format`: RGB_U8 for a lossless frame, any format for an XYB frame.
+void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, uint32_t format, const JxgRegion* region, void* out,
+               size_t stride, bool is_device) {
+  const size_t bpp = format_bpp(format);
+  if (!bpp) throw jxg::Error(JXG_ERR_ARGUMENT, "unknown output format");
+  if (!ms->xyb && format != JXG_FORMAT_RGB_U8)
+    throw jxg::Error(JXG_ERR_UNSUPPORTED, "a lossless Modular frame is stored as RGB_U8 only");
+  if (region && format == JXG_FORMAT_XYB_F32_PLANAR) throw jxg::Error(JXG_ERR_ARGUMENT, "XYB_F32_PLANAR has no region form");
   MFrame f;
   plan_frame(ms, region, f.plan);
-  if (stride < size_t(f.plan.out_w) * 3) throw jxg::Error(JXG_ERR_INVALID_OUTPUT, "output row stride too small");
+  const uint32_t width = format == JXG_FORMAT_XYB_F32_PLANAR ? ms->header.xsize() : f.plan.out_w;
+  if (int r = check_output(bpp, width, stride, out, is_device)) throw jxg::Error(r, g_error);
   check_plan(ms);
   f.ms = ms;
   f.region = region != nullptr;
@@ -562,7 +594,7 @@ void add_frame(ModularBatch* b, jxg::ModularFrameState* ms, const JxgRegion* reg
                                 base = buf_index(f, r.chan, r.x0, r.y0);
                               }});
   add_plan(b, f);
-  add_store(b, f);
+  add_store(b, f, format);
   b->frames.push_back(std::move(f));
 }
 
@@ -674,9 +706,10 @@ int launch_all(ModularBatch* b, cudaStream_t s, bool copy_to_host) {
     b->launches++;
   };
   for (size_t l = 0; l < b->levels.size(); l++) launch_jobs(b->level_kind[l], b->levels[l]);
-  // the jobs of the Modular frames' stores, then the thumbnails' jobs in stage order (each kind waits for the one before)
-  const std::pair<jxg::ModularJobKind, const std::vector<MJobDev>*> tail[4] = {
-      {jxg::kJobStore, &b->store_jobs}, {jxg::kJobLfDequant, &b->lf_dequant_jobs},
+  // the jobs of the Modular frames' stores (lossless, then XYB), then the thumbnails' jobs in stage order (each kind
+  // waits for the one before)
+  const std::pair<jxg::ModularJobKind, const std::vector<MJobDev>*> tail[5] = {
+      {jxg::kJobStore, &b->store_jobs}, {jxg::kJobXybStore, &b->xyb_store_jobs}, {jxg::kJobLfDequant, &b->lf_dequant_jobs},
       {jxg::kJobLfSmooth, &b->lf_smooth_jobs}, {jxg::kJobLfStore, &b->lf_store_jobs}};
   for (const auto& [kind, list] : tail)
     if (!list->empty()) launch_jobs(kind, *list);
@@ -729,7 +762,8 @@ int jxg_modular_batch_add(void* bp, void* parsed, void* out, size_t out_row_stri
   if (b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch already submitted");
   const BatchMark mark(b);
   try {
-    add_frame(b, static_cast<jxg::ModularFrameState*>(parsed), nullptr, out, out_row_stride, out_is_device != 0);
+    add_frame(b, static_cast<jxg::ModularFrameState*>(parsed), JXG_FORMAT_RGB_U8, nullptr, out, out_row_stride,
+              out_is_device != 0);
     return JXG_OK;
   } catch (jxg::Error& e) {
     mark.restore(b);  // a refused frame leaves nothing behind: no streams decode for it, no stats count it
@@ -744,12 +778,48 @@ int jxg_modular_batch_add_region(void* bp, void* parsed, const JxgRegion* region
   if (b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch already submitted");
   const BatchMark mark(b);
   try {
-    add_frame(b, static_cast<jxg::ModularFrameState*>(parsed), region, out, out_row_stride, out_is_device != 0);
+    add_frame(b, static_cast<jxg::ModularFrameState*>(parsed), JXG_FORMAT_RGB_U8, region, out, out_row_stride,
+              out_is_device != 0);
     return JXG_OK;
   } catch (jxg::Error& e) {
     mark.restore(b);
     return set_error(e.code, e.what());
   }
+}
+
+int jxg_modular_batch_add_output(void* bp, void* parsed, uint32_t output_format, const JxgRegion* region, void* out,
+                                 size_t out_row_stride, int out_is_device) {
+  ModularBatch* b = static_cast<ModularBatch*>(bp);
+  if (!b || !parsed || !out) return JXG_ERR_ARGUMENT;
+  if (b->uploaded) return set_error(JXG_ERR_ARGUMENT, "batch already submitted");
+  const BatchMark mark(b);
+  try {
+    add_frame(b, static_cast<jxg::ModularFrameState*>(parsed), output_format, region, out, out_row_stride,
+              out_is_device != 0);
+    return JXG_OK;
+  } catch (jxg::Error& e) {
+    mark.restore(b);
+    return set_error(e.code, e.what());
+  }
+}
+
+int jxg_modular_parsed_colour(void* parsed, uint32_t output_format, int* xyb_encoded, uint32_t* colour_channels,
+                              float* lf_quant, JxgFrameDesc* desc) {
+  if (!parsed) return JXG_ERR_ARGUMENT;
+  if (!format_bpp(output_format)) return set_error(JXG_ERR_ARGUMENT, "unknown output format");
+  const jxg::ModularFrameState* ms = static_cast<const jxg::ModularFrameState*>(parsed);
+  if (xyb_encoded) *xyb_encoded = ms->xyb ? 1 : 0;
+  if (colour_channels) *colour_channels = ms->num_color_channels;
+  if (!ms->xyb) return JXG_OK;
+  if (lf_quant) memcpy(lf_quant, ms->lf_quant, sizeof(ms->lf_quant));
+  if (desc) {
+    memset(desc, 0, sizeof(*desc));
+    desc->abi_version = JXG_ABI_VERSION;
+    desc->width = ms->header.xsize();
+    desc->height = ms->header.ysize();
+    jxg::fill_output_colour(ms->file, output_format, desc);
+  }
+  return JXG_OK;
 }
 
 int jxg_modular_batch_add_lf(void* bp, void* parsed, uint32_t output_format, void* out, size_t out_row_stride,
@@ -844,14 +914,14 @@ int jxg_modular_batch_run(void* bp, void* cuda_stream) {
                                               std::to_string(b->lz_window_elems * 4) + " bytes)");
   }
   for (MFrame& f : b->frames) {
-    MJobDev& j = f.lf ? b->lf_store_jobs[f.store_index] : b->store_jobs[f.store_index];
+    MJobDev& j = store_job(b, f);
     j.out = f.out_is_device ? f.out : static_cast<uint8_t*>(cx->d_out.p) + f.dev_out_off;
     j.out_stride = f.out_is_device ? f.out_stride : f.out_row_bytes;
   }
   if (int r = batch_status(*b, b->streams.size())) return r;
   std::vector<MJobDev> all_jobs;  // the launch order of launch_all
   for (auto& l : b->levels) all_jobs.insert(all_jobs.end(), l.begin(), l.end());
-  for (const auto* l : {&b->store_jobs, &b->lf_dequant_jobs, &b->lf_smooth_jobs, &b->lf_store_jobs})
+  for (const auto* l : {&b->store_jobs, &b->xyb_store_jobs, &b->lf_dequant_jobs, &b->lf_smooth_jobs, &b->lf_store_jobs})
     all_jobs.insert(all_jobs.end(), l->begin(), l->end());
   PinnedArena& blob = cx->blob;
   if (!batch_table(blob, b->streams, b->tab.streams) || !batch_table(blob, b->order, b->tab.order) ||
@@ -891,14 +961,14 @@ int jxg_modular_batch_wait(void* bp, uint32_t* bad_frame, uint32_t* bad_group) {
   return batch_first_failure(*b, b->streams, "Modular group stream failed: frame ", bad_frame, bad_group);
 }
 
-// Parity tap: the final colour planes (3 x H x W i32, before the u8 conversion) of frame f.
+// Parity tap: the final colour planes (3 x H x W i32, before the u8 conversion; Y, X, B of an XYB frame) of frame f.
 int jxg_modular_batch_read_planes(void* bp, uint32_t f, int32_t* out, size_t out_len) {
   ModularBatch* b = static_cast<ModularBatch*>(bp);
   if (!b || !b->uploaded || f >= b->frames.size() || !out) return JXG_ERR_ARGUMENT;
   if (b->frames[f].region) return set_error(JXG_ERR_ARGUMENT, "read_planes: a region frame holds no whole planes");
   if (b->frames[f].lf) return set_error(JXG_ERR_ARGUMENT, "read_planes: a thumbnail holds no Modular colour planes");
   if (int r = batch_wait_last_run(*b)) return r;
-  const MJobDev& j = b->store_jobs[b->frames[f].store_index];  // a whole frame: the planes are whole, rows of width w
+  const MJobDev& j = store_job(b, b->frames[f]);  // a whole frame: the planes are whole, rows of width w
   const size_t n = size_t(j.w) * j.h;
   if (out_len < 3 * n) return set_error(JXG_ERR_ARGUMENT, "plane buffer too small");
   const int32_t* planes = static_cast<const int32_t*>(b->ctx->d_planes_a.p);

@@ -945,27 +945,44 @@ __global__ void __launch_bounds__(256) k_lf_smooth(const MJobDev* jobs, int32_t*
   }
 }
 
-// LF image X, Y, B at a -> the thumbnail: the output stage of the full decode's store (output_stage.h), the u8 dither at
-// the coded LF coordinate, then the orientation (op); XYB_F32_PLANAR writes the planes in the coded orientation,
-// plane c from row c * h. Rows grid-strided over the CTAs, columns over the threads.
-__global__ void __launch_bounds__(256) k_lf_store(const MJobDev* jobs, int32_t* planes, const uint8_t* blob) {
+// XYB samples -> an output through the output stage of the full decode's store (output_stage.h): the u8 dither at the
+// coded coordinate of the w x h image, then the orientation (op); the coded window [x0, x1) x [y0, y1) goes to the
+// output whose top-left pixel is display pixel (out_x, out_y). XYB_F32_PLANAR writes the window's planes in the coded
+// orientation, plane c from row c * (y1 - y0). Rows grid-strided over the CTAs, columns over the threads. The input:
+// * kModularXyb false (kJobLfStore, a thumbnail): the f32 planes X, Y, B at a, a + sa * h, a + 2 * sa * h;
+// * kModularXyb true (kJobXybStore, an XYB Modular frame): the i32 channels Y at a, X at b, B at c (strides sa, sb,
+//   sc), converted as ConvertModularXYBToF32Stage (render/stages/convert.rs:278-343) does with the LfQuantFactors in
+//   p.lf_factors: X = x s_x, Y = y s_y, B = (b + y) s_b, each operation on f32 and correctly rounded.
+template <bool kModularXyb>
+__global__ void __launch_bounds__(256) k_xyb_store(const MJobDev* jobs, const int32_t* planes, const uint8_t* blob) {
   const MJobDev j = jobs[blockIdx.y];
   const MLfFrameDev& p = *reinterpret_cast<const MLfFrameDev*>(blob + j.params);
   const size_t plane = size_t(j.sa) * j.h;
-  const float* in = reinterpret_cast<const float*>(planes + j.a);
   uint8_t* const out = static_cast<uint8_t*>(j.out);
-  for (uint32_t y = blockIdx.x; y < j.h; y += gridDim.x) {
-    for (uint32_t x = threadIdx.x; x < j.w; x += blockDim.x) {
-      const size_t i = size_t(y) * j.sa + x;
+  for (uint32_t y = j.y0 + blockIdx.x; y < j.y1; y += gridDim.x) {
+    for (uint32_t x = j.x0 + threadIdx.x; x < j.x1; x += blockDim.x) {
+      float xyb[3];
+      if (kModularXyb) {
+        const float qy = float(planes[j.a + int64_t(y) * j.sa + x]), qx = float(planes[j.b + int64_t(y) * j.sb + x]),
+                    qb = float(planes[j.c + int64_t(y) * j.sc + x]);
+        xyb[0] = __fmul_rn(qx, p.lf_factors[0]);
+        xyb[1] = __fmul_rn(qy, p.lf_factors[1]);
+        xyb[2] = __fmul_rn(__fadd_rn(qb, qy), p.lf_factors[2]);
+      } else {
+        const float* in = reinterpret_cast<const float*>(planes + j.a) + size_t(y) * j.sa + x;
+        for (int c = 0; c < 3; c++) xyb[c] = in[c * plane];
+      }
       if (p.output_format == JXG_FORMAT_XYB_F32_PLANAR) {
-        for (int c = 0; c < 3; c++) reinterpret_cast<float*>(out + (size_t(c) * j.h + y) * j.out_stride)[x] = in[c * plane + i];
+        for (int c = 0; c < 3; c++)
+          reinterpret_cast<float*>(out + (size_t(c) * (j.y1 - j.y0) + (y - j.y0)) * j.out_stride)[x - j.x0] = xyb[c];
         continue;
       }
       float v[3];
-      xyb_to_output(p, in[i], in[plane + i], in[2 * plane + i], v);
+      xyb_to_output(p, xyb[0], xyb[1], xyb[2], v);
       uint32_t dx, dy;
       display_pixel(j.op, j.w, j.h, x, y, dx, dy);
-      uint8_t* const row = out + size_t(dy) * j.out_stride;
+      dx -= j.out_x;
+      uint8_t* const row = out + size_t(dy - j.out_y) * j.out_stride;
       switch (p.output_format) {
         case JXG_FORMAT_RGB_F32:
           for (int c = 0; c < 3; c++) reinterpret_cast<float*>(row)[size_t(dx) * 3 + c] = v[c];
@@ -1002,7 +1019,9 @@ void launch_modular_jobs(int kind, const MJobDev* jobs, uint32_t num_jobs, uint3
   } else if (kind == 6) {
     k_lf_smooth<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes, blob);
   } else if (kind == 7) {
-    k_lf_store<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes, blob);
+    k_xyb_store<false><<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes, blob);
+  } else if (kind == 8) {
+    k_xyb_store<true><<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes, blob);
   } else {
     k_modular_store<<<dim3(rows, num_jobs), 256, 0, stream>>>(jobs, planes);
   }

@@ -115,13 +115,7 @@ void decode_lf_global(FrameState& fs, BitReader& br) {
   // features/noise.rs:14 + render/stages/noise.rs: noise synthesis is not rendered by this path, and dropping it would
   // silently differ from the reference's pixels, so the frame is refused.
   if (h.has_noise()) fail("noise synthesis is outside the hot-path scope", kErrUnsupported);
-  // LfQuantFactors (quantizer.rs:28-52)
-  if (!br.read_bool()) {
-    for (float& q : fs.lf_quant) {
-      q = read_f16(br) / 128.0f;
-      if (q < 1e-8f) fail("LF quant factor too small");
-    }
-  }
+  read_lf_quant_factors(br, fs.lf_quant);
   // QuantizerParams (quantizer.rs:60-77)
   switch (br.read(2)) {
     case 0: fs.global_scale = uint32_t(br.read(11)) + 1; break;
@@ -879,6 +873,10 @@ void FrameState::fill_desc(JxgFrameDesc* d, uint32_t output_format) {
   d->epf_pass0_sigma_scale = rf.epf_pass0_sigma_scale;
   d->epf_pass2_sigma_scale = rf.epf_pass2_sigma_scale;
   d->epf_border_sad_mul = rf.epf_border_sad_mul;
+  fill_output_colour(file, output_format, d);
+}
+
+void fill_output_colour(const FileHeader& file, uint32_t output_format, JxgFrameDesc* d) {
   memcpy(d->opsin_biases, file.opsin.opsin_biases, sizeof(d->opsin_biases));
   d->intensity_target = file.intensity_target;
   d->output_format = output_format;

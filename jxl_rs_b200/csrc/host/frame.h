@@ -123,6 +123,10 @@ void lf_smoothing_factors(const FrameState& fs, float out[3]);
 // frame/adaptive_lf_smoothing.rs:44 on fs.lf (uses xb, yb, global_scale, quant_lf, lf_quant). Exposed for the tests.
 void adaptive_lf_smoothing(FrameState& fs, int threads = 1);
 
+// The output-stage fields of a JxgFrameDesc for an XYB image (opsin biases and re-targeted matrix, intensity target,
+// transfer function, luminances) and its output_format / orientation; the other fields are left as they are.
+void fill_output_colour(const FileHeader& file, uint32_t output_format, JxgFrameDesc* d);
+
 // JxgImageInfo of a parsed frame (jxg_parse_file, jxg_lf_parse_file, jxg_modular_parse_file): sizes, orientation,
 // groups, passes, encoding and the HF section bytes `hf_bytes`.
 void fill_image_info(const FileHeader& file, const FrameHeader& h, uint64_t hf_bytes, JxgImageInfo* info);

@@ -158,6 +158,18 @@ float read_f16(BitReader& br) {
   return v;
 }
 
+void read_lf_quant_factors(BitReader& br, float out[3]) {
+  static const float kDefault[3] = {1.0f / 4096.0f, 1.0f / 512.0f, 1.0f / 256.0f};
+  if (br.read_bool()) {
+    for (int c = 0; c < 3; c++) out[c] = kDefault[c];
+    return;
+  }
+  for (int c = 0; c < 3; c++) {
+    out[c] = read_f16(br) / 128.0f;
+    if (out[c] < 1e-8f) fail("LF quant factor too small");
+  }
+}
+
 uint64_t read_u64(BitReader& br) {  // encodings.rs:111-139
   switch (br.read(2)) {
     case 0: return 0;

@@ -197,6 +197,8 @@ OutputColour resolve_output_colour(const FileHeader& fh);
 
 float f16_bits_to_float(uint16_t h);
 float read_f16(BitReader& br);  // encodings.rs:59-74 (rejects NaN/Inf)
+// LfQuantFactors of LfGlobal (quantizer.rs:28-52): the defaults (quant_weights::LF_QUANT), or three f16 values / 128.
+void read_lf_quant_factors(BitReader& br, float out[3]);
 uint64_t read_u64(BitReader& br);
 void read_extensions(BitReader& br);
 

@@ -51,8 +51,7 @@ void decode_lf_global_modular(ModularFrameState& ms, BitReader& br) {
   if (h.has_patches()) fail("patches are outside the hot-path scope", kErrUnsupported);
   if (h.has_splines()) fail("splines are outside the hot-path scope", kErrUnsupported);
   if (h.has_noise()) fail("noise synthesis is outside the hot-path scope", kErrUnsupported);
-  if (!br.read_bool())  // LfQuantFactors (quantizer.rs:28-52): present but unused by Modular frames
-    for (int i = 0; i < 3; i++) read_f16(br);
+  read_lf_quant_factors(br, ms.lf_quant);  // used by XYB frames only
   if (br.read_bool()) {
     size_t limit = std::min<size_t>(1024 + size_t(h.width) * h.height * ms.num_color_channels / 16, size_t(1) << 22);
     ms.global_tree = ModularTree::read(br, limit);
@@ -240,7 +239,7 @@ std::unique_ptr<ModularFrameState> parse_modular_file(const uint8_t* data, size_
   FrameHeader& h = ms.header;
   if (h.encoding != 1) fail("not a Modular frame", kErrUnsupported);
   if (h.frame_type != 0) fail("only regular frames are in scope", kErrUnsupported);
-  if (ms.file.xyb_encoded) fail("XYB Modular frames (lossy Modular) are outside the scope", kErrUnsupported);
+  ms.xyb = ms.file.xyb_encoded;
   if (h.do_ycbcr) fail("YCbCr Modular frames are outside the scope", kErrUnsupported);
   if (h.num_extra_channels) fail("extra channels are outside the hot-path scope", kErrUnsupported);
   if (h.upsampling != 1) fail("upsampling is outside the hot-path scope", kErrUnsupported);
@@ -248,9 +247,15 @@ std::unique_ptr<ModularFrameState> parse_modular_file(const uint8_t* data, size_
   if (h.have_crop || h.blending.mode != 0) fail("cropped/blended frames are outside the hot-path scope", kErrUnsupported);
   if (h.passes.num_passes != 1) fail("multi-pass Modular frames are outside the scope", kErrUnsupported);
   check_single_still_frame(ms.file, h);
-  if (ms.file.bit_depth.floating_point || ms.file.bit_depth.bits_per_sample != 8)
+  if (ms.xyb) {
+    // The reference filters a Modular XYB frame with a constant EPF sigma of its own; the device path has no such stage.
+    if (h.rf.gab || h.rf.epf_iters > 0) fail("XYB Modular frames with Gaborish or EPF are outside the scope", kErrUnsupported);
+    resolve_output_colour(ms.file);  // refuses the colour encodings the output stage cannot reproduce
+  } else if (ms.file.bit_depth.floating_point || ms.file.bit_depth.bits_per_sample != 8) {
     fail("only 8-bit integer samples are in scope", kErrUnsupported);
-  ms.num_color_channels = ms.file.color_encoding.color_space == ColorSpace::Gray ? 1 : 3;
+  }
+  // frame/decode.rs:167-170: an XYB frame codes three colour channels whatever the colour encoding
+  ms.num_color_channels = !ms.xyb && ms.file.color_encoding.color_space == ColorSpace::Gray ? 1 : 3;
   ms.toc = read_toc(br, h.num_toc_entries());
   ms.sections_base = br.byte_pos();
   const uint8_t* base = ms.codestream.data() + ms.sections_base;

@@ -51,6 +51,7 @@ enum ModularJobKind : uint32_t {
   kJobLfDequant = 5,  // quantised Y, X, B (i32) of one LF group's rectangle -> dequantised X, Y, B (f32)
   kJobLfSmooth = 6,   // adaptive LF smoothing, X, Y, B at a -> c (out of place)
   kJobLfStore = 7,    // X, Y, B planes -> the thumbnail output
+  kJobXybStore = 8,   // final Y, X, B channels of an XYB frame -> XYB floats -> the output (device job only)
 };
 struct ModularStep {
   ModularJobKind kind = kJobRct;
@@ -70,7 +71,11 @@ struct ModularFrameState {
   ModularTree global_tree;
   GroupHeader global_header;
   uint32_t nb_meta = 0;
-  uint32_t num_color_channels = 3;
+  uint32_t num_color_channels = 3;  // coded colour channels: 3 for an XYB frame, also of a grey image
+  // An XYB frame (lossy Modular, file.xyb_encoded): its colour channels are quantised Y, X, B, converted to XYB floats
+  // with the LfQuantFactors (render/stages/convert.rs ConvertModularXYBToF32Stage) and stored through the output stage.
+  bool xyb = false;
+  float lf_quant[3] = {0.0f, 0.0f, 0.0f};
   std::vector<ModularChannel> coded;   // channel list after the global meta-apply, full-size planes
   std::vector<uint8_t> host_decoded;   // per coded channel: 1 = filled by the host (section 0 / ModularLF)
   std::vector<ModularGroupStream> hf;  // one per group (single pass)

@@ -570,6 +570,18 @@ class ModularParsedFrame:
     def height(self):
         return self.info.height
 
+    def colour(self, output_format=abi.FORMAT_RGB_U8):
+        """jxg_modular_parsed_colour: {"xyb": bool, "colour_channels": coded colour channels, "lf_quant": the
+        LfQuantFactors (X, Y, B) of an XYB frame, "desc": the JxgFrameDesc with the output stage a batch applies for
+        `output_format`} (lf_quant and desc are None for a lossless frame)."""
+        xyb, nc = C.c_int(), C.c_uint32()
+        q = (C.c_float * 3)()
+        d = abi.JxgFrameDesc()
+        abi.check(self._lib, self._lib.jxg_modular_parsed_colour(self._h, output_format, C.byref(xyb), C.byref(nc), q,
+                                                                 C.byref(d)))
+        return {"xyb": bool(xyb.value), "colour_channels": nc.value, "lf_quant": tuple(q) if xyb.value else None,
+                "desc": d if xyb.value else None}
+
     def region_plan(self, region):
         """The dependency cone of a region (x, y, w, h in output coordinates; jxg_modular_parsed_region_plan), no device
         needed: (groups, arena, need) with groups the whole-frame indices of the group streams decoded, and per buffer
@@ -635,11 +647,17 @@ class ModularBatch(_BatchHandle):
         abi.check(self._lib, self._lib.jxg_modular_batch_set_lanes(self._h, lanes_per_warp))
         self.frames = []
 
-    def add(self, frame: ModularParsedFrame, out_ptr: int, row_stride: int, out_is_device: bool, region=None):
+    def add(self, frame: ModularParsedFrame, out_ptr: int, row_stride: int, out_is_device: bool, region=None, fmt=None):
         """region: None for the whole frame, or (x, y, w, h) in output coordinates: only what that rectangle depends on
-        is decoded, and only it is stored, into a buffer of h rows of w pixels (jxg_modular_batch_add_region)."""
+        is decoded, and only it is stored, into a buffer of h rows of w pixels (jxg_modular_batch_add_region).
+        fmt: None (RGB u8), or a FORMAT_* of abi (jxg_modular_batch_add_output): any format for an XYB frame, RGB_U8
+        for a lossless one."""
         dev = 1 if out_is_device else 0
-        if region is None:
+        if fmt is not None:
+            reg = None if region is None else C.byref(_region(region))
+            abi.check(self._lib, self._lib.jxg_modular_batch_add_output(self._h, frame._h, fmt, reg, C.c_void_p(out_ptr),
+                                                                        row_stride, dev))
+        elif region is None:
             abi.check(self._lib, self._lib.jxg_modular_batch_add(self._h, frame._h, C.c_void_p(out_ptr), row_stride, dev))
         else:
             abi.check(self._lib, self._lib.jxg_modular_batch_add_region(self._h, frame._h, C.byref(_region(region)),
@@ -694,20 +712,26 @@ class ModularBatch(_BatchHandle):
         return out
 
 
-def decode_modular_files(ctx: JxgContext, files, to_host: bool = True, lanes_per_warp: int = 1):
-    """Decodes a list of Modular .jxl byte strings on the GPU; returns H x W x 3 uint8 torch tensors."""
+def decode_modular_files(ctx: JxgContext, files, to_host: bool = True, lanes_per_warp: int = 1,
+                         pixel_format: JxlPixelFormat = JxlPixelFormat()):
+    """Decodes a list of Modular .jxl byte strings on the GPU; returns H x W x C torch tensors of the display-oriented
+    images in `pixel_format`. Lossless frames take the default RGB U8 only; XYB (lossy) frames take every format."""
     import torch
+    fmt = pixel_format.abi_format()
+    ch = 4 if fmt == abi.FORMAT_RGBA_U8 else 3
+    dt = {abi.FORMAT_RGB_F32: torch.float32, abi.FORMAT_RGB_U16: torch.uint16, abi.FORMAT_RGB_F16: torch.float16}.get(fmt, torch.uint8)
     frames = [ModularParsedFrame(f) for f in files]
     batch = ModularBatch(ctx, lanes_per_warp)
     outs = []
     try:
         for fr in frames:
             if to_host:
-                t = torch.empty((fr.height, fr.width, 3), dtype=torch.uint8).pin_memory()
+                t = torch.empty((fr.height, fr.width, ch), dtype=dt).pin_memory()
             else:
-                t = torch.empty((fr.height, fr.width, 3), dtype=torch.uint8, device=f"cuda:{ctx.device}")
+                t = torch.empty((fr.height, fr.width, ch), dtype=dt, device=f"cuda:{ctx.device}")
             outs.append(t)
-            batch.add(fr, t.data_ptr(), fr.width * 3, not to_host)
+            batch.add(fr, t.data_ptr(), fr.width * ch * t.element_size(), not to_host,
+                      fmt=None if fmt == abi.FORMAT_RGB_U8 else fmt)
         batch.run()
         batch.wait()
     finally:

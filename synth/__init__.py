@@ -37,6 +37,11 @@ def _lib():
         _LIB.jxs_encode_modular_lz77.restype = C.c_int64
         _LIB.jxs_encode_modular_lz77.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
                                                  C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t]
+        _LIB.jxs_encode_modular_xyb.restype = C.c_int64
+        _LIB.jxs_encode_modular_xyb.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
+                                                C.c_size_t]
+        _LIB.jxs_modular_xyb_source.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         _LIB.jxs_modular_lz77_census.argtypes = [C.c_void_p]
         _LIB.jxs_modular_lz77_census.restype = None
         _LIB.jxs_encode_vardct_tokens.restype = C.c_int64
@@ -202,7 +207,18 @@ def modular_source(width, height, seed, palette=0):
     return out
 
 
-def encode_modular(width, height, seed, rct=6, squeeze=0, tree_kind=1, source=None, palette=0, lz77=0) -> bytes:
+def modular_xyb_source(width, height, seed, lf_quant=None):
+    """The coded channels Y, X, B ((3, H, W) int32 numpy array) of encode_modular(..., xyb={"lf_quant": lf_quant}) for
+    `seed`: what any correct decoder holds before the conversion to XYB floats."""
+    import numpy as np
+    out = np.zeros((3, height, width), np.int32)
+    qa = None if lf_quant is None else (C.c_float * 3)(*lf_quant)
+    if _lib().jxs_modular_xyb_source(width, height, seed, qa, out.ctypes.data) != 0:
+        raise RuntimeError("synthetic XYB source failed: " + _lib().jxs_modular_last_error().decode())
+    return out
+
+
+def encode_modular(width, height, seed, rct=6, squeeze=0, tree_kind=1, source=None, palette=0, lz77=0, xyb=None) -> bytes:
     """One synthetic lossless Modular frame (8-bit RGB, group size 256). rct: 0 or 6 (YCoCg); squeeze: default
     Squeeze transform on/off; tree_kind: 0 single Gradient leaf, 1 property tree, 2 weighted-predictor tree,
     3 tree on properties of the previous channel (17, 19); palette: 1 = global palette transform over the colour
@@ -210,7 +226,13 @@ def encode_modular(width, height, seed, rct=6, squeeze=0, tree_kind=1, source=No
     source: optional H x W x 3 uint8 array to encode instead of the procedural image.
     lz77: 0 no LZ77; 1 run-length copies in the group streams (every copy at distance 1, the shape libjxl's fastest
     lossless mode writes); 2 general copies (special distances relative to the stream's widest channel, plain
-    distances, copies across row ends and channels, copies the decoder clamps). lz77_census() describes the copies."""
+    distances, copies across row ends and channels, copies the decoder clamps). lz77_census() describes the copies.
+    xyb: None (lossless RGB), or a dict for an XYB-encoded (lossy) frame: the procedural picture of `seed` in XYB,
+    quantised to the Y, X, B channels the decoder turns back into X = x s_x, Y = y s_y, B = (b + y) s_b. Keys, all
+    optional: "lf_quant" (the three LfQuantFactors as written, f16-exact values, the factors times 128; absent: the
+    default factors), "colour" (0..7, the colour encodings of encode_synthetic, 6 grey), "orientation" (1..8), "gab"
+    (0/1) and "epf_iters" (0..3) (the restoration filter flags; the decoder refuses XYB frames with either). source,
+    palette and lz77 must be unset."""
     lib = _lib()
     src = None
     if source is not None:
@@ -221,7 +243,17 @@ def encode_modular(width, height, seed, rct=6, squeeze=0, tree_kind=1, source=No
     cap = max(1 << 16, width * height * 4)
     buf = C.create_string_buffer(cap)
 
+    if xyb is not None:
+        if source is not None or palette or lz77:
+            raise ValueError("the XYB mode takes no source, palette or lz77")
+        q = xyb.get("lf_quant")
+        qa = None if q is None else (C.c_float * 3)(*q)
+        args = (width, height, seed, rct, squeeze, tree_kind, qa, xyb.get("colour", 0), xyb.get("orientation", 1),
+                xyb.get("gab", 0), xyb.get("epf_iters", 0))
+
     def run(buf, cap):
+        if xyb is not None:
+            return lib.jxs_encode_modular_xyb(*args, buf, cap)
         if lz77:
             return lib.jxs_encode_modular_lz77(width, height, seed, rct, squeeze, tree_kind, palette, lz77, src, buf, cap)
         return lib.jxs_encode_modular_ex(width, height, seed, rct, squeeze, tree_kind, palette, src, buf, cap)

@@ -203,6 +203,89 @@ static void make_image(const Params& p, std::vector<float> (&rgb)[3]) {
     }
 }
 
+// ImageMetadata of an XYB-encoded image with 8-bit integer samples (headers/image_metadata.rs:197-236): orientation
+// 1..8 and the colour encoding variant `colour` (see Params::colour). Shared with the Modular writer's XYB mode.
+void write_xyb_image_metadata(BitWriter& out, uint32_t orientation, uint32_t colour) {
+  if (orientation == 1 && colour == 0) {
+    out.write(1, 1);  // ImageMetadata all_default
+  } else {  // headers/image_metadata.rs:197-236
+    auto write_enum = [&](uint32_t v) {  // jxl_macros default enum coder: u2S(0, 1, Bits(4) + 2, Bits(6) + 18)
+      if (v == 0) out.u2s_sel(0);
+      else if (v == 1) out.u2s_sel(1);
+      else if (v < 18) out.u2s_sel(2, v - 2, 4);
+      else out.u2s_sel(3, v - 18, 6);
+    };
+    auto write_f16 = [&](float v) {  // exactly representable positive values only (headers/encodings.rs:59-74)
+      int e = 0;
+      float m = std::frexp(v, &e);  // v = m * 2^e, m in [0.5, 1)
+      const uint32_t mant = uint32_t(std::lround((m * 2.0f - 1.0f) * 1024.0f));
+      out.write(v == 0.0f ? 0u : (uint32_t(e - 1 + 15) << 10) | mant, 16);
+    };
+    auto write_xy = [&](double x, double y) {  // CustomXY: pack_signed(round(v * 1e6)) through u2S (color_encoding.rs:91-100)
+      for (double v : {x, y}) {
+        const uint32_t u = pack_signed(int32_t(std::lround(v * 1e6)));
+        if (u < (1u << 19)) out.u2s_sel(0, u, 19);
+        else if (u < 524288u + (1u << 19)) out.u2s_sel(1, u - 524288u, 19);
+        else if (u < 1048576u + (1u << 20)) out.u2s_sel(2, u - 1048576u, 20);
+        else out.u2s_sel(3, u - 2097152u, 21);
+      }
+    };
+    out.write(0, 1);                    // all_default
+    out.write(1, 1);                    // extra_fields
+    out.write(orientation - 1, 3);
+    out.write(0, 1);                    // have_intrinsic_size
+    out.write(0, 1);                    // have_preview
+    out.write(0, 1);                    // have_animation
+    out.write(0, 1);                    // BitDepth: integer samples
+    out.u2s_sel(0);                     //           8 bits
+    out.write(1, 1);                    // modular_16bit_sufficient
+    out.u2s_sel(0);                     // no extra channels
+    out.write(1, 1);                    // xyb_encoded
+    bool hdr = false;
+    if (colour == 0) {
+      out.write(1, 1);                  // ColorEncoding all_default
+    } else {  // headers/color_encoding.rs:166-196
+      out.write(0, 1);
+      out.write(0, 1);                  // want_icc
+      write_enum(colour == 6 ? 1 : 0);  // colour space RGB / Gray
+      uint32_t wp = 1, prim = 1, tf = 13;  // D65, sRGB primaries, sRGB curve
+      bool gamma = false;
+      switch (colour) {
+        case 1: tf = 8; break;
+        case 2: gamma = true; break;
+        case 3: prim = 11; tf = 16; hdr = true; break;
+        case 4: prim = 9; tf = 18; hdr = true; break;
+        case 5: wp = 11; prim = 2; tf = 1; break;
+        case 6: break;
+        default: wp = 10; tf = 17; break;
+      }
+      write_enum(wp);
+      if (colour != 6) {
+        write_enum(prim);
+        if (prim == 2) {
+          write_xy(0.66, 0.31);
+          write_xy(0.28, 0.62);
+          write_xy(0.14, 0.07);
+        }
+      }
+      out.write(gamma ? 1 : 0, 1);      // have_gamma
+      if (gamma) out.write(4545455, 24);
+      else write_enum(tf);
+      write_enum(1);                    // rendering intent: relative
+    }
+    if (hdr) {  // ToneMapping (image_metadata.rs:156-167)
+      out.write(0, 1);
+      write_f16(1000.0f);               // intensity_target
+      write_f16(0.0f);                  // min_nits
+      out.write(0, 1);                  // relative_to_max_display
+      write_f16(0.0f);                  // linear_below
+    } else {
+      out.write(1, 1);                  // ToneMapping all_default
+    }
+    out.write_u64(0);                   // extensions
+  }
+}
+
 // inverse of render/stages/xyb.rs:197-241 with the default opsin matrix
 static void to_xyb(std::vector<float> (&rgb)[3], const jxg::OpsinInverseMatrix& op) {
   double m[9], inv[9];
@@ -1066,84 +1149,7 @@ std::vector<uint8_t> encode(const Params& p) {
   write_dim(H);
   out.write(0, 3);  // ratio 0: explicit xsize
   write_dim(W);
-  if (p.orientation == 1 && p.colour == 0) {
-    out.write(1, 1);  // ImageMetadata all_default
-  } else {  // headers/image_metadata.rs:197-236
-    auto write_enum = [&](uint32_t v) {  // jxl_macros default enum coder: u2S(0, 1, Bits(4) + 2, Bits(6) + 18)
-      if (v == 0) out.u2s_sel(0);
-      else if (v == 1) out.u2s_sel(1);
-      else if (v < 18) out.u2s_sel(2, v - 2, 4);
-      else out.u2s_sel(3, v - 18, 6);
-    };
-    auto write_f16 = [&](float v) {  // exactly representable positive values only (headers/encodings.rs:59-74)
-      int e = 0;
-      float m = std::frexp(v, &e);  // v = m * 2^e, m in [0.5, 1)
-      const uint32_t mant = uint32_t(std::lround((m * 2.0f - 1.0f) * 1024.0f));
-      out.write(v == 0.0f ? 0u : (uint32_t(e - 1 + 15) << 10) | mant, 16);
-    };
-    auto write_xy = [&](double x, double y) {  // CustomXY: pack_signed(round(v * 1e6)) through u2S (color_encoding.rs:91-100)
-      for (double v : {x, y}) {
-        const uint32_t u = pack_signed(int32_t(std::lround(v * 1e6)));
-        if (u < (1u << 19)) out.u2s_sel(0, u, 19);
-        else if (u < 524288u + (1u << 19)) out.u2s_sel(1, u - 524288u, 19);
-        else if (u < 1048576u + (1u << 20)) out.u2s_sel(2, u - 1048576u, 20);
-        else out.u2s_sel(3, u - 2097152u, 21);
-      }
-    };
-    out.write(0, 1);                    // all_default
-    out.write(1, 1);                    // extra_fields
-    out.write(p.orientation - 1, 3);
-    out.write(0, 1);                    // have_intrinsic_size
-    out.write(0, 1);                    // have_preview
-    out.write(0, 1);                    // have_animation
-    out.write(0, 1);                    // BitDepth: integer samples
-    out.u2s_sel(0);                     //           8 bits
-    out.write(1, 1);                    // modular_16bit_sufficient
-    out.u2s_sel(0);                     // no extra channels
-    out.write(1, 1);                    // xyb_encoded
-    bool hdr = false;
-    if (p.colour == 0) {
-      out.write(1, 1);                  // ColorEncoding all_default
-    } else {  // headers/color_encoding.rs:166-196
-      out.write(0, 1);
-      out.write(0, 1);                  // want_icc
-      write_enum(p.colour == 6 ? 1 : 0);  // colour space RGB / Gray
-      uint32_t wp = 1, prim = 1, tf = 13;  // D65, sRGB primaries, sRGB curve
-      bool gamma = false;
-      switch (p.colour) {
-        case 1: tf = 8; break;
-        case 2: gamma = true; break;
-        case 3: prim = 11; tf = 16; hdr = true; break;
-        case 4: prim = 9; tf = 18; hdr = true; break;
-        case 5: wp = 11; prim = 2; tf = 1; break;
-        case 6: break;
-        default: wp = 10; tf = 17; break;
-      }
-      write_enum(wp);
-      if (p.colour != 6) {
-        write_enum(prim);
-        if (prim == 2) {
-          write_xy(0.66, 0.31);
-          write_xy(0.28, 0.62);
-          write_xy(0.14, 0.07);
-        }
-      }
-      out.write(gamma ? 1 : 0, 1);      // have_gamma
-      if (gamma) out.write(4545455, 24);
-      else write_enum(tf);
-      write_enum(1);                    // rendering intent: relative
-    }
-    if (hdr) {  // ToneMapping (image_metadata.rs:156-167)
-      out.write(0, 1);
-      write_f16(1000.0f);               // intensity_target
-      write_f16(0.0f);                  // min_nits
-      out.write(0, 1);                  // relative_to_max_display
-      write_f16(0.0f);                  // linear_below
-    } else {
-      out.write(1, 1);                  // ToneMapping all_default
-    }
-    out.write_u64(0);                   // extensions
-  }
+  write_xyb_image_metadata(out, p.orientation, p.colour);
   write_custom_transform_data(out, hd);
   out.zero_pad_to_byte();
   // FrameHeader (frame_header.rs:267-444)
@@ -1598,6 +1604,13 @@ void make_image_u8(uint32_t width, uint32_t height, uint64_t seed, std::vector<u
   rgb.resize(size_t(width) * height * 3);
   for (size_t i = 0; i < size_t(width) * height; i++)
     for (int c = 0; c < 3; c++) rgb[i * 3 + c] = uint8_t(std::lround(std::min(1.0f, std::max(0.0f, img[c][i])) * 255.0f));
+}
+
+// The procedural picture of `seed` as XYB planes (X, Y, B; the default opsin matrix), as the VarDCT writer codes it.
+void make_xyb_image(uint32_t width, uint32_t height, uint64_t seed, std::vector<float> (&xyb)[3]) {
+  Params p{width, height, seed, 1.0f, 0, 0, 0, 0, 0};
+  make_image(p, xyb);
+  to_xyb(xyb, jxg::OpsinInverseMatrix());
 }
 
 }  // namespace jxs

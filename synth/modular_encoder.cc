@@ -1,21 +1,34 @@
 // Synthetic *Modular* (lossless, 8-bit RGB) JPEG XL writer: test-data tooling for BASELINE config 5, like
-// encoder.cc is for the VarDCT configs (the reference has no encoder). It emits: non-XYB image metadata, a Modular
+// encoder.cc is for the VarDCT configs (the reference has no encoder). It emits: non-XYB image metadata (or, in the XYB
+// mode, XYB-encoded metadata and the procedural picture quantised to Y, X, B channels: a lossy Modular frame), a Modular
 // frame header (group size 256, no restoration filter), LfGlobal with a global MA tree + one clustered ANS code,
 // global transforms RCT (YCoCg) and/or Squeeze (default parameters), and one sub-bitstream per section following
 // the channel -> section rules of modular/mod.rs:353-400. Forward RCT / forward Squeeze are derived here from the
 // decoder definitions (rct.rs:9-40, squeeze.rs:144-195); the round trip "decode == source" is part of the tests.
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <deque>
 #include <stdexcept>
 #include <string>
 
+#include "../jxl_rs_b200/csrc/host/headers.h"
 #include "../jxl_rs_b200/csrc/host/modular.h"
 #include "entropy_writer.h"
 
 namespace jxs {
 
 void make_image_u8(uint32_t width, uint32_t height, uint64_t seed, std::vector<uint8_t>& rgb);
+void make_xyb_image(uint32_t width, uint32_t height, uint64_t seed, std::vector<float> (&xyb)[3]);
+void write_xyb_image_metadata(BitWriter& out, uint32_t orientation, uint32_t colour);
+
+// XYB mode of encode_modular. lf_quant_f16: the LfQuantFactors as written (f16 values, the factors times 128; all zero:
+// the default factors); colour / orientation: as the VarDCT writer's; gab / epf_iters: the restoration filter flags.
+struct ModularXyb {
+  bool on = false;
+  float lf_quant_f16[3] = {0.0f, 0.0f, 0.0f};
+  uint32_t colour = 0, orientation = 1, gab = 0, epf_iters = 0;
+};
 
 namespace {
 
@@ -440,11 +453,41 @@ void snap_to_palette_colours(uint32_t W, uint32_t H, std::vector<uint8_t>& rgb) 
       }
 }
 
+// f16 bits of a finite value that f16 represents exactly (headers/encodings.rs:59-74 reads it back unchanged).
+uint16_t f16_bits_exact(float v) {
+  if (v == 0.0f) return 0;
+  int e = 0;
+  const float m = std::frexp(std::fabs(v), &e);  // |v| = m * 2^e, m in [0.5, 1)
+  const float mant = (m * 2.0f - 1.0f) * 1024.0f;
+  if (e - 1 < -14 || e - 1 > 15 || mant != std::floor(mant)) throw std::runtime_error("value not exact in f16");
+  return uint16_t((v < 0 ? 0x8000u : 0u) | (uint32_t(e - 1 + 15) << 10) | uint32_t(mant));
+}
+
+// The XYB mode's coded colour channels Y, X, B: the procedural picture in XYB quantised so that the decoder's
+// X = x s_x, Y = y s_y, B = (b + y) s_b (render/stages/convert.rs:278-343) gives it back to within half a step.
+void xyb_channels(uint32_t W, uint32_t H, uint64_t seed, const ModularXyb& xyb, std::vector<ModularChannel>& ch) {
+  float lf_quant[3] = {1.0f / 4096.0f, 1.0f / 512.0f, 1.0f / 256.0f};  // quant_weights::LF_QUANT
+  if (xyb.lf_quant_f16[0] != 0.0f || xyb.lf_quant_f16[1] != 0.0f || xyb.lf_quant_f16[2] != 0.0f)
+    for (int c = 0; c < 3; c++) lf_quant[c] = jxg::f16_bits_to_float(f16_bits_exact(xyb.lf_quant_f16[c])) / 128.0f;
+  std::vector<float> img[3];
+  make_xyb_image(W, H, seed, img);
+  ch.clear();
+  for (int c = 0; c < 3; c++) ch.emplace_back(W, H, 0, 0);
+  for (size_t i = 0; i < size_t(W) * H; i++) {
+    const int32_t y = int32_t(std::lround(img[1][i] / lf_quant[1]));
+    ch[0].data[i] = y;
+    ch[1].data[i] = int32_t(std::lround(img[0][i] / lf_quant[0]));
+    ch[2].data[i] = int32_t(std::lround(img[2][i] / lf_quant[2])) - y;
+  }
+}
+
 std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint32_t rct_type, uint32_t squeeze,
-                                    uint32_t tree_kind, const uint8_t* source_rgb, uint32_t palette, uint32_t lz77) {
+                                    uint32_t tree_kind, const uint8_t* source_rgb, uint32_t palette, uint32_t lz77,
+                                    const ModularXyb& xyb = ModularXyb()) {
+  if (xyb.on && (source_rgb || palette)) throw std::runtime_error("the XYB mode takes no source image and no palette");
   std::vector<uint8_t> rgb;
   if (source_rgb) rgb.assign(source_rgb, source_rgb + size_t(W) * H * 3);
-  else make_image_u8(W, H, seed, rgb);
+  else if (!xyb.on) make_image_u8(W, H, seed, rgb);
   if (palette && !source_rgb) snap_to_palette_colours(W, H, rgb);
   const uint32_t group_dim = 256;
   const uint32_t xg = (W + group_dim - 1) / group_dim, yg = (H + group_dim - 1) / group_dim, num_groups = xg * yg;
@@ -453,9 +496,14 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
 
   // ---- channels + forward transforms ----
   std::vector<ModularChannel> ch;
-  for (int c = 0; c < 3; c++) {
-    ch.emplace_back(W, H, 0, 0);
-    for (size_t i = 0; i < size_t(W) * H; i++) ch[c].data[i] = rgb[i * 3 + c];
+  const bool custom_quant = xyb.lf_quant_f16[0] != 0.0f || xyb.lf_quant_f16[1] != 0.0f || xyb.lf_quant_f16[2] != 0.0f;
+  if (xyb.on) {
+    xyb_channels(W, H, seed, xyb, ch);
+  } else {
+    for (int c = 0; c < 3; c++) {
+      ch.emplace_back(W, H, 0, 0);
+      for (size_t i = 0; i < size_t(W) * H; i++) ch[c].data[i] = rgb[i * 3 + c];
+    }
   }
   jxg::GroupHeader gh;
   gh.use_global_tree = true;
@@ -635,7 +683,9 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
 
   // ---- sections ----
   BitWriter lf_global;
-  lf_global.write(1, 1);  // LfQuantFactors all_default
+  lf_global.write(custom_quant ? 0 : 1, 1);  // LfQuantFactors all_default
+  if (custom_quant)
+    for (int c = 0; c < 3; c++) lf_global.write(f16_bits_exact(xyb.lf_quant_f16[c]), 16);
   lf_global.write(1, 1);  // global tree present
   {
     std::vector<Token> tt;  // tree.rs:284-340: contexts 0 splitval, 1 property+1, 2 predictor, 3 offset, 4 mul_log, 5 mul_bits
@@ -690,15 +740,19 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
   out.write(0, 3);  // ratio 0
   write_dim(W);
   // ImageMetadata (image_metadata.rs:197-236)
-  out.write(0, 1);   // all_default
-  out.write(0, 1);   // extra_fields
-  out.write(0, 1);   // bit depth: integer samples
-  out.write(0, 2);   // 8 bits
-  out.write(1, 1);   // modular_16bit_buffers
-  out.write(0, 2);   // no extra channels
-  out.write(0, 1);   // xyb_encoded = false
-  out.write(1, 1);   // ColorEncoding all_default (sRGB)
-  out.write_u64(0);  // extensions
+  if (xyb.on) {
+    write_xyb_image_metadata(out, xyb.orientation, xyb.colour);
+  } else {
+    out.write(0, 1);   // all_default
+    out.write(0, 1);   // extra_fields
+    out.write(0, 1);   // bit depth: integer samples
+    out.write(0, 2);   // 8 bits
+    out.write(1, 1);   // modular_16bit_buffers
+    out.write(0, 2);   // no extra channels
+    out.write(0, 1);   // xyb_encoded = false
+    out.write(1, 1);   // ColorEncoding all_default (sRGB)
+    out.write_u64(0);  // extensions
+  }
   out.write(1, 1);   // CustomTransformData all_default
   out.zero_pad_to_byte();
   // FrameHeader (frame_header.rs:267-444)
@@ -706,7 +760,7 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
   out.write(0, 2);   // RegularFrame
   out.write(1, 1);   // Modular
   out.write_u64(0);  // flags
-  out.write(0, 1);   // do_ycbcr
+  if (!xyb.on) out.write(0, 1);  // do_ycbcr (absent for XYB images)
   out.write(0, 2);   // upsampling 1
   out.write(1, 2);   // group_size_shift 1 (256)
   out.write(0, 2);   // one pass
@@ -715,8 +769,14 @@ std::vector<uint8_t> encode_modular(uint32_t W, uint32_t H, uint64_t seed, uint3
   out.write(1, 1);   // is_last
   out.write(0, 2);   // name length 0
   out.write(0, 1);   // RestorationFilter all_default = 0
-  out.write(0, 1);   // gab off
-  out.write(0, 2);   // epf off
+  out.write(xyb.gab, 1);
+  if (xyb.gab) out.write(0, 1);  // default Gaborish weights
+  out.write(xyb.epf_iters, 2);
+  if (xyb.epf_iters) {  // frame_header.rs:185-227 for a Modular frame: default weights and sigmas, then the EPF sigma
+    out.write(0, 1);
+    out.write(0, 1);
+    out.write(f16_bits_exact(1.0f), 16);
+  }
   out.write_u64(0);  // restoration filter extensions
   out.write_u64(0);  // frame header extensions
   std::vector<std::vector<uint8_t>> sections;
@@ -1161,6 +1221,44 @@ void jxs_modular_lz77_census(uint64_t* out) {
 }
 
 // The token-level writer (encode_modular_tokens above): `words` is the flat frame description.
+// The coded channels Y, X, B (3 x height x width i32) of the XYB mode's frame of `seed` and factors q_f16.
+int jxs_modular_xyb_source(uint32_t width, uint32_t height, uint64_t seed, const float* q_f16, int32_t* out) {
+  try {
+    jxs::ModularXyb x;
+    for (int c = 0; c < 3; c++) x.lf_quant_f16[c] = q_f16 ? q_f16[c] : 0.0f;
+    std::vector<jxg::ModularChannel> ch;
+    jxs::xyb_channels(width, height, seed, x, ch);
+    for (int c = 0; c < 3; c++) memcpy(out + size_t(c) * width * height, ch[c].data.data(), size_t(width) * height * 4);
+    return 0;
+  } catch (std::exception& e) {
+    g_merr = e.what();
+    return -1;
+  }
+}
+
+// The XYB mode (ModularXyb): q_f16 the three LfQuantFactors as written (NULL or all zero: the defaults).
+int64_t jxs_encode_modular_xyb(uint32_t width, uint32_t height, uint64_t seed, uint32_t rct, uint32_t squeeze,
+                               uint32_t tree_kind, const float* q_f16, uint32_t colour, uint32_t orientation, uint32_t gab,
+                               uint32_t epf_iters, uint8_t* out, size_t cap) {
+  try {
+    if (orientation < 1 || orientation > 8 || colour > 7 || gab > 1 || epf_iters > 3)
+      throw std::runtime_error("XYB mode: orientation 1..8, colour 0..7, gab 0/1, epf_iters 0..3");
+    jxs::ModularXyb x;
+    x.on = true;
+    for (int c = 0; c < 3; c++) x.lf_quant_f16[c] = q_f16 ? q_f16[c] : 0.0f;
+    x.colour = colour;
+    x.orientation = orientation;
+    x.gab = gab;
+    x.epf_iters = epf_iters;
+    std::vector<uint8_t> b = jxs::encode_modular(width, height, seed, rct, squeeze, tree_kind, nullptr, 0, 0, x);
+    if (b.size() <= cap) memcpy(out, b.data(), b.size());
+    return int64_t(b.size());
+  } catch (std::exception& e) {
+    g_merr = e.what();
+    return -1;
+  }
+}
+
 int64_t jxs_encode_modular_tokens(const uint32_t* words, size_t nwords, uint8_t* out, size_t cap) {
   try {
     std::vector<uint8_t> b = jxs::encode_modular_tokens(words, nwords);
