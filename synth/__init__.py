@@ -51,7 +51,7 @@ def _lib():
 
 def encode_synthetic(width, height, seed, distance=1.0, epf_iters=2, gab=1, profile=1, lf_tree=0, entropy=0, orientation=1,
                      colour=0, dequant=None, x_qm_scale=3, b_qm_scale=2, header=None, lf_extra_precision=0,
-                     skip_lf_smoothing=False, lf_entropy=0) -> bytes:
+                     skip_lf_smoothing=False, lf_entropy=0, toc=None) -> bytes:
     """One synthetic VarDCT frame. profile 0: DCT8x8 only; 1: mixed transforms up to 32x32;
     2: also 64x64 / 64x32 / 32x64; 3: also the 128 / 256 families (DCT128X128 ... DCT256X256, transform types 21..26);
     4: profile 3 plus IDENTITY, DCT2X2 and AFV0-3 among the 8x8 blocks, so that every dequantisation table is used.
@@ -74,7 +74,11 @@ def encode_synthetic(width, height, seed, distance=1.0, epf_iters=2, gab=1, prof
     lf_extra_precision: 0..3, written in every LF group with the quantised LF samples unchanged (the decoded LF image is
     scaled by 2^-lf_extra_precision, a valid frame of a different picture). skip_lf_smoothing: sets the frame flag that
     turns the adaptive LF smoothing off. lf_entropy: code of the LF image's pixel symbols, as `entropy` (0 ANS, 1 prefix
-    codes, 2 / 3 the same with LZ77 copies at plain distances)."""
+    codes, 2 / 3 the same with LZ77 copies at plain distances).
+    toc: None (sections in logical order) or a permutation of the frame's TOC entries, in the decoder's convention
+    (frame/decode.rs:263-285): logical section i is stored as bitstream entry toc[i]. The logical order is LfGlobal,
+    the LF groups, HfGlobal, then the HF sections pass by pass, each in group order. A frame of one group has a
+    single TOC entry and is refused."""
     profile = ((profile & 0xff) | ((lf_tree & 1) << 8) | ((entropy & 3) << 9) | (((orientation - 1) & 7) << 12)
                | ((colour & 15) << 16) | ((lf_extra_precision & 3) << 20) | ((1 if skip_lf_smoothing else 0) << 22)
                | ((lf_entropy & 3) << 23))
@@ -83,12 +87,14 @@ def encode_synthetic(width, height, seed, distance=1.0, epf_iters=2, gab=1, prof
     arr = (C.c_uint32 * max(1, len(words)))(*[w & 0xFFFFFFFF for w in words])
     hwords = _header_words(header)
     harr = (C.c_uint32 * max(1, len(hwords)))(*[int(w) & 0xFFFFFFFF for w in hwords])
+    toc = [] if toc is None else [int(v) for v in toc]
+    tarr = (C.c_uint32 * max(1, len(toc)))(*toc)
 
     def run(buf, cap):
-        if not words and not hwords and (x_qm_scale, b_qm_scale) == (3, 2):
+        if not words and not hwords and not toc and (x_qm_scale, b_qm_scale) == (3, 2):
             return lib.jxs_encode_synthetic(width, height, seed, distance, epf_iters, gab, profile, buf, cap)
         return lib.jxs_encode_synthetic_ex(width, height, seed, distance, epf_iters, gab, profile, x_qm_scale, b_qm_scale,
-                                           arr, len(words), harr, len(hwords), buf, cap)
+                                           arr, len(words), harr, len(hwords), tarr, len(toc), buf, cap)
     cap = max(1 << 16, width * height * 2 + 4 * len(words))
     buf = C.create_string_buffer(cap)
     n = run(buf, cap)
@@ -377,7 +383,9 @@ def encode_vardct_tokens(spec) -> bytes:
       sections: per pass, per group: (histogram index, [(context, u32 value), ...]);
       header (optional): the header fields of encode_synthetic's `header` dict (_header_words), written as given; its
       restoration filter groups apply to the frame's Gaborish + EPF 2 header;
-      cfl (optional): (ytox, ytob) CfL tile maps, one i32 per 64x64 tile in raster order (default: zeros)."""
+      cfl (optional): (ytox, ytob) CfL tile maps, one i32 per 64x64 tile in raster order (default: zeros);
+      toc (optional): a permutation of the frame's TOC entries, as encode_synthetic's `toc` (refused for a frame of
+      one group and one pass, whose single TOC entry cannot be permuted)."""
     import numpy as np
     header = dict(spec.get("header") or {})
     if spec.get("cfl") is not None:
@@ -412,6 +420,8 @@ def encode_vardct_tokens(spec) -> bytes:
         words += [hist, len(toks)]
         for c, v in toks:
             words += [c, v]
+    if spec.get("toc") is not None:  # a trailing group: specs without it (and their files) stay as they were
+        words += [len(spec["toc"])] + [int(v) for v in spec["toc"]]
     lib = _lib()
     arr = np.asarray([int(w) & 0xFFFFFFFF for w in words], np.uint32)
     cap = max(1 << 16, 8 * len(words))

@@ -85,6 +85,7 @@ struct Params {
     uint16_t weights8[210] = {};
     std::vector<int32_t> cfl_x, cfl_b;  // CfL tile maps, one value per 64x64 tile; empty: random small values
   } hdr = {};
+  std::vector<uint32_t> toc = {};  // TOC permutation (finish_with_toc); empty: not permuted
 };
 
 // Worker threads inside one encode (jxs_set_threads): only loops whose result does not depend on the order of
@@ -719,6 +720,44 @@ static void write_toc_entry(BitWriter& bw, uint32_t v) {  // toc.rs:28
   else bw.u2s_sel(3, v - 4211712, 30);
 }
 
+static void permutation_tokens(const std::vector<uint32_t>& perm, uint32_t skip, std::vector<Token>& out);
+
+// The TOC (toc.rs:20-32) and the sections after it. perm empty: not permuted, sections in logical order. Otherwise the
+// decoder's convention (encodings.rs:173-194, frame/decode.rs:263-285): logical section i is bitstream entry perm[i],
+// written as the permuted bit, a Lehmer code with skip 0 over 8 contexts in its own entropy code, then the sizes and
+// the sections in stored order. Returns the header bytes followed by the sections.
+static std::vector<uint8_t> finish_with_toc(BitWriter& out, const std::vector<std::vector<uint8_t>>& sections,
+                                            const std::vector<uint32_t>& perm) {
+  const size_t n = sections.size();
+  std::vector<size_t> stored(n);  // stored position -> logical section
+  for (size_t i = 0; i < n; i++) stored[i] = i;
+  if (perm.empty()) {
+    out.write(0, 1);  // not permuted
+  } else {
+    if (n == 1) throw std::runtime_error("a frame with a single TOC entry cannot be permuted");
+    if (perm.size() != n) throw std::runtime_error("TOC permutation of the wrong size");
+    std::vector<bool> seen(n, false);
+    for (size_t i = 0; i < n; i++) {
+      if (perm[i] >= n || seen[perm[i]]) throw std::runtime_error("TOC permutation is not a permutation");
+      seen[perm[i]] = true;
+      stored[perm[i]] = i;
+    }
+    out.write(1, 1);
+    std::vector<Token> toks;
+    permutation_tokens(perm, 0, toks);
+    std::vector<uint8_t> one(8, 0);
+    AnsCode code = build_code(8, one, 1, {&toks}, 6);
+    write_code(out, code);
+    write_tokens(out, code, toks);
+  }
+  out.zero_pad_to_byte();
+  for (size_t k = 0; k < n; k++) write_toc_entry(out, uint32_t(sections[stored[k]].size()));
+  out.zero_pad_to_byte();
+  std::vector<uint8_t> bytes = out.finish();
+  for (size_t k = 0; k < n; k++) bytes.insert(bytes.end(), sections[stored[k]].begin(), sections[stored[k]].end());
+  return bytes;
+}
+
 // block_context_map.rs:20-31
 static const uint16_t kFreqCtx[64] = {0xBAD, 0,  1,  2,  3,  4,  5,  6,  7,  8,  9,  10, 11, 12, 13, 14, 15, 15, 16, 16, 17, 17,
                                       18,    18, 19, 19, 20, 20, 21, 21, 22, 22, 23, 23, 23, 23, 24, 24, 24, 24, 25, 25, 25, 25,
@@ -1189,14 +1228,7 @@ std::vector<uint8_t> encode(const Params& p) {
     sections.push_back(hf_global.finish());
     for (auto& b : hf_groups) sections.push_back(b.finish());
   }
-  // TOC (toc.rs:20-32)
-  out.write(0, 1);  // not permuted
-  out.zero_pad_to_byte();
-  for (auto& s : sections) write_toc_entry(out, uint32_t(s.size()));
-  out.zero_pad_to_byte();
-  std::vector<uint8_t> bytes = out.finish();
-  for (auto& s : sections) bytes.insert(bytes.end(), s.begin(), s.end());
-  return bytes;
+  return finish_with_toc(out, sections, p.toc);
 }
 
 // The header words of jxs_encode_synthetic_ex (synth/__init__.py _header_words gives the layout).
@@ -1495,6 +1527,11 @@ std::vector<uint8_t> encode_vardct_tokens(const uint32_t* w, size_t len) {
       t.value = next();
     }
   }
+  std::vector<uint32_t> toc;  // optional trailing group: the TOC permutation
+  if (pos < len) {
+    toc.resize(next());
+    for (auto& v : toc) v = next();
+  }
   if (pos != len) throw std::runtime_error("VarDCT token spec too long");
   std::vector<std::vector<Sym>> syms(toks.size());
   for (uint32_t p = 0; p < num_passes; p++) {
@@ -1587,13 +1624,7 @@ std::vector<uint8_t> encode_vardct_tokens(const uint32_t* w, size_t len) {
     sections.push_back(hf_global.finish());
     for (auto& b : hf_groups) sections.push_back(b.finish());
   }
-  out.write(0, 1);  // TOC not permuted
-  out.zero_pad_to_byte();
-  for (auto& s : sections) write_toc_entry(out, uint32_t(s.size()));
-  out.zero_pad_to_byte();
-  std::vector<uint8_t> bytes = out.finish();
-  for (auto& s : sections) bytes.insert(bytes.end(), s.begin(), s.end());
-  return bytes;
+  return finish_with_toc(out, sections, toc);
 }
 
 // 8-bit RGB rendering of the same procedural image (source of the synthetic Modular frames).
@@ -1651,10 +1682,11 @@ int64_t jxs_encode_synthetic(uint32_t width, uint32_t height, uint64_t seed, flo
 //               order, 8 * REQUIRED_SIZE_X wide), written as a Modular sub-bitstream after the fields.
 // dequant_len 0: all library tables (the same bitstream as jxs_encode_synthetic).
 // header: the restoration filter, colour correlation, opsin and CfL fields to write (header_len 0: defaults).
+// toc: the TOC permutation, logical section i stored as bitstream entry toc[i] (toc_len 0: not permuted).
 int64_t jxs_encode_synthetic_ex(uint32_t width, uint32_t height, uint64_t seed, float distance, uint32_t epf_iters,
                                 uint32_t gab, uint32_t profile, uint32_t x_qm_scale, uint32_t b_qm_scale,
                                 const uint32_t* dequant, size_t dequant_len, const uint32_t* header, size_t header_len,
-                                uint8_t* out, size_t cap) {
+                                const uint32_t* toc, size_t toc_len, uint8_t* out, size_t cap) {
   try {
     jxs::Params p{width, height, seed, distance, epf_iters, gab, profile & 0xff, (profile >> 8) & 1, (profile >> 9) & 3,
                   ((profile >> 12) & 7) + 1, (profile >> 16) & 15};
@@ -1691,6 +1723,7 @@ int64_t jxs_encode_synthetic_ex(uint32_t width, uint32_t height, uint64_t seed, 
       if (pos != dequant_len) throw std::runtime_error("dequant array too long");
     }
     if (header_len) jxs::read_header_words(header, header_len, p.hdr);
+    p.toc.assign(toc, toc + toc_len);
     std::vector<uint8_t> b = jxs::encode(p);
     if (b.size() <= cap && out) memcpy(out, b.data(), b.size());
     return int64_t(b.size());

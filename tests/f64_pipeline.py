@@ -295,6 +295,9 @@ class Frame:
         self.encodings = encodings
         self.global_scale, self.x_qm_scale, self.b_qm_scale = int(d.global_scale), int(d.x_qm_scale), int(d.b_qm_scale)
         self.lf = np.stack([_arr(d.lf[c], C.c_float, (yb, xb)) for c in range(3)]).astype(np.float64)
+        # an LF image computed elsewhere in float64 (tests/f64_prefix.py) may replace lf; lf_mag then carries its own
+        # error bound, in units of K_A 2^-24, added to |lf| in stage A's magnitudes
+        self.lf_mag = None
         self.transform_map = _arr(d.transform_map, C.c_uint8, (yb, xb))
         self.raw_quant = _arr(d.raw_quant_map, C.c_int32, (yb, xb))
         self.epf_map = _arr(d.epf_map, C.c_uint8, (yb, xb))
@@ -404,7 +407,8 @@ def stage_a(fr, coeffs):
         lcols = bxs[:, None, None] + np.arange(cx)[None, None, :]
         for c in range(3):
             lf = fr.lf[c][lrows, lcols]  # (N, cy, cx), group.rs:227-235
-            pix, m = transform_to_pixels_batch(t, deq[c], lf, mdeq[c], np.abs(lf))
+            mlf = np.abs(lf) if fr.lf_mag is None else np.abs(lf) + fr.lf_mag[c][lrows, lcols]
+            pix, m = transform_to_pixels_batch(t, deq[c], lf, mdeq[c], mlf)
             planes[c][rows, cols] = pix
             mag[c][rows, cols] = m
     return planes, mag

@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 from tests.f64_pipeline import MIN_SIGMA, epf_stage_f64, sigma_image_f64
+from tests.f64_prefix import dequant_lf_f64
 
 
 def _lib():
@@ -107,11 +108,8 @@ def test_dequant_lf_against_f64_restatement(extra_precision):
     gs, ql, cf, ytox, ytob = 4587, 16, 84, -7, 21
     lib.jxo_t_dequant_lf(w, h, q.ctypes.data, gs, ql, lf_quant.ctypes.data, extra_precision, 0.0, 1.0, ytox, ytob, cf, tall.ctypes.data,
                          nthr.ctypes.data, out.ctypes.data, qlf.ctypes.data)
-    mul = 1.0 / (1 << extra_precision)
-    fac = lf_quant.astype(np.float64) * (65536.0 / (gs * ql)) * mul
-    qy, qx, qb = q[0].astype(np.float64), q[1].astype(np.float64), q[2].astype(np.float64)
-    in_y = qy * fac[1]
-    want = np.stack([in_y * (0.0 + ytox / cf) + qx * fac[0], in_y, in_y * (1.0 + ytob / cf) + qb * fac[2]])
+    want, _ = dequant_lf_f64(q[1], q[0], q[2], gs, ql, 0.0, ytox, 1.0, ytob, cf, mul=1.0 / (1 << extra_precision),
+                             lf_quant=lf_quant.astype(np.float64))
     assert np.allclose(out, want, rtol=3e-6, atol=1e-7), np.abs(out - want).max()
     # mod.rs:898-924: bucket = (bucket_x * (|thr_b| + 1) + bucket_b) * (|thr_y| + 1) + bucket_y, strict comparisons
     bx = (q[1][..., None] > thr[0]).sum(-1)
